@@ -2,7 +2,7 @@
 """Benchmark of the text2video denoising hot path: denoised frames/s = F / (sampling loop + VAE decode) for
 ModelScope 24 frames x 256x256, 50-step DDIM (UI-default scheduler "DDIM_Gaussian", cfg 17), fp16, synthetic weights.
 
-    python bench.py --gpus 1 --steps K --warmup W                      # this repo (B200, libt2v_b200.so)
+    python bench.py --gpus 1 --steps K --warmup W                      # this repo (H100, libt2v_b200.so)
     torchrun --nproc-per-node N ... bench.py --gpus N ...              # one independent clip per GPU (sample-DP, weak)
     python bench.py --impl reference ...                               # the reference algorithm on the host cores
     python bench.py --impl torch_gpu ...                               # the reference's GPU path (fp16 autocast + SDPA eager torch ops)
@@ -10,7 +10,9 @@ ModelScope 24 frames x 256x256, 50-step DDIM (UI-default scheduler "DDIM_Gaussia
 A "step" is one whole clip: 50 scheduler steps (each = one batched cond+uncond UNet forward + fused CFG/DDIM update)
 followed by the VAE decode of all frames.  `value` has inputs resident in HBM; `e2e` goes through the public
 `TextToVideoSynthesis.infer` with host buffers (H2D of conditioning + noise and D2H of the finished uint8 clip inside
-the timed region).  One JSON line is printed by rank 0.
+the timed region).  One JSON line is printed by rank 0.  `--dump-outputs DIR` writes what the last timed clip computed
+(decoded frames and final latent, float32 .npy, at most 64 MB in all) so that two builds can be compared output for output:
+inputs are seeded, identical from run to run for the same arguments.
 """
 import argparse
 import json
@@ -51,6 +53,11 @@ def parse():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-gpu-baseline', action='store_true', help='skip the torch-eager GPU comparator leg of the N=1 run')
     ap.add_argument('--cpu-frames', type=int, default=0, help='frames of the CPU sample (0 = the metric\'s F)')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='after the timed clips, write the last timed clip\'s outputs as DIR/frames.npy (decoded frames, '
+                         '[F, H, W, 3] 0..255) and DIR/latents.npy (final latent, [1, 4, F, h, w]), float32, at most 64 MB in '
+                         'all: when the whole clip is larger, both hold the same fixed, seeded subset of frames, listed in '
+                         'DIR/frame_index.npy')
     return ap.parse_args()
 
 
@@ -61,8 +68,9 @@ def peaks():
         return {'tflops_sustained': p['bf16_tflops_sustained'], 'tflops_burst': p['bf16_tflops'], 'hbm_gbs': p['hbm_gbs'],
                 'source': 'measured (MEASURED_PEAKS.json)'}
     except Exception:
-        return {'tflops_sustained': 1400.0, 'tflops_burst': 1590.0, 'hbm_gbs': 6650.0,
-                'source': 'fallback (B200_PROFILING.md)'}
+        # NVIDIA H100 SXM data sheet, dense FP16 tensor / HBM3, for a card allowed 700 W: an upper bound, not a measured rate
+        return {'tflops_sustained': 989.0, 'tflops_burst': 989.0, 'hbm_gbs': 3350.0,
+                'source': 'H100 SXM data sheet (dense FP16, 700 W)'}
 
 
 class ClockSampler(threading.Thread):
@@ -179,11 +187,10 @@ def run_reference(args):
 def torch_gpu_clip_fn(args, dev):
     """The reference's own GPU path, SURVEY.md section 8d / BASELINE.md section 4.1 (the ">= 15x" denominator): the same torch
     ops as the reference module tree (oracle/, pinned against the reference on CPU) with fp16 weights under
-    torch.autocast('cuda') (t2v_pipeline.py:271), attention through F.scaled_dot_product_attention (t2v_model.py:566-569, the
-    only backend reachable on sm_100), TWO sequential B = 1 forwards per step (gaussian_sampler.py:161-162), the reference
-    sampler arithmetic, and the per-frame VAE loop with a .cpu() per frame (t2v_pipeline.py:347-355).  /root/reference does
-    not exist on the GPU box, so the module tree itself cannot be timed there; its restatement issues the same library
-    kernels (cuDNN / cuBLAS / SDPA / elementwise).  Model movement and torch_gc() calls of the reference are left out (they
+    torch.autocast('cuda') (t2v_pipeline.py:271), attention through F.scaled_dot_product_attention (t2v_model.py:566-569),
+    TWO sequential B = 1 forwards per step (gaussian_sampler.py:161-162), the reference sampler arithmetic, and the
+    per-frame VAE loop with a .cpu() per frame (t2v_pipeline.py:347-355).  The reference's module tree needs the webui to
+    import, so its restatement is timed instead; it issues the same library kernels (cuDNN / cuBLAS / SDPA / elementwise).  Model movement and torch_gc() calls of the reference are left out (they
     would only slow it down).  Returns fn(seed) -> list of decoded frames on the host."""
     from oracle import unet_oracle as UO, vae_oracle as VO, samplers_oracle as SO
     cfg = UO.UNetConfig()
@@ -251,18 +258,25 @@ def run_torch_gpu(args):
     print(json.dumps(line), flush=True)
 
 
-def recorded_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per gemm_tc_kernel launch (bytes), from the committed ncu capture of the
-    434 GEMM launches of one forward (profiles/r01_gemm_dram_traffic.json); None when the file is absent.  A number taken
-    under ncu cannot be produced inside a timed run, so it is recorded, not live."""
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'r01_gemm_dram_traffic.json')) as f:
-            return float(json.load(f)['dram_bytes_per_launch'])
-    except Exception:
-        return None
-
-
 # --------------------------------------------------------------------------------------------- this repo
+DUMP_BUDGET = 64 * 10 ** 6 - 2 ** 16      # bytes of array data per --dump-outputs (64 MB less room for .npy headers / index)
+
+
+def dump_outputs(out_dir, frames, latents):
+    """frames [F, H, W, 3], latents [B, 4, F, h, w] -> float32 .npy files.  Over DUMP_BUDGET, keep the largest number of
+    frames that fits, chosen by a fixed seed (the same frames for both arrays and for every run of the same shape)."""
+    import numpy as np
+    F = frames.shape[0]
+    per_frame = 4 * (frames[0].numel() + latents[:, :, 0].numel())
+    keep = min(F, DUMP_BUDGET // per_frame)
+    idx = torch.arange(F) if keep == F else torch.randperm(F, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, 'frames.npy'), frames[idx.to(frames.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, 'latents.npy'), latents[:, :, idx.to(latents.device)].float().cpu().numpy())
+    if keep < F:
+        np.save(os.path.join(out_dir, 'frame_index.npy'), idx.double().numpy())
+
+
 def run_b200(args):
     import torch.distributed as dist
     world = int(os.environ.get('WORLD_SIZE', '1'))
@@ -299,6 +313,7 @@ def run_b200(args):
     uc_host = torch.randn(1, 77, 1024, generator=g).half().pin_memory()
     c_dev, uc_dev = c_host.to(dev), uc_host.to(dev)
     entry = [s for s in samplers.available_samplers if s.name == args.sampler][0]
+    last = {}                       # outputs of the most recent clip_device call (--dump-outputs)
 
     def clip_device(seed):
         """inputs resident in HBM; result (uint8 frames) stays on the device"""
@@ -312,10 +327,14 @@ def run_b200(args):
                                 unconditional_guidance_scale=args.cfg_scale, x_T=x_l, shape=tuple(x_l.shape), eta=0.0, batch_size=1)
             finally:
                 fs.end()
-            return fs.decode(fs.gather_latent(x0), 1.0 / SCALE_FACTOR)
+            last['latents'] = fs.gather_latent(x0)
+            last['frames'] = fs.decode(last['latents'], 1.0 / SCALE_FACTOR)
+            return last['frames']
         x0 = smp.sample(S=S, conditioning=c_dev, unconditional_conditioning=uc_dev, unconditional_guidance_scale=args.cfg_scale,
                         x_T=x_T, shape=tuple(x_T.shape), eta=0.0, batch_size=1)
-        return pipe.autoencoder.decode_video(x0, 1.0 / SCALE_FACTOR, as_uint8=True)
+        last['latents'] = x0
+        last['frames'] = pipe.autoencoder.decode_video(x0, 1.0 / SCALE_FACTOR, as_uint8=True)
+        return last['frames']
 
     def clip_e2e(seed):
         """public API with host buffers: H2D of conditioning + CPU-generated noise, D2H of the finished clip"""
@@ -360,6 +379,8 @@ def run_b200(args):
     clk.stop_flag = True
     clk.join(timeout=2)
     fps = n_units * args.steps * F / (ms / 1000.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last['frames'], last['latents'])
     clip_e2e(7)                                   # warm the e2e path (pinned staging, plan for B=2 already built)
     ms_e2e = timed(clip_e2e, args.steps, 123, False)
     fps_e2e = n_units * args.steps * F / (ms_e2e / 1000.0)
@@ -452,11 +473,11 @@ def run_b200(args):
             'gpu_launches': int(launches_clip * args.steps),
             'clocks': clk.summary(),
             'roofline': {'bound': 'tensor', 'achieved': achieved, 'peak': pk['tflops_sustained'], 'unit': 'TFLOP/s',
-                         'frac': achieved / pk['tflops_sustained'], 'traffic': recorded_traffic(), 'peak_source': pk['source'],
+                         'frac': achieved / pk['tflops_sustained'], 'peak_source': pk['source'],
                          'kernel_frac': achieved / pk['tflops_sustained'],
                          'whole_clip_tflops': whole_clip_tflops, 'whole_clip_frac': whole_clip_tflops / pk['tflops_sustained'],
                          'whole_clip_frac_of_burst': whole_clip_tflops / pk['tflops_burst'],
-                         'kernel': 'gemm_tc_kernel (tcgen05 implicit GEMM), all launches of one B=2 forward, CUDA events per launch',
+                         'kernel': 'gemm_tc_kernel (wgmma implicit GEMM), all launches of one B=2 forward, CUDA events per launch',
                          'gemm_share_of_forward': gemm['ms'] / prof['total_ms'] if prof['total_ms'] else None,
                          'forward_breakdown_ms': {k: round(v['ms'], 3) for k, v in prof.items() if isinstance(v, dict)}},
         }

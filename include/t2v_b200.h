@@ -1,4 +1,4 @@
-/* t2v_b200 -- C ABI of the B200-native text2video denoising path.
+/* t2v_b200 -- C ABI of the GPU-native (sm_90a) text2video denoising path.
  *
  * The reference (kabachuha/sd-webui-text2video) has NO FFI boundary: its hot path is plain Python that calls
  * PyTorch library kernels.  This header is the boundary a maintainer would bind instead (ctypes stubs in
@@ -76,7 +76,7 @@ double t2v_unet_flops(t2v_unet* u, int B, int F, int h, int w, int L);
 int t2v_unet_num_launches(t2v_unet* u);
 /* Measurement aid: replays the plan of this shape once (inputs = whatever the last forward left in the staging
  * buffers) with a CUDA-event pair around every launch on `stream` and sums per kernel family:
- *   out[3k + 0] = milliseconds, out[3k + 1] = algorithmic flop, out[3k + 2] = launches, k = 0 implicit-GEMM (tcgen05),
+ *   out[3k + 0] = milliseconds, out[3k + 1] = algorithmic flop, out[3k + 2] = launches, k = 0 implicit-GEMM (wgmma),
  *   1 attention, 2 group/layer norm, 3 glue; out[12] = total ms.  Synchronises the stream (bench/tests only).   */
 int t2v_unet_profile(t2v_unet* u, int B, int F, int h, int w, int L, void* stream, double* out13);
 /* copies an internal activation (debug / parity taps): name = reference module path (e.g. "input_blocks.1.0"),
@@ -105,7 +105,7 @@ int t2v_unet_lora_clear(t2v_unet* u, void* stream);
 int t2v_unet_lora_merged(t2v_unet* u);          /* number of weights currently carrying a merge */
 
 /* ------------------------------------------------------------------------------------------ frame-sharded clip
- * ONE clip split over the GPUs of a node, one process per GPU (BASELINE config 4: 125 frames over 8 x B200).  Frames are
+ * ONE clip split over the GPUs of a node, one process per GPU (e.g. BASELINE config 4's 125 frames over 8 GPUs).  Frames are
  * independent inside the spatial modules and coupled in TemporalConvBlock_v2 (t2v_model.py:1201-1212), TemporalTransformer
  * (:724, :734-738) and every 5-D GroupNorm; the library keeps activations frame-sharded in the spatial modules, transposes
  * them to a pixel-sharded layout around each temporal module with a kernel that writes straight into the peers' buffers

@@ -18,6 +18,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, 'sd-webui-text2video_b200'))
 from oracle import ref_shim                                   # noqa: E402
 from oracle import unet_oracle as UO                          # noqa: E402
 from oracle import vae_oracle as VO                           # noqa: E402
@@ -164,7 +165,7 @@ def gold_unet(m, name, cfg, F, h, w, wseed, keep_taps):
 
 
 
-def gold_unet_step(m, name, cfg, F, h, w, wseed, unipc=True):
+def gold_unet_step(m, name, cfg, F, h, w, wseed, unipc=True, keep_frames=None):
     """Full-size single-step gate at a BASELINE shape (config 2: 24 f x 32 x 32 latent): the reference module's eps for the
     cond / uncond branch at the first timestep and the latent after ONE update of each scheduler, produced by the reference
     sampler classes.  Reference forwards are memoised on (x, t, ctx) -- the first two model calls of DDIM_Gaussian and DDIM
@@ -258,6 +259,11 @@ def gold_unet_step(m, name, cfg, F, h, w, wseed, unipc=True):
         d = (om.calls[-1] - out[key]).abs().max().item()
         print(f'[{name}] {key}: oracle-sampler-vs-reference max|d| = {d:.3e}', flush=True)
         assert d < 5e-4, (key, d)
+    if keep_frames is not None:      # files stay under 1 MB: a fixed subset of the frames, exact values
+        for k in ('eps_cond', 'eps_uncond', 'ddim_gaussian_x1', 'ddim_x1', 'unipc_x1'):
+            if k in out:
+                out[k] = out[k][:, :, keep_frames].contiguous().clone()
+        out['frames'] = list(keep_frames)
     torch.save(out, os.path.join(GOLD, name + '.pt'))
     return out
 
@@ -517,6 +523,55 @@ def gold_vid2vid_encode():
     torch.save(out, os.path.join(GOLD, 'vid2vid_encode.pt'))
 
 
+# the key-frame schedules of tests/test_modules_cpu.py::test_inpainting_weight_schedule_matches_reference
+KEY_FRAME_CASES = [
+    (8, 4, '0:(t/max_i_f), "max_i_f":(1)'), (24, 8, '0:(t/max_i_f), "max_i_f":(1)'), (6, 4, '0:(0.25), 3:(1.0)'),
+    (10, 3, '0:(0), 4:(0.5), "max_f":(1)'), (12, 6, '0:(sin(t/max_f)), 9:(0.2)'),
+    (8, 4, '0:(t/max_i_f), "max_i_f":(1*1)'), (16, 5, '0:(0.1+t/max_f), 11:(t*t/(max_f*max_f))')]
+
+
+def layout_digest(d):
+    """sha256 of a {name: shape or kind} dict in canonical (sorted JSON) form: equal digests <=> equal dicts."""
+    import hashlib
+    import json
+    return hashlib.sha256(json.dumps(sorted((k, list(v) if isinstance(v, tuple) else v) for k, v in d.items())).encode()).hexdigest()
+
+
+def gold_reference_live(m):
+    """What the CPU tests compare the mirrors / oracle against: digests of the reference UNetSD / AutoencoderKL state-dict
+    layout and module kinds, the reference UNetSD output at the narrow config, and the reference key-frame schedules (None
+    where the unmodified reference raises on the installed pandas)."""
+    from types import SimpleNamespace as NS
+    from t2v_b200.pipeline import VAE_DDCONFIG
+    cfg = UO.UNetConfig(dim=64)
+    net = build_ref_unet(m, cfg)
+    kinds = ('Linear', 'Conv1d', 'Conv2d', 'Conv3d')
+    rv = m.AutoencoderKL(dict(VAE_DDCONFIG), 4, None)
+    out = {'unet_shapes_sha256': layout_digest({k: tuple(v.shape) for k, v in net.state_dict().items()}),
+           'unet_kinds_sha256': layout_digest({n: type(x).__name__ for n, x in net.named_modules() if type(x).__name__ in kinds}),
+           'vae_shapes_sha256': layout_digest({k: tuple(v.shape) for k, v in rv.state_dict().items()}),
+           'n_unet_params': len(net.state_dict()), 'n_vae_params': len(rv.state_dict())}
+    W = UO.make_weights(UO.param_specs(cfg), seed=5)
+    net.load_state_dict(W, strict=True)
+    g = torch.Generator().manual_seed(9)
+    x = torch.randn(2, 4, 3, 8, 8, generator=g)
+    y = torch.randn(2, 77, 1024, generator=g)
+    t = torch.tensor([500, 20])
+    with torch.no_grad():
+        out['unet_out'] = net(x, t, y)
+    print('reference_live: oracle vs reference UNetSD max |err|', (UO.unet_forward(W, cfg, x, t, y) - out['unet_out']).abs().max().item())
+    kf = ref_shim.load_key_frames()
+    out['key_frames'] = {}
+    for frames, i_frames, spec in KEY_FRAME_CASES:
+        try:
+            w = kf.T2VAnimKeys(NS(max_frames=frames, inpainting_weights=spec), 7, i_frames).inpainting_weights_series
+            w = [float(v) for v in np.asarray(w, dtype=np.float64)]
+        except TypeError:
+            w = None
+        out['key_frames'][repr((frames, i_frames, spec))] = w
+    torch.save(out, os.path.join(GOLD, 'reference_live.pt'))
+
+
 def main(only=None):
     os.makedirs(GOLD, exist_ok=True)
     m = ref_shim.load_modelscope()
@@ -529,6 +584,8 @@ def main(only=None):
         gold_vae_encode(m)
     if want('vid2vid_encode'):
         gold_vid2vid_encode()
+    if want('reference_live'):
+        gold_reference_live(m)
     tiny = UO.UNetConfig(dim=64)
     keep = ['input_blocks.0.0', 'input_blocks.0.1', 'input_blocks.1.0', 'input_blocks.1.1', 'input_blocks.1.2',
             'input_blocks.3', 'input_blocks.4.0', 'input_blocks.11.0', 'middle_block.1', 'middle_block.3',
@@ -542,7 +599,8 @@ def main(only=None):
     if full and want('unet_cfg1'):
         gold_unet(m, 'unet_cfg1', UO.UNetConfig(), F=4, h=16, w=16, wseed=0, keep_taps=[])
     if full and want('unet_cfg2'):       # the shape every bench number is quoted on: 24 frames x 256^2
-        gold_unet_step(m, 'unet_cfg2', UO.UNetConfig(), F=24, h=32, w=32, wseed=0)
+        gold_unet_step(m, 'unet_cfg2', UO.UNetConfig(), F=24, h=32, w=32, wseed=0,
+                       keep_frames=[int(round(v)) for v in torch.linspace(0, 23, 10).tolist()])
     if full and want('unet_cfg3_slice'):  # config 3's spatial sequence length S = 72 * 128 = 9216, 2 frames
         gold_unet_forward_only(m, 'unet_cfg3_slice', UO.UNetConfig(), F=2, h=72, w=128, wseed=0)
     if want('vc_ddim'):

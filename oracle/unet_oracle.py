@@ -188,8 +188,8 @@ def sinusoidal_embedding(t, dim):
 
 
 # Which branch of CrossAttention.forward (:556-582) is restated: 'math' = the einsum + softmax fallback (:570-580; the CPU
-# gate), 'sdpa' = F.scaled_dot_product_attention on (b h) n d tensors (:566-569; the only backend the reference can reach
-# on sm_100: xformers is capped at capability 9.0, :556).  bench.py's GPU comparator and the autocast parity tests set 'sdpa'.
+# gate), 'sdpa' = F.scaled_dot_product_attention on (b h) n d tensors (:566-569; the backend the reference takes without
+# xformers installed).  bench.py's GPU comparator and the autocast parity tests set 'sdpa'.
 ATTN_IMPL = 'math'
 
 

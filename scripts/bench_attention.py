@@ -1,4 +1,4 @@
-"""Times spatial self-attention on the fused [tokens, 3C] matrix: tcgen05 kernel vs the warp-MMA kernel.
+"""Times spatial self-attention on the fused [tokens, 3C] matrix: wgmma kernel vs the warp-MMA kernel.
 usage: python scripts/bench_attention.py            (prints one line per shape)"""
 import os
 import sys
@@ -42,5 +42,5 @@ for shp in SHAPES:
     ms_w, tf_w, o_w = run(*shp)
     os.environ.pop('T2V_ATTN_WARP_MMA', None)
     d = (o_tc.float() - o_w.float()).abs().max().item()
-    print(f'batch {shp[0]} heads {shp[1]} S {shp[2]}: tcgen05 {ms_tc:.3f} ms {tf_tc:.0f} TF/s | warp-mma {ms_w:.3f} ms {tf_w:.0f} TF/s '
+    print(f'batch {shp[0]} heads {shp[1]} S {shp[2]}: wgmma {ms_tc:.3f} ms {tf_tc:.0f} TF/s | warp-mma {ms_w:.3f} ms {tf_w:.0f} TF/s '
           f'| max|diff| {d:.2e}', flush=True)

@@ -13,7 +13,7 @@ namespace t2v {
 
 static char g_err[512] = "";
 static int g_device = -1;
-static int g_num_sms = 148;
+static int g_num_sms = 132;
 static void* g_gn_ws = nullptr;
 static size_t g_gn_ws_bytes = 0;
 
@@ -37,7 +37,7 @@ int launch_status(const char* what) {
     return -2;
 }
 bool pdl_enabled() {
-    static const bool on = getenv("T2V_PDL") != nullptr;      // opt-in: measured 2.7 % SLOWER on the graphed forward (DESIGN.md)
+    static const bool on = getenv("T2V_PDL") != nullptr;      // opt-in (common.cuh)
     return on;
 }
 
@@ -68,8 +68,8 @@ int t2v_init(int device) {
         set_error("cudaGetDeviceProperties failed");
         return -1;
     }
-    if (prop.major != 10) {
-        set_error("t2v_b200 is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("t2v_b200 is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
         return -2;
     }
     g_device = device;
@@ -82,7 +82,7 @@ int t2v_init(int device) {
 }
 const char* t2v_last_error(void) { return g_err; }
 int t2v_num_sms(void) { return g_num_sms; }
-const char* t2v_version(void) { return "t2v_b200 0.1 (sm_100a; tcgen05+TMA implicit GEMM)"; }
+const char* t2v_version(void) { return "t2v_b200 0.2 (sm_90a; wgmma+TMA implicit GEMM)"; }
 
 int t2v_op_gemm(const void* a, long long lda, int K, int nd, const int* dims, int ntaps, const int* tap_off,
                 const void* w_packed, int n_alloc, int N, int b_batch_dim, int flags, void* out, long long ldo,

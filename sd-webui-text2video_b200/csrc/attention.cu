@@ -6,9 +6,9 @@
 // (t2v_model.py:548-583, :727-761) never materialise.
 //
 // This file: flash-style online softmax with warp-level mma.sync.m16n8k16 (fp16 in, fp32 accumulate, fp32 softmax,
-// P rounded to fp16 for P.V -- the numerics of torch SDPA's fused kernels that the reference dispatches to on sm_100,
+// P rounded to fp16 for P.V -- the numerics of torch SDPA's fused kernels that the reference dispatches to on the GPU,
 // t2v_model.py:566-569).  It serves the SHORT sequences: temporal attention (S = frames, 32 x 32 tiles), cross-attention
-// (77 keys) and the coarse levels (h*w < 256).  Long spatial sequences go to the tcgen05 kernel in attention_tc.cu.
+// (77 keys) and the coarse levels (h*w < 256).  Long spatial sequences go to the wgmma kernel in attention_tc.cu.
 #include <cstdlib>
 
 #include "common.cuh"

@@ -1,31 +1,21 @@
-// Spatial self-attention on the 5th-gen tensor cores: softmax(Q K^T * scale) V, head_dim 64, long sequences
+// Spatial self-attention on the Hopper tensor cores (wgmma): softmax(Q K^T * scale) V, head_dim 64, long sequences
 // (S = h*w tokens of one frame, t2v_model.py:540-584 with the (b, hw, c) token layout of :639-658).
 //
-// One CTA owns 256 queries (two 128-row tiles) of one (frame, head) and streams the keys/values in 128-row tiles:
+// One CTA owns 128 queries of one (frame, head) and streams the keys/values in 128-row tiles:
 //
-//   warp 8      TMA producer   Q (2 x 16 KB, once), then K_j / V_j tiles into a 4-stage ring -- straight out of the fused
-//                              [tokens, 3C] QKV matrix: the head is a column offset of the tensor map, rows past the end
-//                              of the frame are TMA zero fill.
-//   warp 9      MMA issuer     S_t  = Q_t K_j^T  4 x tcgen05.mma M128 N128 K16, both operands from shared memory,
-//                                                fp32 scores in TMEM columns t*128 + [0,128)
-//                              O_t += P_t V_j    8 x tcgen05.mma M128 N64 K16: A = P_t read from TMEM (fp16 pairs, columns
-//                                                256 + t*64 + [0,64)), B = V_j as it lies in the token matrix ([key][d] rows)
-//                                                through an MN-major shared-memory descriptor -- no transposed copy of V, no
-//                                                shared-memory round trip for P; fp32 O_t in TMEM columns 384 + t*64 + [0,64)
-//   warps 0-3   softmax, query tile 0 } thread = query row (TMEM lane): the 128 scores of the row are pulled into registers
-//   warps 4-7   softmax, query tile 1 } in one go and the TMEM copy released at once (S_t(j+1) is computed while the
-//                              exponentials of S_t(j) are evaluated); row max, exp2 on the MUFU, fp16 pairs stored back
-//                              to TMEM with tcgen05.st.
-//   setmaxnreg moves registers from the TMA/MMA warpgroup (72) to the softmax warpgroups (216).
+//   warpgroup 0      TMA producer   Q (16 KB, once), then K_j / V_j tiles into a 4-stage ring -- straight out of the fused
+//                                   [tokens, 3C] QKV matrix: the head is a column offset of the tensor map, rows past the
+//                                   end of the frame are TMA zero fill.
+//   warpgroups 1, 2  consumers      64 query rows each:
+//                                   S  = Q K_j^T   4 x wgmma m64n128k16, both operands from shared memory, fp32 in registers
+//                                   online softmax on the accumulator fragment (row max / sum across the 4 threads of a row)
+//                                   O += P V_j     8 x wgmma m64n64k16: A = P as fp16 register fragments (the S accumulator
+//                                                  layout IS the A-fragment layout, no shared-memory round trip), B = V_j as
+//                                                  it lies in the token matrix ([key][d] rows) through an MN-major descriptor
+//                                                  -- no transposed copy of V.
+//   setmaxnreg moves registers from the producer warpgroup to the consumers.
 //
-// O_t accumulates inside the tensor core across key tiles.  The exponent offset m of a row is therefore only moved
-// (and O_t, l rescaled by exp2((m_old - m_new) c) through a TMEM read-modify-write) when the running max outgrew it by
-// more than 2^8: until then P = exp2(S c - m c) <= 256 is exact in fp16's range and the final O / l is unchanged
-// (every term carries the same factor).  In steady state the softmax warps never touch O_t.
-//
-// The two query tiles run out of phase: while one group evaluates exponentials the tensor core works on the other
-// tile's S / P.V; both share every K/V tile (one L2 read per 256 queries).  Shared-memory traffic per key tile is
-// Q,K operand reads 64 KB + V reads 32 KB + TMA fill 32 KB (128 B/clk/SM), exponentials 32768 / (16/clk/SM).
+// Both consumer warpgroups share every K/V tile (one L2 read per 128 queries).
 //
 // Numerics (= torch SDPA fused kernels the reference dispatches to, t2v_model.py:561-569): fp16 operands, fp32 scores,
 // fp32 online softmax with the scale folded into exp2, P rounded to fp16 for P.V, fp32 output accumulation,
@@ -44,24 +34,18 @@ namespace t2v {
 namespace {
 
 constexpr int HD = 64;
-constexpr int BQ = 128;                 // query rows per tile (= TMEM lanes)
-constexpr int NT = 2;                   // query tiles per CTA
+constexpr int BQ = 128;                 // query rows per CTA (64 per consumer warpgroup)
 constexpr int BKV = 128;                // keys per iteration
 constexpr int ST = 4;                   // K/V ring stages
 constexpr int TILE_BYTES = 128 * 128;   // 128 rows x 64 fp16
 constexpr int SMEM_Q = 0;
-constexpr int SMEM_K = SMEM_Q + NT * TILE_BYTES;
+constexpr int SMEM_K = SMEM_Q + TILE_BYTES;
 constexpr int SMEM_V = SMEM_K + ST * TILE_BYTES;
 constexpr int SMEM_BAR = SMEM_V + ST * TILE_BYTES;
 constexpr int SMEM_TOTAL = SMEM_BAR + 256 + 1024;          // + alignment slack
-constexpr int NTHREADS = 384;           // warpgroups: softmax tile 0 | softmax tile 1 | TMA, MMA (+2 idle warps)
-constexpr int REGS_SOFTMAX = 216;       // 2 x 128 x 216 + 128 x 72 = 384 x 168
-constexpr int REGS_OTHER = 72;
-
-constexpr int TMEM_S = 0;               // S_t : fp32 scores, columns t*128 + [0, 128)
-constexpr int TMEM_P = 256;             // P_t : fp16 probabilities, two keys per column, columns 256 + t*64 + [0, 64)
-constexpr int TMEM_O = 384;             // O_t : fp32 running output, columns 384 + t*64 + [0, 64)
-constexpr float RESCALE_LOG2 = 8.f;     // the exponent offset lags the true running max by at most 2^8 (P <= 256 in fp16)
+constexpr int NTHREADS = 384;           // warpgroups: TMA | consumer rows 0-63 | consumer rows 64-127
+constexpr int REGS_CONSUMER = 232;      // 2 x 128 x 232 + 128 x 40 <= 64 K
+constexpr int REGS_PRODUCER = 40;
 
 struct Args {
     __half* o;
@@ -70,24 +54,23 @@ struct Args {
     float sl2;                          // scale * log2(e)
 };
 
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+    const __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
+
 __global__ void __launch_bounds__(NTHREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                     const __grid_constant__ CUtensorMap map_v, const Args a) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SMEM_BAR);
-    uint64_t* bar_q = bars;                    // Q tiles landed
+    uint64_t* bar_q = bars;                    // Q tile landed
     uint64_t* kv_full = bars + 1;              // [ST] K_j, V_j landed
-    uint64_t* kv_empty = kv_full + ST;         // [ST] all MMAs reading the stage retired
-    uint64_t* s_full = kv_empty + ST;          // [NT] S_t(j) in TMEM
-    uint64_t* s_free = s_full + NT;            // [NT] S_t(j) copied to registers: S_t(j+1) may be issued
-    uint64_t* p_full = s_free + NT;            // [NT] P_t(j) in TMEM (and O_t rescaled if the row max moved)
-    uint64_t* pv_full = p_full + NT;           // [NT] O_t += P_t(j) V_j retired: P_t may be overwritten, O_t read
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_full + NT);
+    uint64_t* kv_empty = kv_full + ST;         // [ST] both consumer warpgroups are done with the stage
 
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const int q0 = blockIdx.x * (NT * BQ);
+    const int wg = threadIdx.x >> 7;
+    const int q0 = blockIdx.x * BQ;
     const int head = blockIdx.y;
     const int b = blockIdx.z;
     const int n_kv = a.n_kv;
@@ -96,225 +79,133 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         mbar_init(bar_q, 1);
         for (int s = 0; s < ST; ++s) {
             mbar_init(&kv_full[s], 1);
-            mbar_init(&kv_empty[s], 1);
-        }
-        for (int t = 0; t < NT; ++t) {
-            mbar_init(&s_full[t], 1);
-            mbar_init(&s_free[t], 4);          // one arrival per softmax warp
-            mbar_init(&p_full[t], 4);
-            mbar_init(&pv_full[t], 1);
+            mbar_init(&kv_empty[s], 2);
         }
         fence_barrier_init();
     }
-    if (warp == 9) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     griddep_wait();        // the prologue above overlaps the previous kernel's tail (PDL, common.cuh)
 
-    if (warp >= 8) {
-        setmaxnreg_dec<REGS_OTHER>();
-        if (warp == 8) {
-            // -------------------------------------------------------------- TMA producer
-            if (elect_one()) {
-                tma_prefetch_desc(&map_q);
-                tma_prefetch_desc(&map_k);
-                tma_prefetch_desc(&map_v);
-                mbar_expect_tx(bar_q, NT * TILE_BYTES);
-                for (int t = 0; t < NT; ++t)
-                    tma_load_3d(smem + SMEM_Q + t * TILE_BYTES, &map_q, bar_q, head * HD, q0 + t * BQ, b);
-                const int bkv = b / a.kv_batch_div;
-                for (int j = 0; j < n_kv; ++j) {
-                    const int s = j % ST;
-                    if (j >= ST) mbar_wait(&kv_empty[s], ((j / ST) - 1) & 1);
-                    mbar_expect_tx(&kv_full[s], 2 * TILE_BYTES);
-                    tma_load_3d(smem + SMEM_K + s * TILE_BYTES, &map_k, &kv_full[s], head * HD, j * BKV, bkv);
-                    tma_load_3d(smem + SMEM_V + s * TILE_BYTES, &map_v, &kv_full[s], head * HD, j * BKV, bkv);
-                }
-                griddep_launch();          // all loads issued: dependents may be scheduled as SMs drain
+    if (wg == 0) {
+        // ------------------------------------------------------------------ TMA producer
+        setmaxnreg_dec<REGS_PRODUCER>();
+        if (threadIdx.x < 32 && elect_one()) {
+            tma_prefetch_desc(&map_q);
+            tma_prefetch_desc(&map_k);
+            tma_prefetch_desc(&map_v);
+            mbar_expect_tx(bar_q, TILE_BYTES);
+            tma_load_3d(smem + SMEM_Q, &map_q, bar_q, head * HD, q0, b);
+            const int bkv = b / a.kv_batch_div;
+            for (int j = 0; j < n_kv; ++j) {
+                const int s = j % ST;
+                if (j >= ST) mbar_wait(&kv_empty[s], ((j / ST) - 1) & 1);
+                mbar_expect_tx(&kv_full[s], 2 * TILE_BYTES);
+                tma_load_3d(smem + SMEM_K + s * TILE_BYTES, &map_k, &kv_full[s], head * HD, j * BKV, bkv);
+                tma_load_3d(smem + SMEM_V + s * TILE_BYTES, &map_v, &kv_full[s], head * HD, j * BKV, bkv);
             }
-        } else if (warp == 9) {
-            // -------------------------------------------------------------- MMA issuer
-            if (elect_one()) {
-                constexpr uint32_t idesc_s = umma_idesc_f16(BQ, BKV);
-                constexpr uint32_t idesc_pv = umma_idesc_f16(BQ, HD) | UMMA_IDESC_B_MN_MAJOR;
-                const uint32_t sq_addr = smem_u32(smem + SMEM_Q);
-                const uint32_t sk_addr = smem_u32(smem + SMEM_K);
-                const uint32_t sv_addr = smem_u32(smem + SMEM_V);
-                auto issue_s = [&](int t, int s) {
-                    const uint64_t dq = umma_desc_k_sw128(sq_addr + t * TILE_BYTES);
-                    const uint64_t dk = umma_desc_k_sw128(sk_addr + s * TILE_BYTES);
-#pragma unroll
-                    for (int ks = 0; ks < HD / 16; ++ks)
-                        umma_f16(tmem_base + TMEM_S + t * BKV, dq + 2 * ks, dk + 2 * ks, idesc_s, ks > 0);
-                    umma_commit(&s_full[t]);
-                };
-                auto issue_pv = [&](int t, int j) {
-                    const int s = j % ST;
-#pragma unroll
-                    for (int ks = 0; ks < BKV / 16; ++ks) {
-                        // A = P_t from TMEM: 16 keys = 8 packed columns per k-step; B = V: 16 key rows = 2048 B per k-step
-                        const uint64_t dv = umma_desc_mn_sw128(sv_addr + s * TILE_BYTES + ks * 2048);
-                        umma_f16_ts(tmem_base + TMEM_O + t * HD, tmem_base + TMEM_P + t * (BKV / 2) + ks * 8, dv, idesc_pv,
-                                    (j > 0 || ks > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&pv_full[t]);
-                };
-                mbar_wait(bar_q, 0);
-                for (int j = 0; j < n_kv; ++j) {
-                    const int s = j % ST;
-                    mbar_wait(&kv_full[s], (j / ST) & 1);
-                    tc_fence_after();
-                    for (int t = 0; t < NT; ++t) {
-                        if (j > 0) {
-                            mbar_wait(&s_free[t], (j - 1) & 1);
-                            tc_fence_after();
-                        }
-                        issue_s(t, s);
-                    }
-                    if (j > 0) {
-                        for (int t = 0; t < NT; ++t) {
-                            mbar_wait(&p_full[t], (j - 1) & 1);
-                            tc_fence_after();
-                            issue_pv(t, j - 1);
-                        }
-                        umma_commit(&kv_empty[(j - 1) % ST]);
-                    }
-                }
-                for (int t = 0; t < NT; ++t) {
-                    mbar_wait(&p_full[t], (n_kv - 1) & 1);
-                    tc_fence_after();
-                    issue_pv(t, n_kv - 1);
-                }
-            }
+            griddep_launch();          // all loads issued: dependents may be scheduled as SMs drain
         }
+        __syncwarp();
     } else {
-        // ------------------------------------------------------------------ softmax / output (thread = query row)
-        setmaxnreg_inc<REGS_SOFTMAX>();
-        const int t = warp >> 2;
-        const int row = (warp & 3) * 32 + lane;                      // row inside the tile = TMEM lane
-        const uint32_t lane_base = static_cast<uint32_t>((warp & 3) * 32) << 16;
-        const uint32_t tS = tmem_base + lane_base + TMEM_S + t * BKV;
-        const uint32_t tP = tmem_base + lane_base + TMEM_P + t * (BKV / 2);
-        const uint32_t tO = tmem_base + lane_base + TMEM_O + t * HD;
+        // ------------------------------------------------------------------ consumers (64 query rows each)
+        setmaxnreg_inc<REGS_CONSUMER>();
+        const int cw = wg - 1;
+        const int lt = threadIdx.x & 127;
+        const int wr = lt >> 5, lane = lt & 31;
+        const int quad = lane & 3;
         const float sl2 = a.sl2;
-        if (t == 1) named_bar_arrive(2, 2 * BQ);             // MUFU turn-taking: group 0 goes first
-        float m_used = -INFINITY;        // exponent offset in use (<= true running max, lags it by at most RESCALE_LOG2)
-        float l_run = 0.f;
+        const uint64_t dq = wgmma_desc_sw128(smem_u32(smem + SMEM_Q) + cw * (64 * 128));
+        const uint32_t sk_addr = smem_u32(smem + SMEM_K);
+        const uint32_t sv_addr = smem_u32(smem + SMEM_V);
+        float o[HD / 2];
+#pragma unroll
+        for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+        float m_run[2] = {-INFINITY, -INFINITY};      // running max of rows g, g + 8 (g = lane / 4)
+        float l_run[2] = {0.f, 0.f};                  // this thread's share of the row sums
+        mbar_wait(bar_q, 0);
 
         for (int j = 0; j < n_kv; ++j) {
-            const int valid = a.skv - j * BKV;                       // >= BKV: the whole tile is real keys
-            mbar_wait(&s_full[t], j & 1);
-            tc_fence_after();
-            uint32_t s[BKV];
+            const int s = j % ST;
+            mbar_wait(&kv_full[s], (j / ST) & 1);
+            float sc[BKV / 2];
+            const uint64_t dk = wgmma_desc_sw128(sk_addr + s * TILE_BYTES);
+            wgmma_fence();
 #pragma unroll
-            for (int c = 0; c < BKV / 32; ++c) tmem_ld_32x32_p(tS + c * 32, s + c * 32);
-            tmem_ld_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s_free[t]);                  // S_t(j+1) may overwrite the TMEM copy now
+            for (int ks = 0; ks < HD / 16; ++ks) wgmma_ss<BKV>(sc, dq + 2 * ks, dk + 2 * ks, ks > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int i = 0; i < BKV / 2; ++i) reg_fence(sc[i]);
 
-            // ---- row max (padding keys of a ragged last tile -> -inf); four independent chains
+            // ---- padding keys of a ragged last tile -> -inf; row max over the quad's 4 threads
+            const int valid = a.skv - j * BKV;
             if (valid < BKV) {
 #pragma unroll
-                for (int i = 0; i < BKV; ++i)
-                    if (i >= valid) s[i] = 0xff800000u;
+                for (int i = 0; i < BKV / 2; ++i)
+                    if (8 * (i >> 2) + 2 * quad + (i & 1) >= valid) sc[i] = -INFINITY;
             }
-            float mx4[4];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                mx4[c] = fmaxf(__uint_as_float(s[c * 32]), __uint_as_float(s[c * 32 + 1]));
-#pragma unroll
-                for (int i = 2; i < 32; i += 2)
-                    mx4[c] = fmax3(mx4[c], __uint_as_float(s[c * 32 + i]), __uint_as_float(s[c * 32 + i + 1]));
-            }
-            const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-
-            // ---- move the exponent offset only when the row max outgrew it by 2^RESCALE_LOG2 (warp-uniform decision:
-            //      the TMEM accesses are warp-collective); rescaling a row that did not need it is exact (corr <= 1)
-            if (j == 0) {
-                m_used = mx;
-            } else if (__any_sync(0xffffffffu, (mx - m_used) * sl2 > RESCALE_LOG2)) {
-                mbar_wait(&pv_full[t], (j - 1) & 1);                 // O_t quiescent once PV_t(j-1) retired
-                tc_fence_after();
-                const float m_new = fmaxf(m_used, mx);
-                const float corr = ex2_approx((m_used - m_new) * sl2);
-                m_used = m_new;
-                l_run *= corr;
-                uint32_t r[HD];
-                tmem_ld_32x32_p(tO, r);
-                tmem_ld_32x32_p(tO + 32, r + 32);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < HD; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * corr);
-                tmem_st_32x32_p(tO, r);
-                tmem_st_32x32_p(tO + 32, r + 32);
-            }
-            // ---- P = exp2(S * c - m * c) -> fp16 pairs -> TMEM (A operand of the P.V MMA).  The MUFU is the scarcest unit
-            //      of the whole kernel (16 exp2/clk/SM): the two softmax groups take turns on it, so that one group's
-            //      loads / max / stores always run under the other group's exponentials instead of both stalling on it.
-            const float msc = m_used * sl2;
-            float sum0 = 0.f, sum1 = 0.f;
-            named_bar_sync(2 + t, 2 * BQ);
+            float corr[2], msc[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                uint32_t pk[BKV / 4];
+                float mx = -INFINITY;
 #pragma unroll
-                for (int i = 0; i < BKV / 2; i += 2) {
-                    const float p0 = ex2_approx(fmaf(__uint_as_float(s[h * 64 + i]), sl2, -msc));    // exp2(-inf) = 0
-                    const float p1 = ex2_approx(fmaf(__uint_as_float(s[h * 64 + i + 1]), sl2, -msc));
-                    sum0 += p0;
-                    sum1 += p1;
-                    const __half2 hh = __floats2half2_rn(p0, p1);
-                    pk[i >> 1] = *reinterpret_cast<const uint32_t*>(&hh);
-                }
-                if (h == 0 && j > 0) {                               // P_t(j-1) consumed once PV_t(j-1) retired
-                    mbar_wait(&pv_full[t], (j - 1) & 1);
-                    tc_fence_after();
-                }
-                if (h == 1 && !(t == 1 && j == n_kv - 1)) named_bar_arrive(2 + (t ^ 1), 2 * BQ);   // hand the MUFU over
-                tmem_st_32x32_p(tP + h * 32, pk);
+                for (int jj = 0; jj < BKV / 8; ++jj) mx = fmaxf(mx, fmaxf(sc[4 * jj + 2 * h], sc[4 * jj + 2 * h + 1]));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                const float m_new = fmaxf(m_run[h], mx);
+                corr[h] = ex2_approx((m_run[h] - m_new) * sl2);         // exp2(-inf) = 0 on the first tile
+                m_run[h] = m_new;
+                msc[h] = m_new * sl2;
+                l_run[h] *= corr[h];
             }
-            l_run += sum0 + sum1;
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&p_full[t]);
+#pragma unroll
+            for (int i = 0; i < HD / 2; ++i) o[i] *= corr[(i >> 1) & 1];
+
+            // ---- P = exp2(S * c - m * c) -> fp16 A fragments (k-step ks covers keys 16 ks .. 16 ks + 15)
+            uint32_t pf[BKV / 16][4];
+#pragma unroll
+            for (int ks = 0; ks < BKV / 16; ++ks) {
+                float pv[8];
+#pragma unroll
+                for (int e = 0; e < 8; ++e) {
+                    const int h = (e >> 1) & 1;
+                    pv[e] = ex2_approx(fmaf(sc[8 * ks + e], sl2, -msc[h]));     // exp2(-inf) = 0
+                    l_run[h] += pv[e];
+                }
+                pf[ks][0] = pack_half2(pv[0], pv[1]);      // row g,     keys 16 ks + 2 quad + {0, 1}
+                pf[ks][1] = pack_half2(pv[2], pv[3]);      // row g + 8, same keys
+                pf[ks][2] = pack_half2(pv[4], pv[5]);      // row g,     keys 16 ks + 8 + 2 quad + {0, 1}
+                pf[ks][3] = pack_half2(pv[6], pv[7]);      // row g + 8, same keys
+            }
+            // ---- O += P V_j: 16 key rows of V = 2048 B per k-step
+#pragma unroll
+            for (int i = 0; i < HD / 2; ++i) reg_fence(o[i]);
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < BKV / 16; ++ks)
+                wgmma_rs_n64_tb(o, pf[ks], wgmma_desc_sw128(sv_addr + s * TILE_BYTES + ks * 2048));
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int i = 0; i < HD / 2; ++i) reg_fence(o[i]);
+            if (lt == 0) mbar_arrive(&kv_empty[s]);
         }
         // ---- normalise, store
-        mbar_wait(&pv_full[t], (n_kv - 1) & 1);
-        tc_fence_after();
-        const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
-        const int qrow = q0 + t * BQ + row;
-        __half* orow = a.o + static_cast<long long>(b) * a.o_bs + static_cast<long long>(qrow) * a.o_ss + head * HD;
 #pragma unroll
-        for (int c = 0; c < HD / 32; ++c) {
-            uint32_t r[32];
-            tmem_ld_32x32(tO + c * 32, r);
-            tmem_ld_wait();
-            uint32_t w[16];
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-                const __half2 h = __floats2half2_rn(__uint_as_float(r[i]) * inv, __uint_as_float(r[i + 1]) * inv);
-                w[i >> 1] = *reinterpret_cast<const uint32_t*>(&h);
-            }
+        for (int h = 0; h < 2; ++h) {
+            float l = l_run[h];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv = l > 0.f ? 1.f / l : 0.f;
+            const int qrow = q0 + cw * 64 + wr * 16 + (lane >> 2) + 8 * h;
             if (qrow < a.sq) {
+                __half* orow = a.o + static_cast<long long>(b) * a.o_bs + static_cast<long long>(qrow) * a.o_ss + head * HD;
 #pragma unroll
-                for (int q = 0; q < 2; ++q) {
-                    U32x8 v;
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) v.v[i] = w[q * 8 + i];
-                    stg_256(orow + c * 32 + q * 16, v);
-                }
+                for (int jj = 0; jj < HD / 8; ++jj)
+                    *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * quad) =
+                        pack_half2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 9) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
     }
 }
 
@@ -328,12 +219,12 @@ bool attention_tc_eligible(const AttnParams& p) {
     const long long strides[] = {p.q_bs, p.q_ss, p.k_bs, p.k_ss, p.v_bs, p.v_ss};
     for (long long s : strides)
         if (s <= 0 || (s & 7) != 0) return false;                   // TMA: 16 B multiples
-    if ((p.o_bs & 15) != 0 || (p.o_ss & 15) != 0) return false;     // 32 B output stores
+    if ((p.o_bs & 1) != 0 || (p.o_ss & 1) != 0) return false;       // fp16 pairs per store
     const uintptr_t ptrs[] = {reinterpret_cast<uintptr_t>(p.q), reinterpret_cast<uintptr_t>(p.k),
                               reinterpret_cast<uintptr_t>(p.v)};
     for (uintptr_t x : ptrs)
         if (x & 15) return false;
-    if (reinterpret_cast<uintptr_t>(p.o) & 31) return false;
+    if (reinterpret_cast<uintptr_t>(p.o) & 3) return false;
     if (p.heads > 65535 || p.batch > 65535) return false;
     return true;
 }
@@ -342,7 +233,7 @@ int attention_tc_plan(const AttnParams& p, AttnTcPlan* plan) {
     if (!attention_tc_eligible(p)) return -1;
     if (!g_attr_set) {
         if (cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL) != cudaSuccess) {
-            fprintf(stderr, "[t2v_b200] attention_tc: cudaFuncSetAttribute failed: %s\n", cudaGetErrorString(cudaGetLastError()));
+            fprintf(stderr, "[t2v] attention_tc: cudaFuncSetAttribute failed: %s\n", cudaGetErrorString(cudaGetLastError()));
             return -2;
         }
         g_attr_set = true;
@@ -385,7 +276,7 @@ int attention_tc_launch(const AttnTcPlan& pl, cudaStream_t stream) {
     a.kv_batch_div = pl.kv_batch_div;
     a.n_kv = (pl.skv + BKV - 1) / BKV;
     a.sl2 = pl.sl2;
-    dim3 grid((pl.sq + NT * BQ - 1) / (NT * BQ), pl.heads, pl.batch);
+    dim3 grid((pl.sq + BQ - 1) / BQ, pl.heads, pl.batch);
     launch_pdl(attention_tc_kernel, grid, NTHREADS, SMEM_TOTAL, stream, pl.map_q, pl.map_k, pl.map_v, a);
     return launch_status("attention_tc launch");
 }

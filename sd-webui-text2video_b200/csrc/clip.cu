@@ -6,7 +6,7 @@
 // architecture restated here is open_clip's published ResidualAttentionBlock, pinned in tests against torch's own
 // nn.MultiheadAttention / nn.LayerNorm modules.
 //
-// Same engine as the denoiser: LayerNorm folded into the consuming tcgen05 GEMM, residual adds in the GEMM epilogue; the
+// Same engine as the denoiser: LayerNorm folded into the consuming wgmma GEMM, residual adds in the GEMM epilogue; the
 // 77-token causal attention and the GELU are small dedicated kernels (the tower runs once per prompt: 2 x 77 rows).
 #include "../../include/t2v_b200.h"
 #include "runtime.cuh"

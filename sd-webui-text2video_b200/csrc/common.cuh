@@ -15,9 +15,8 @@ void clear_pending_error(const char* where);
 // Every kernel of the library executes griddep_wait() (all prerequisite grids complete, their writes visible) once its
 // input-independent prologue is done; the GEMM / attention producers signal griddep_launch() when they have issued their
 // last load, so the NEXT kernel of the stream may be scheduled onto SMs as they drain and run ITS prologue (barrier init,
-// TMEM allocation, tensor-map prefetch, index math) under this kernel's tail.  Measured on the CUDA-graphed B=2 forward
-// at 24f x 256^2: 26.02-26.15 ms with PDL edges vs 25.40 ms with plain stream order (both trigger placements tried), so
-// the attribute is NOT set by default; without it the device-side instructions are no-ops.
+// tensor-map prefetch, index math) under this kernel's tail.  The attribute is NOT set by default (it has not been shown
+// to shorten the CUDA-graphed forward); without it the device-side instructions are no-ops.
 bool pdl_enabled();
 #ifdef __CUDACC__
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

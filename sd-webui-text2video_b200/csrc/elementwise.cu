@@ -10,7 +10,7 @@ namespace t2v {
 
 namespace {
 
-inline int grid_for(long long n, int threads, int cap = 148 * 16) {
+inline int grid_for(long long n, int threads, int cap = 132 * 16) {
     long long b = (n + threads - 1) / threads;
     if (b > cap) b = cap;
     if (b < 1) b = 1;

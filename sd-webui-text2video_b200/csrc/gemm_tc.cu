@@ -1,11 +1,14 @@
-// tcgen05 / TMEM / TMA implicit-GEMM kernel (sm_100a).  See gemm_tc.cuh for the data model.
+// wgmma / TMA implicit-GEMM kernel (sm_90a).  See gemm_tc.cuh for the data model.
 //
-// Per CTA (persistent, 320 threads, 1 CTA/SM):
-//   warp 0      TMA producer  : per k-iteration one A box (128 rows x 64 K, tap-shifted coordinates, OOB = zero
-//                               padding) + one B box (BN x 64 K) into a SWIZZLE_128B smem ring
-//   warp 1      MMA issuer    : lane 0 issues 4 x tcgen05.mma (M=128, N=BN, K=16) per stage into a double-buffered
-//                               fp32 accumulator in TMEM; tcgen05.commit releases the smem stage / publishes the tile
-//   warps 2..9  epilogue      : tcgen05.ld 32 lanes x 32 columns -> registers -> alpha, bias, residual, GEGLU -> HBM
+// Per CTA (persistent, 384 threads = 3 warpgroups, 1 CTA/SM):
+//   warpgroup 0     TMA producer : one elected thread issues, per k-iteration, one A box (128 rows x 64 K, tap-shifted
+//                                  coordinates, OOB = zero padding) + one B box (BN x 64 K) into a SWIZZLE_128B smem ring
+//   warpgroups 1, 2 consumers    : each owns 64 rows of the 128-row tile; per ring stage 4 k-steps of wgmma m64 x BN x 16
+//                                  (both operands from shared memory) into fp32 registers, then the epilogue (alpha, bias,
+//                                  LayerNorm fold, residual, GEGLU) straight from the accumulator registers to global memory.
+// The producer runs ahead into the next tile while the consumers are in the epilogue.
+// CG = 2: a cluster of two CTAs owns two consecutive M-tiles of the same N-tile; each CTA fetches half of the B box and
+// TMA-multicasts it into both CTAs, so B crosses L2 -> SM once per pair.
 // Roofline: tensor-bound (2*M*N*K*taps flop per launch) whenever K*taps is large; see DESIGN.md.
 #include "common.cuh"
 #include "gemm_tc.cuh"
@@ -20,80 +23,26 @@ namespace t2v {
 
 namespace {
 
-// TMA warp + MMA warp + EW epilogue warps (8: two per TMEM lane quadrant).  The GEGLU epilogue has its own lean loop
-// (A&S erfc-form GELU on MUFU, paired fp16 conversions, HMUL2 product, no residual / scalar fallbacks): with the generic
-// path and erff() it was capped at 96 registers with spills and ran at 364 TFLOP/s on the level-0 FF (K = 320); the
-// dedicated loop reaches 740 (profiles/r01_gemm_isolation.txt).  -DT2V_GEGLU_EW=16 builds the 16-warp / 16-column variant.
-#ifndef T2V_GEGLU_EW
-#define T2V_GEGLU_EW 8
-#endif
-// Epilogue latency-hiding experiments for the generic (non-GEGLU) path, build-time switches.  Both measured on B200
-// (profiles/r02_gemm_epilogue_ab.txt): neither moves the K = 320 layers nor the forward (23.00 / 23.26 / 23.06 / 23.27 ms for
-// 00 / 10 / 01 / 11, run-to-run noise +-0.15 ms), so they are OFF by default:
-//   T2V_EPI_PIPE   : the tcgen05.ld of the NEXT column chunk is in flight while the current chunk is converted and stored
-//   T2V_EPI_STAGE2 : two TMA-store staging buffers per epilogue warp (the store of chunk i reads its buffer while chunk i+1 is staged)
-#ifndef T2V_RES_LATE
-#define T2V_RES_LATE 1
-#endif
-#ifndef T2V_RES_DEPTH
-#define T2V_RES_DEPTH 3
-#endif
-#ifndef T2V_EPI_PIPE
-#define T2V_EPI_PIPE 0
-#endif
-// T2V_MMA_UNROLL2: two ring stages per MMA-loop trip (one wait / fence per 8 MMAs).  Measured SLOWER (forward 22.77 vs 21.91 ms,
-// profiles/r02_gemm_single_thread_roles_ab.txt): waiting for the second stage delays the first MMAs more than the saved loop trip.
-#ifndef T2V_MMA_UNROLL2
-#define T2V_MMA_UNROLL2 0
-#endif
-#ifndef T2V_EPI_STAGE2
-#define T2V_EPI_STAGE2 0
-#endif
-// In-kernel timeline (build with -DT2V_GEMM_TRACE=1 into a separate library, scripts/gemm_trace.py): two CTAs record clock64
-// stamps of what each role waits for -- producer: ring slot free; MMA: operands landed / accumulator drained / tile committed;
-// two epilogue warps: accumulator ready, chunk loaded, staging buffer free, store issued.  Compiles to nothing by default.
-#ifndef T2V_GEMM_TRACE
-#define T2V_GEMM_TRACE 0
-#endif
-#if T2V_GEMM_TRACE
-constexpr int TRACE_CAP = 4096;
-__device__ unsigned long long* g_trace_buf = nullptr;      // [2 CTAs][4 roles][TRACE_CAP]
-#define TRACE_DECL(role)                                                                                         \
-    unsigned long long* tr_ = nullptr;                                                                           \
-    int tri_ = 0;                                                                                                \
-    {                                                                                                            \
-        const int slot_ = blockIdx.x == 0 ? 0 : (blockIdx.x == gridDim.x / 2 ? 1 : -1);                          \
-        if (g_trace_buf != nullptr && slot_ >= 0 && (role) >= 0) tr_ = g_trace_buf + (slot_ * 4 + (role)) * TRACE_CAP; \
-    }
-#define TRACE(tag)                                                                                               \
-    do {                                                                                                         \
-        if (tr_ != nullptr && tri_ < TRACE_CAP) tr_[tri_++] = (static_cast<unsigned long long>(clock64()) << 8) | static_cast<unsigned long long>(tag); \
-    } while (0)
-#else
-#define TRACE_DECL(role)
-#define TRACE(tag)
-#endif
-constexpr int epi_warps(bool geglu) { return geglu ? T2V_GEGLU_EW : 8; }
-constexpr int n_threads(bool geglu) { return 64 + 32 * epi_warps(geglu); }
-constexpr int kABytes = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;   // 16 KB
-constexpr int kSmemBudget = 200 * 1024;                     // ring budget (barriers + alignment slack on top)
+constexpr int kThreads = 384;
+constexpr int kRegsProducer = 40;                            // setmaxnreg budgets: 128 x 40 + 256 x 232 <= 64 K registers
+constexpr int kRegsConsumer = 232;
+constexpr int kABytes = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;     // 16 KB
+constexpr int kSmemBudget = 216 * 1024;                      // ring (barriers + alignment slack on top; 227 KB per block)
+constexpr int kMaxStages = 8;
 
-template <int BN, int CG>
+template <int BN>
 struct Cfg {
-    static constexpr int kBBytes = (BN / CG) * GEMM_BLOCK_K * 2;      // a CTA of a pair stages half of the B tile
+    static constexpr int kBBytes = BN * GEMM_BLOCK_K * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kStages = (kSmemBudget / kStageBytes) > 8 ? 8 : (kSmemBudget / kStageBytes);
-    static constexpr int kBaseBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + 4096 /*bias + colsum tiles*/ +
-                                      256 /*pad to 512*/ + 8 * 2048 /*TMA-store staging, one 32x32 fp16 chunk per epilogue warp*/;
-    static constexpr bool kStage2 = T2V_EPI_STAGE2 != 0 && kBaseBytes + 8 * 2048 <= 227 * 1024;     // second staging bank where it fits
-    static constexpr int kSmemBytes = kBaseBytes + (kStage2 ? 8 * 2048 : 0);
+    static constexpr int kStages = (kSmemBudget / kStageBytes) > kMaxStages ? kMaxStages : (kSmemBudget / kStageBytes);
+    static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
-constexpr int kBsRing = kSmemBudget - (T2V_EPI_STAGE2 ? 8 * 2048 : 0);      // B-stationary: resident weights + A ring live below this offset
+constexpr int kBsSmemBytes = kSmemBudget + 1024 + 256;      // B-stationary: resident weights + A ring fill the budget
 
 // erf-form GELU x * Phi(x) (F.gelu default, t2v_model.py:821).  Phi(x) = 1/2 erfc(-x / sqrt 2); for z = |x| / sqrt 2
 // erfc(z) = t (a1 + t (a2 + t (a3 + t (a4 + t a5)))) exp(-z^2), t = 1 / (1 + p z) (Abramowitz-Stegun 7.1.26, |error| <=
 // 1.5e-7 -- three orders below the fp16 rounding the reference applies to the result).  2 MUFU (rcp, ex2) + 13 FMA-pipe
-// instructions instead of erff's ~32: the GEGLU epilogue is instruction-issue bound at K = 320.
+// instructions instead of erff's ~32.
 __device__ __forceinline__ float gelu_erf(float x) {
     const float z = fabsf(x) * 0.70710678118654752440f;
     float t;
@@ -106,70 +55,63 @@ __device__ __forceinline__ float gelu_erf(float x) {
     return x * (x < 0.f ? q : 1.0f - q);
 }
 
+// One K = 16 step of a 64 x BN tile: BN is split into wgmma widths of 256 / 128 / 64 / 32 / 16.  Chunk n0 reads B rows
+// n0.. (n0 * 128 B further, a whole number of 1024 B swizzle atoms) and accumulates into registers acc[n0 / 2 ..].
+template <int BN>
+__device__ __forceinline__ void mma_k16(float* acc, uint64_t da, uint64_t db, uint32_t scale_d) {
+    if constexpr (BN == 256 || BN == 128 || BN == 64 || BN == 32 || BN == 16) {
+        wgmma_ss<BN>(acc, da, db, scale_d);
+    } else if constexpr (BN > 128) {
+        wgmma_ss<128>(acc, da, db, scale_d);
+        mma_k16<BN - 128>(acc + 64, da, db + static_cast<uint64_t>((128 * 128) >> 4), scale_d);
+    } else if constexpr (BN > 64) {
+        wgmma_ss<64>(acc, da, db, scale_d);
+        mma_k16<BN - 64>(acc + 32, da, db + static_cast<uint64_t>((64 * 128) >> 4), scale_d);
+    } else {
+        static_assert(BN < 0, "unsupported tile width");
+    }
+}
+
 // BS = "B-stationary": the CTA keeps the WHOLE weight slice of its N-tile (all taps x K chunks) resident in shared memory and
-// walks M-tiles of that N-tile only, so per tile just the A box moves through the ring.  Chosen by gemm_plan for the K = 320
-// layers (level 0: 30 % of the forward's GEMM time at 15-37 % tensor pipe): those are bound by the aggregate L2 -> SM operand
-// stream (~12 TB/s, profiles/r01_gemm_isolation.txt), and with BN = 160 the B box (100 KB) outweighs the A box (80 KB) --
-// re-fetching it for every tile was more than half of the traffic.
+// walks M-tiles of that N-tile only, so per tile just the A box moves through the ring.
 template <int BN, bool GEGLU, int CG, bool BS = false>
-__global__ void __launch_bounds__(n_threads(GEGLU), 1) gemm_tc_kernel(const __grid_constant__ GemmDesc g) {
-    constexpr int EW = epi_warps(GEGLU);
-    using C = Cfg<BN, CG>;
+__global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmDesc g) {
+    using Cf = Cfg<BN>;
     static_assert(!BS || CG == 1, "B-stationary tiles are single-CTA");
-    constexpr int kBarStages = BS ? 8 : C::kStages;                 // barrier slots (BS: ring depth is a run-time value <= 8)
-    const uint32_t rank = CG == 2 ? cluster_ctarank() : 0u;      // position in the CTA pair
-    const bool leader = rank == 0;
+    constexpr int kBarStages = BS ? kMaxStages : Cf::kStages;      // barrier slots (BS: ring depth is a run-time value <= 8)
+    const uint32_t rank = CG == 2 ? cluster_ctarank() : 0u;       // position in the cluster
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
-    uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);      // SWIZZLE_128B atoms need 1024 B alignment
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (BS ? kBsRing : C::kStages * C::kStageBytes));
-    constexpr bool kStage2 = BS ? (T2V_EPI_STAGE2 != 0) : C::kStage2;
-    uint64_t* full = bars;                       // [kStages] TMA -> MMA
-    uint64_t* empty = bars + kBarStages;         // [kStages] MMA -> TMA
-    uint64_t* tfull = bars + 2 * kBarStages;     // [2] MMA -> epilogue
-    uint64_t* tempty = tfull + 2;                // [2] epilogue -> MMA
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-    uint64_t* bfull = tempty + 4;                // BS: the resident weight slice has landed (<= 8 * 20 + 8 = 168 B < 256)
+    uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);   // SWIZZLE_128B atoms need 1024 B alignment
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (BS ? kSmemBudget : Cf::kStages * Cf::kStageBytes));
+    uint64_t* full = bars;                       // [kStages] TMA -> consumers
+    uint64_t* empty = bars + kBarStages;         // [kStages] consumers (of both CTAs of a cluster) -> TMA
+    uint64_t* bfull = empty + kBarStages;        // BS: the resident weight slice has landed
     // BS smem map: [resident B: k_total chunks of BN x 64][A ring: bs_stages x 16 KB] ... barriers at the fixed ring budget
-    const int nst = BS ? g.bs_stages : C::kStages;
+    const int nst = BS ? g.bs_stages : Cf::kStages;
     uint8_t* const sB_res = smem;
-    uint8_t* const sA_ring = smem + (BS ? g.ntaps * g.k_chunks * C::kBBytes : 0);
-    float* bias_s = reinterpret_cast<float*>(bars) + 64;         // [2 accumulator stages][256] fp32 bias tile (256 B after the barriers)
-    float* csum_s = bias_s + 512;                                // [2][256] column sums of the gamma-scaled weights (GEMM_LN)
-    uint8_t* stage_s = reinterpret_cast<uint8_t*>(bars) + 4608;  // [8 warps][32 rows][64 B], 512 B aligned (SWIZZLE_64B atoms)
+    uint8_t* const sA_ring = smem + (BS ? g.ntaps * g.k_chunks * Cf::kBBytes : 0);
 
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&g.map_a);
         tma_prefetch_desc(&g.map_b);
         for (int i = 0; i < kBarStages; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 1);
+            mbar_init(&empty[i], 2 * CG);         // one arrival per consumer warpgroup of every CTA that writes this stage
         }
         if constexpr (BS) mbar_init(bfull, 1);
-        mbar_init(&tfull[0], 1);
-        mbar_init(&tfull[1], 1);
-        mbar_init(&tempty[0], EW * CG);           // the leader's barrier also collects the peer's epilogue warps
-        mbar_init(&tempty[1], EW * CG);
         fence_barrier_init();
     }
-    if (warp == 1) {                              // 2 accumulator stages x 256 fp32 columns
-        if constexpr (CG == 2) tmem_alloc_2sm(tmem_slot, 512);
-        else tmem_alloc(tmem_slot, 512);
-    }
-    tc_fence_before();
-    if constexpr (CG == 2) cluster_sync_all();    // peer barriers are initialised before any remote arrive / multicast
+    if constexpr (CG == 2) cluster_sync_all();    // peer barriers are initialised before any multicast / remote arrive
     else __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     griddep_wait();        // everything above is independent of the previous kernel's output (PDL, common.cuh)
 
-    // work items: (pair of consecutive M-tiles, N-tile); CTA `rank` of the pair owns M-tile 2*pm + rank
+    // work items: (pair of consecutive M-tiles, N-tile, K split); CTA `rank` of a cluster owns M-tile CG*pm + rank
     const int pairs_m = (g.tiles_m + CG - 1) / CG;
     const int nsplit = g.splits > 1 ? g.splits : 1;
-    const int total_pairs = pairs_m * g.tiles_n * nsplit;      // work items: (pair of M-tiles, N-tile, K split)
+    const int total_pairs = pairs_m * g.tiles_n * nsplit;
     const int k_total = g.ntaps * g.k_chunks;
     const int k_per = g.splits > 1 ? g.k_per_split : k_total;
     // BS: this CTA owns N-tile bs_tn and walks the M-tiles first_pair, first_pair + pair_stride, ... (work item = M-tile)
@@ -178,23 +120,20 @@ __global__ void __launch_bounds__(n_threads(GEGLU), 1) gemm_tc_kernel(const __gr
     const int pair_stride = BS ? (static_cast<int>(gridDim.x) - bs_tn + g.tiles_n - 1) / g.tiles_n : static_cast<int>(gridDim.x) / CG;
     const int total_items = BS ? g.tiles_m : total_pairs;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ------------------------------------------------------------------ TMA producer
-        // ONE ELECTED lane (elect.sync) runs the whole loop.  Inside an `if (lane == 0)` region the compiler cannot prove the
-        // operands of the uniform-datapath instructions (UTMALDG / UTCHMMA / UTCBAR) uniform and wraps every one of them in an
-        // ELECT + R2UR.BROADCAST + BRA.U.ANY "waterfall" loop -- measured with the in-kernel timeline: 240-320 clk per TMA issue,
-        // 496 clk for the four MMAs + commit of a stage, i.e. the ISSUING THREADS paced the pipe at ~700 clk per K step for
-        // every tile width (the tensor pipe needs 320-512).  An elect.sync region is compiled as single-threaded code.
-        if (elect_one()) {
-            TRACE_DECL(0);
+        setmaxnreg_dec<kRegsProducer>();
+        // One elected thread runs the whole loop (an elect.sync region compiles to single-threaded code for the uniform TMA
+        // instructions).  Loop-invariant descriptor fields are hoisted into registers and (tap, K chunk) advance by counters.
+        if (threadIdx.x < 32 && elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
             if constexpr (BS) {
                 if (first_pair < total_items) {        // the resident weight slice: every (tap, K chunk) box of N-tile bs_tn, once
-                    mbar_expect_tx(bfull, static_cast<uint32_t>(k_total * C::kBBytes));
+                    mbar_expect_tx(bfull, static_cast<uint32_t>(k_total * Cf::kBBytes));
                     const int kch0 = g.k_chunks;
                     for (int it = 0, tap = 0, kc = 0; it < k_total; ++it) {
-                        tma_load_3d(sB_res + it * C::kBBytes, &g.map_b, bfull, kc * GEMM_BLOCK_K, bs_tn * BN, tap);
+                        tma_load_3d(sB_res + it * Cf::kBBytes, &g.map_b, bfull, kc * GEMM_BLOCK_K, bs_tn * BN, tap);
                         if (++kc == kch0) {
                             kc = 0;
                             ++tap;
@@ -202,12 +141,6 @@ __global__ void __launch_bounds__(n_threads(GEGLU), 1) gemm_tc_kernel(const __gr
                     }
                 }
             }
-            // The loop below is ONE thread's dependent instruction chain per k-iteration; the in-kernel timeline
-            // (profiles/r02_gemm_timeline.md) showed it at 700-900 clk per iteration -- integer divisions, indexed constant loads and
-            // the tile-origin div/mod chain -- i.e. SLOWER than the 320-512 clk the tensor pipe needs per stage, so the producer, not
-            // the MMA or L2, paced every K <= 640 layer.  Hence: kernel parameters hoisted into registers, (tap, K chunk) advanced
-            // by counters instead of divided out, tap offsets re-read only when the tap changes, plain row matrices (nd == 1)
-            // skip the origin div/mod chain.
             const int kch = g.k_chunks, nd = g.nd, a_tx = g.a_tx_bytes, tiles_n_ = g.tiles_n, tiles_m_ = g.tiles_m;
             const int bdim = g.b_batch_dim;
             for (int wi = first_pair; wi < total_items; wi += pair_stride) {
@@ -238,8 +171,8 @@ __global__ void __launch_bounds__(n_threads(GEGLU), 1) gemm_tc_kernel(const __gr
                         }
                     }
                 }
-                if (tmi >= tiles_m_) org[0] = g.dim[0];       // odd tail: this CTA's half is all out of bounds (zeros)
-                const int bbatch = bdim < 0 ? 0 : (bdim == 0 ? org[0] : (bdim == 1 ? org[1] : (bdim == 2 ? org[2] : org[3])));     // no indexed local array
+                if (tmi >= tiles_m_) org[0] = g.dim[0];       // odd tail of a cluster: this CTA's tile is all out of bounds (zeros)
+                const int bbatch = bdim < 0 ? 0 : (bdim == 0 ? org[0] : (bdim == 1 ? org[1] : (bdim == 2 ? org[2] : org[3])));
                 int tap = 0, kc = it0;
                 if (it0 >= kch) {
                     tap = it0 / kch;
@@ -249,37 +182,21 @@ __global__ void __launch_bounds__(n_threads(GEGLU), 1) gemm_tc_kernel(const __gr
                 int c3 = org[2] + g.tap_off[tap][2], c4 = org[3] + g.tap_off[tap][3];
                 for (int it = it0; it < it1; ++it) {
                     mbar_wait(&empty[stage], phase ^ 1u);
-                    TRACE(1);
-                    uint8_t* sa = BS ? sA_ring + stage * kABytes : smem + stage * C::kStageBytes;
+                    uint8_t* sa = BS ? sA_ring + stage * kABytes : smem + stage * Cf::kStageBytes;
                     uint8_t* sb = sa + kABytes;
                     const int k0 = kc * GEMM_BLOCK_K;
-                    if constexpr (BS) {
-                        mbar_expect_tx(&full[stage], static_cast<uint32_t>(a_tx));
-                        TRACE(11);
-                        if (nd == 1) tma_load_2d(sa, &g.map_a, &full[stage], k0, c1);
-                        else if (nd == 2) tma_load_3d(sa, &g.map_a, &full[stage], k0, c1, c2);
-                        else if (nd == 3) tma_load_4d(sa, &g.map_a, &full[stage], k0, c1, c2, c3);
-                        else tma_load_5d(sa, &g.map_a, &full[stage], k0, c1, c2, c3, c4);
-                        TRACE(12);
-                    } else if constexpr (CG == 2) {
-                        // both CTAs' bytes complete on the LEADER's barrier; only the leader arms it
-                        if (leader) mbar_expect_tx(&full[stage], static_cast<uint32_t>(2 * (a_tx + C::kBBytes)));
-                        const uint32_t lb = leader_bar_addr(&full[stage]);
-                        if (nd == 1) tma_load_2d_2sm(sa, &g.map_a, lb, k0, c1);
-                        else if (nd == 2) tma_load_3d_2sm(sa, &g.map_a, lb, k0, c1, c2);
-                        else if (nd == 3) tma_load_4d_2sm(sa, &g.map_a, lb, k0, c1, c2, c3);
-                        else tma_load_5d_2sm(sa, &g.map_a, lb, k0, c1, c2, c3, c4);
-                        tma_load_3d_2sm(sb, &g.map_b, lb, k0, tn * BN + static_cast<int>(rank) * (BN / 2), tap + bbatch);
-                    } else {
-                        mbar_expect_tx(&full[stage], static_cast<uint32_t>(a_tx + C::kBBytes));
-                        TRACE(11);
-                        if (nd == 1) tma_load_2d(sa, &g.map_a, &full[stage], k0, c1);
-                        else if (nd == 2) tma_load_3d(sa, &g.map_a, &full[stage], k0, c1, c2);
-                        else if (nd == 3) tma_load_4d(sa, &g.map_a, &full[stage], k0, c1, c2, c3);
-                        else tma_load_5d(sa, &g.map_a, &full[stage], k0, c1, c2, c3, c4);
-                        TRACE(12);
+                    mbar_expect_tx(&full[stage], static_cast<uint32_t>(a_tx + (BS ? 0 : Cf::kBBytes)));
+                    if (nd == 1) tma_load_2d(sa, &g.map_a, &full[stage], k0, c1);
+                    else if (nd == 2) tma_load_3d(sa, &g.map_a, &full[stage], k0, c1, c2);
+                    else if (nd == 3) tma_load_4d(sa, &g.map_a, &full[stage], k0, c1, c2, c3);
+                    else tma_load_5d(sa, &g.map_a, &full[stage], k0, c1, c2, c3, c4);
+                    if constexpr (CG == 2) {
+                        // this CTA's half of the B box, into the same place of both CTAs' stage
+                        constexpr int kHalf = BN / 2;
+                        tma_load_3d_mc(sb + rank * (kHalf * GEMM_BLOCK_K * 2), &g.map_b, &full[stage], k0,
+                                       tn * BN + static_cast<int>(rank) * kHalf, tap + bbatch, static_cast<uint16_t>(3));
+                    } else if constexpr (!BS) {
                         tma_load_3d(sb, &g.map_b, &full[stage], k0, tn * BN, tap + bbatch);
-                        TRACE(13);
                     }
                     if (++kc == kch) {              // next tap: new coordinate offsets (at most 9 times per tile)
                         kc = 0;
@@ -297,490 +214,178 @@ __global__ void __launch_bounds__(n_threads(GEGLU), 1) gemm_tc_kernel(const __gr
                     }
                 }
             }
-            // nothing left to fetch: only this CTA's last MMAs / epilogue remain -> let the next kernel's CTAs be scheduled
-            // (they run their prologue and block in griddepcontrol.wait until this grid has completed)
+            // nothing left to fetch: let the next kernel's CTAs be scheduled as SMs drain (PDL)
             griddep_launch();
         }
         __syncwarp();
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (pair leader only)
-        constexpr uint32_t idesc = umma_idesc_f16(GEMM_BLOCK_M * CG, BN);
-        if (leader && elect_one()) {
-        TRACE_DECL(1);
+    } else {
+        // ------------------------------------------------------------------ consumers: MMA + epilogue
+        setmaxnreg_inc<kRegsConsumer>();
+        const int cw = wg - 1;                        // rows 64 cw .. 64 cw + 63 of the tile
+        const int lt = threadIdx.x & 127;
+        const int wr = lt >> 5, lane = lt & 31;
+        const int quad = lane & 3;
         int stage = 0;
         uint32_t phase = 0;
-        int acc = 0;
-        uint32_t acc_phase = 0;
         if constexpr (BS) {
-            if (first_pair < total_items) {
-                mbar_wait(bfull, 0u);
-                tc_fence_after();
-            }
+            if (first_pair < total_items) mbar_wait(bfull, 0u);
         }
-        for (int wi = first_pair; wi < total_items; wi += pair_stride) {
-            const int it0s = BS ? 0 : (wi % nsplit) * k_per;
-            const int k_iters = min(k_total, it0s + k_per) - it0s;
-            TRACE(2);
-            mbar_wait(&tempty[acc], acc_phase ^ 1u);      // epilogue(s) have drained this accumulator stage
-            TRACE(3);
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(acc * 256);
-            auto issue_stage = [&](int st, int it) {
-                const bool skip_mma = (g.flags & GEMM_DBG_NO_MMA) != 0;
-                const uint32_t sa = smem_u32(BS ? sA_ring + st * kABytes : smem + st * C::kStageBytes);
-                const uint64_t da = umma_desc_k_sw128(sa);
-                const uint64_t db = umma_desc_k_sw128(BS ? smem_u32(sB_res + it * C::kBBytes) : sa + kABytes);
-#pragma unroll
-                for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
-                    if (skip_mma) break;
-                    // +32 B per K=16 step: start-address field is in 16 B units
-                    if constexpr (CG == 2)
-                        umma_f16_2sm(tmem_d, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), idesc,
-                                     (it | k) != 0 ? 1u : 0u);
-                    else
-                        umma_f16(tmem_d, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), idesc,
-                                 (it | k) != 0 ? 1u : 0u);
-                }
-                if constexpr (CG == 2) {
-                    umma_commit_2sm(&empty[st]);                          // frees the stage in BOTH CTAs
-                    if (it == k_iters - 1) umma_commit_2sm(&tfull[acc]);  // both epilogues may drain their half
-                } else {
-                    umma_commit(&empty[st]);                          // smem stage reusable once these MMAs retire
-                    if (it == k_iters - 1) umma_commit(&tfull[acc]);  // accumulator complete
-                }
-                TRACE(14);
-            };
-#if T2V_MMA_UNROLL2
-            // two ring stages per loop trip: one wait / fence / loop-around per 8 MMAs instead of per 4
-            for (int it = 0; it < k_iters; it += 2) {
-                const bool two = it + 1 < k_iters;
-                const bool wrap = stage + 1 == nst;
-                const int st2 = wrap ? 0 : stage + 1;
-                mbar_wait(&full[stage], phase);
-                if (two) mbar_wait(&full[st2], wrap ? phase ^ 1u : phase);
-                TRACE(4);
-                tc_fence_after();
-                issue_stage(stage, it);
-                if (two) issue_stage(st2, it + 1);
-                for (int a = 0; a < (two ? 2 : 1); ++a)
-                    if (++stage == nst) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-            }
-#else
-            for (int it = 0; it < k_iters; ++it) {
-                mbar_wait(&full[stage], phase);
-                TRACE(4);
-                tc_fence_after();
-                issue_stage(stage, it);
-                if (++stage == nst) {
-                    stage = 0;
-                    phase ^= 1u;
-                }
-            }
-#endif
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1u;
-        }
-        }   // leader's elected thread
-        __syncwarp();
-    } else {
-        // ------------------------------------------------------------------ epilogue (warps 2..9)
-        // 8 warps: TMEM lane quadrant q = warp & 3 (a warp may only touch lanes 32q..32q+31), column chunks are
-        // interleaved between the two warps of a quadrant.  Per chunk the residual row segment is prefetched one
-        // chunk ahead so that HBM/L2 latency overlaps the previous chunk's math and stores.
-        const int q = warp & 3;
-        const int hsel = (warp - 2) >> 2;              // which share of the chunks this warp handles (EW/4 warps per quadrant)
-        constexpr int CSTEP = EW / 4;
-        const int r = q * 32 + lane;                   // row of the tile held by this thread
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        constexpr bool geglu = GEGLU;
         const bool out_f32 = (g.flags & GEMM_OUT_F32) != 0;
-        constexpr int CW = (BN >= 32 && (!GEGLU || EW == 8)) ? 32 : 16;        // columns per tcgen05.ld
-        constexpr int NV = CW / 8;                     // 16-byte vectors per chunk row segment
-        const int ncols_tile = geglu ? BN / 2 : BN;
-        const int nchunks = ncols_tile / CW;
-        const int nvalid = geglu ? g.N / 2 : g.N;
-        const bool vec_ok = ((g.ldo & 7) == 0) && ((g.N & 7) == 0) && (!geglu || (g.N & 15) == 0) &&
-                            (g.residual == nullptr || (g.ldr & 7) == 0);
-        // 32-byte (one full sector per thread) stores / residual loads when every row segment is 32 B aligned
-        const bool vec32 = vec_ok && !out_f32 && ((g.ldo & 15) == 0) && ((nvalid & 15) == 0) &&
-                           ((reinterpret_cast<uintptr_t>(g.out) & 31) == 0) &&
-                           (g.residual == nullptr || (((g.ldr & 15) == 0) && ((reinterpret_cast<uintptr_t>(g.residual) & 31) == 0)));
-        // A bias shared by all rows is staged once per tile in smem (its L2 latency hides behind the wait for the
-        // accumulator); per-sample bias rows (time-embedding add of the ResBlock convs) are read per thread.
         const bool ln = (g.flags & GEMM_LN) != 0;
-        const bool tma_st = !GEGLU && (g.flags & GEMM_TMA_STORE) != 0 && EW == 8;
-        const uint32_t my_stage0 = smem_u32(stage_s) + static_cast<uint32_t>(warp - 2) * 2048u;
-        uint32_t stage_bank = 0;                       // kStage2: alternates between the two staging banks (16 KB apart)
-        const bool bias_staged = GEGLU || ln || ((g.bias != nullptr) && (g.bias_rows == 0));   // GEGLU: always (zeros if no bias)
-        const int et = static_cast<int>(threadIdx.x) - 64;       // 0..255 among the epilogue threads
-        TRACE_DECL(lane == 0 ? (warp == 2 ? 2 : (warp == 6 ? 3 : -1)) : -1);
+        const int nvalid = GEGLU ? g.N / 2 : g.N;
+        // column pairs as one 4 / 8-byte access when every row segment starts at an even element
+        const bool pair_ok = ((g.ldo & 1) == 0) && ((reinterpret_cast<uintptr_t>(g.out) & (out_f32 ? 7 : 3)) == 0) &&
+                             ((g.split_stride & 1) == 0) &&
+                             (g.residual == nullptr || (((g.ldr & 1) == 0) && ((reinterpret_cast<uintptr_t>(g.residual) & 3) == 0)));
+        float acc[BN / 2];
         for (int wi = first_pair; wi < total_items; wi += pair_stride) {
             const int sp = BS ? 0 : wi % nsplit;
             const int pt = wi / nsplit;
             const int tn = BS ? bs_tn : pt % g.tiles_n;
             const int tmi = BS ? wi : (pt / g.tiles_n) * CG + static_cast<int>(rank);
-            int tm = tmi;
-            // tile row r -> global row
-            long long grow = 0;
-            long long mul = 1;
-            bool valid = tmi < g.tiles_m;
-            int torg[GEMM_MAX_RDIMS] = {0, 0, 0, 0};   // tile origin in the row grid (TMA-store coordinates)
-            if (g.nd == 1) {                           // plain row matrix: no div/mod chain (16 integer divisions per tile otherwise)
-                const int o = tmi * g.box[0];
-                torg[0] = o;
-                valid = valid && (r < g.box[0]) && (o + r < g.dim[0]);
-                grow = o + r;
-            } else {
-                int rr = r;
+            const int it0s = BS ? 0 : sp * k_per;
+            const int k_iters = min(k_total, it0s + k_per) - it0s;
+
+            // ---- main loop: one ring stage per iteration, one wgmma group kept in flight
+            int prev = -1;
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);       // the previous tile's epilogue reads stay before the MMAs
+            for (int it = 0; it < k_iters; ++it) {
+                mbar_wait(&full[stage], phase);
+                const uint32_t sa = smem_u32(BS ? sA_ring + stage * kABytes : smem + stage * Cf::kStageBytes) + cw * (64 * 128);
+                const uint32_t sb = BS ? smem_u32(sB_res + it * Cf::kBBytes) : smem_u32(smem + stage * Cf::kStageBytes) + kABytes;
+                const uint64_t da = wgmma_desc_sw128(sa);
+                const uint64_t db = wgmma_desc_sw128(sb);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < GEMM_BLOCK_K / 16; ++k)          // +32 B per K = 16 step (start address in 16 B units)
+                    mma_k16<BN>(acc, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), (it | k) != 0 ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<1>();                                      // the previous stage's group has retired
+                if (prev >= 0 && lt == 0) {
+                    mbar_arrive(&empty[prev]);
+                    if constexpr (CG == 2) mbar_arrive_cluster(&empty[prev], rank ^ 1u);
+                }
+                prev = stage;
+                if (++stage == nst) {
+                    stage = 0;
+                    phase ^= 1u;
+                }
+            }
+            wgmma_wait<0>();
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);       // epilogue reads stay behind the wait
+            if (prev >= 0 && lt == 0) {
+                mbar_arrive(&empty[prev]);
+                if constexpr (CG == 2) mbar_arrive_cluster(&empty[prev], rank ^ 1u);
+            }
+
+            // ---- epilogue: this thread holds rows r0, r0 + 8 and, per 8-column group j, columns 8j + 2 quad + {0, 1}
+            const int r0 = cw * 64 + wr * 16 + (lane >> 2);
+            int tm_org[GEMM_MAX_RDIMS] = {0, 0, 0, 0};
+            if (g.nd > 1) {
+                int tm = tmi;
 #pragma unroll
                 for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
                     const int td = g.tdim[d];
-                    const int o = (tm % td) * g.box[d];
-                    torg[d] = o;
+                    tm_org[d] = (tm % td) * g.box[d];
                     tm /= td;
-                    const int i = rr % g.box[d];
-                    rr /= g.box[d];
-                    const int c = o + i;
-                    valid = valid && (c < g.dim[d]);
-                    grow += mul * c;
-                    mul *= g.dim[d];
                 }
-                valid = valid && (rr == 0);
             }
-            const __half* bias = g.bias;
-            if (bias != nullptr && g.bias_rows > 0) bias += (grow / g.bias_rows) * g.bias_stride;
-            const int ocol0 = geglu ? tn * (BN / 2) : tn * BN;
-            const __half* res_row = (g.residual != nullptr && valid) ? g.residual + grow * g.ldr + ocol0 : nullptr;
-
-            // Residual row segments are fetched kResDepth chunks ahead into a register queue (static indices only).  The timeline
-            // (profiles/r02_gemm_timeline.md) showed ~1000 clk of exposed fetch latency per chunk with one chunk of look-ahead issued
-            // after the previous chunk's store; with depth 3 a 160-wide tile (3 + 2 chunks per warp pair) has its whole residual in
-            // flight while the warp still waits for the accumulator, and no generic load is outstanding at the chunk's fence.
-            // (wider tiles keep depth 1: their epilogue has no registers to spare -- 224 / 256 spilled and the residual-free layers
-            //  lost 5-12 % with the queue compiled in; A/B in profiles/r02_gemm_residual_depth_ab.txt: out-projection 34.8 -> 31.3 us)
-            constexpr int kResDepth = (GEGLU || BN > 160) ? 1 : T2V_RES_DEPTH;
-            uint4 rq[kResDepth][NV];
-            auto load_res = [&](uint4 (&dst)[NV], int ci) {
-                if (res_row != nullptr && vec_ok) {
-                    if (vec32) {
 #pragma unroll
-                        for (int k = 0; k < NV; k += 2) {
-                            const int col = ci * CW + k * 8;
-                            if (ocol0 + col < nvalid) {
-                                const U32x8 t8 = ldg_256(res_row + col);
-                                dst[k] = make_uint4(t8.v[0], t8.v[1], t8.v[2], t8.v[3]);
-                                dst[k + 1] = make_uint4(t8.v[4], t8.v[5], t8.v[6], t8.v[7]);
-                            }
-                        }
-                    } else {
-#pragma unroll
-                        for (int k = 0; k < NV; ++k) {
-                            const int col = ci * CW + k * 8;
-                            if (ocol0 + col < nvalid) dst[k] = __ldg(reinterpret_cast<const uint4*>(res_row + col));
-                        }
-                    }
-                }
-            };
-            if constexpr (!GEGLU) {
-#pragma unroll
-                for (int d = 0; d < kResDepth; ++d)
-                    if (hsel + d * CSTEP < nchunks) load_res(rq[d], hsel + d * CSTEP);
-            }
-            float bstage = 0.f, cstage = 0.f;
-            if (bias_staged && et < BN) {
-                const int col = tn * BN + et;
-                if (col < g.N) {
-                    if (ln) {
-                        bstage = __ldg(g.bias32 + col);
-                        cstage = __ldg(g.colsum + col);
-                    } else if (g.bias != nullptr) {
-                        bstage = __half2float(__ldg(g.bias + col));
-                    }
-                }
-            }
-            float2 rs = make_float2(0.f, 1.f);                    // (mean, rstd) of this thread's row
-            if (ln && valid) rs = __ldg(g.rowstat + grow);
-
-            TRACE(5);
-            mbar_wait(&tfull[acc], acc_phase);
-            TRACE(6);
-            tc_fence_after();
-            const float* bs = bias_s + acc * 256;
-            const float* cs = csum_s + acc * 256;
-            if (bias_staged) {
-                if (et < BN) {
-                    bias_s[acc * 256 + et] = bstage;
-                    if (ln) csum_s[acc * 256 + et] = cstage;
-                }
-                asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");     // epilogue warps only (named barrier 1)
-            }
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * 256);
-            constexpr bool kPipe = !GEGLU && T2V_EPI_PIPE != 0;
-            uint32_t un[CW];                           // kPipe: accumulator chunk in flight (loaded one iteration ahead)
-            if constexpr (kPipe) {
-                if (hsel < nchunks && !(g.flags & GEMM_DBG_NO_EPI)) {
-                    if constexpr (CW == 32) tmem_ld_32x32(taddr + hsel * CW, un);
-                    else tmem_ld_32x16(taddr + hsel * CW, un);
-                }
-            }
-            for (int ci = hsel; ci < nchunks; ci += CSTEP) {
-                if (g.flags & GEMM_DBG_NO_EPI) break;
-                const int c0 = ci * CW;
-                uint32_t u[CW];
-                uint32_t ug[CW];
-                if constexpr (kPipe) {
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < CW; ++j) u[j] = un[j];
-                    if (ci + CSTEP < nchunks) {
-                        if constexpr (CW == 32) tmem_ld_32x32(taddr + (ci + CSTEP) * CW, un);
-                        else tmem_ld_32x16(taddr + (ci + CSTEP) * CW, un);
-                    }
+            for (int h = 0; h < 2; ++h) {
+                const int r = r0 + 8 * h;
+                long long grow = 0;
+                bool valid = tmi < g.tiles_m;
+                if (g.nd == 1) {                       // plain row matrix: no div/mod chain
+                    const int o = tmi * g.box[0];
+                    valid = valid && (r < g.box[0]) && (o + r < g.dim[0]);
+                    grow = o + r;
                 } else {
-                    if constexpr (CW == 32) tmem_ld_32x32(taddr + c0, u);
-                    else tmem_ld_32x16(taddr + c0, u);
-                }
-                if (geglu) {
-                    if constexpr (CW == 32) tmem_ld_32x32(taddr + BN / 2 + c0, ug);
-                    else tmem_ld_32x16(taddr + BN / 2 + c0, ug);
-                }
-                if constexpr (GEGLU) {
-                    // GEGLU tile: out = fp16(value) * fp16(gelu(fp16(gate))) with the reference's fp16 rounding points
-                    // (t2v_model.py:819-821 under autocast: proj output, gelu output, product).  Bias / LayerNorm-fold
-                    // vectors come from the staged smem tile, no residual, 32 B aligned fp16 rows (gemm_plan checks).
-                    tmem_ld_wait();
-                    TRACE(7);
-                    uint32_t ow[CW / 2];
+                    int rr = r;
+                    long long mul = 1;
 #pragma unroll
-                    for (int j = 0; j < CW; j += 2) {
-                        const float2 bx = *reinterpret_cast<const float2*>(bs + c0 + j);
-                        const float2 bgt = *reinterpret_cast<const float2*>(bs + BN / 2 + c0 + j);
-                        float x0, x1, g0, g1;
-                        if (ln) {
-                            const float2 cx = *reinterpret_cast<const float2*>(cs + c0 + j);
-                            const float2 cg = *reinterpret_cast<const float2*>(cs + BN / 2 + c0 + j);
-                            x0 = fmaf(rs.y, fmaf(-rs.x, cx.x, __uint_as_float(u[j])), bx.x);
-                            x1 = fmaf(rs.y, fmaf(-rs.x, cx.y, __uint_as_float(u[j + 1])), bx.y);
-                            g0 = fmaf(rs.y, fmaf(-rs.x, cg.x, __uint_as_float(ug[j])), bgt.x);
-                            g1 = fmaf(rs.y, fmaf(-rs.x, cg.y, __uint_as_float(ug[j + 1])), bgt.y);
-                        } else {
-                            x0 = fmaf(__uint_as_float(u[j]), g.alpha, bx.x);
-                            x1 = fmaf(__uint_as_float(u[j + 1]), g.alpha, bx.y);
-                            g0 = fmaf(__uint_as_float(ug[j]), g.alpha, bgt.x);
-                            g1 = fmaf(__uint_as_float(ug[j + 1]), g.alpha, bgt.y);
-                        }
+                    for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
+                        const int i = rr % g.box[d];
+                        rr /= g.box[d];
+                        const int c = tm_org[d] + i;
+                        valid = valid && (c < g.dim[d]);
+                        grow += mul * c;
+                        mul *= g.dim[d];
+                    }
+                    valid = valid && (rr == 0);
+                }
+                if (!valid) continue;
+                const __half* bias = g.bias;
+                if (bias != nullptr && g.bias_rows > 0) bias += (grow / g.bias_rows) * g.bias_stride;
+                float2 rs = make_float2(0.f, 1.f);                    // (mean, rstd) of this row
+                if (ln) rs = __ldg(g.rowstat + grow);
+                // accumulator -> alpha / LayerNorm fold -> + bias, for packed column pcol
+                auto affine = [&](float v, int pcol) {
+                    if (ln) return fmaf(rs.y, fmaf(-rs.x, __ldg(g.colsum + pcol), v), __ldg(g.bias32 + pcol));
+                    return fmaf(v, g.alpha, bias != nullptr ? __half2float(__ldg(bias + pcol)) : 0.f);
+                };
+                if constexpr (GEGLU) {
+                    // out = fp16(value) * fp16(gelu(fp16(gate))) with the reference's fp16 rounding points (t2v_model.py:819-821
+                    // under autocast: proj output, gelu output, product).  Value column c and gate column BN/2 + c of the tile
+                    // sit BN/4 registers apart; gemm_plan guarantees N % BN == 0 and 32 B aligned fp16 rows.
+                    __half* orow = reinterpret_cast<__half*>(g.out) + grow * g.ldo + tn * (BN / 2);
+#pragma unroll
+                    for (int j = 0; j < BN / 16; ++j) {
+                        const int c = 8 * j + 2 * quad;
+                        const int pc = tn * BN + c;
+                        const float x0 = affine(acc[4 * j + 2 * h], pc), x1 = affine(acc[4 * j + 2 * h + 1], pc + 1);
+                        const float g0 = affine(acc[BN / 4 + 4 * j + 2 * h], pc + BN / 2);
+                        const float g1 = affine(acc[BN / 4 + 4 * j + 2 * h + 1], pc + BN / 2 + 1);
                         const __half2 xh = __floats2half2_rn(x0, x1);
                         const float2 gf = __half22float2(__floats2half2_rn(g0, g1));
                         const __half2 ge = __floats2half2_rn(gelu_erf(gf.x), gelu_erf(gf.y));
-                        const __half2 oh = __hmul2(xh, ge);            // fp16 x fp16 -> fp16 (RN) == the reference's product
-                        ow[j >> 1] = *reinterpret_cast<const uint32_t*>(&oh);
-                    }
-                    if (valid && !(g.flags & GEMM_DBG_NO_STORE)) {
-                        __half* op = reinterpret_cast<__half*>(g.out) + grow * g.ldo + ocol0 + c0;
-#pragma unroll
-                        for (int k = 0; k < CW / 16; ++k) {
-                            U32x8 ov;
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) ov.v[e] = ow[k * 8 + e];
-                            stg_256(op + k * 16, ov);
-                        }
+                        *reinterpret_cast<__half2*>(orow + c) = __hmul2(xh, ge);     // fp16 x fp16 -> fp16 (RN)
                     }
                 } else {
-                uint4 rcur[NV];
+                    const int ocol0 = tn * BN;
+                    const __half* res_row = g.residual != nullptr ? g.residual + grow * g.ldr + ocol0 : nullptr;
 #pragma unroll
-                for (int k = 0; k < NV; ++k) rcur[k] = rq[0][k];
-#pragma unroll
-                for (int d = 0; d + 1 < kResDepth; ++d)
-#pragma unroll
-                    for (int k = 0; k < NV; ++k) rq[d][k] = rq[d + 1][k];
-                // ncu (profiles/r02_ncu_gemm_k320.md): fence.proxy.async in the TMA-store path waits for EVERY outstanding generic
-                // memory operation of the thread, so a residual prefetch issued here is paid in full at the fence of this very
-                // chunk (long-scoreboard stall on FENCE.VIEW.ASYNC).  On that path the prefetch of the next chunk is issued
-                // after this chunk's store instead (T2V_RES_LATE); it then overlaps the next chunk's TMEM load.
-                constexpr bool kResLate = T2V_RES_LATE != 0;
-                if (!(kResLate && tma_st) && ci + kResDepth * CSTEP < nchunks) load_res(rq[kResDepth - 1], ci + kResDepth * CSTEP);
-                const int pcol = tn * BN + c0;                    // packed (accumulator) column of v[0]
-                float bv[CW];
-                if (bias_staged) {
-#pragma unroll
-                    for (int j = 0; j < CW; j += 4) {
-                        const float4 t4 = *reinterpret_cast<const float4*>(bs + c0 + j);       // smem broadcast
-                        bv[j] = t4.x; bv[j + 1] = t4.y; bv[j + 2] = t4.z; bv[j + 3] = t4.w;
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < CW; ++j) {
-                        bv[j] = (bias != nullptr && pcol + j < g.N) ? __half2float(__ldg(bias + pcol + j)) : 0.f;
-                    }
-                }
-                if constexpr (!kPipe) tmem_ld_wait();
-                TRACE(7);
-                float v[CW];
-                if (ln) {
-#pragma unroll
-                    for (int j = 0; j < CW; ++j) v[j] = fmaf(rs.y, fmaf(-rs.x, cs[c0 + j], __uint_as_float(u[j])), bv[j]);
-                } else {
-#pragma unroll
-                    for (int j = 0; j < CW; ++j) v[j] = fmaf(__uint_as_float(u[j]), g.alpha, bv[j]);
-                }
-                const int ocol = ocol0 + c0;
-                if (tma_st) {
-                    // ---- TMA-store path: residual add, fp16 pack, swizzled smem staging, one bulk tensor store per chunk.
-                    //      Row-per-thread global stores cost one L1 wavefront per 32 B; the bulk copy writes full lines.
-                    if (res_row != nullptr) {
-#pragma unroll
-                        for (int k = 0; k < NV; ++k) {
-                            if (ocol + k * 8 < nvalid) {
-                                const __half2* h2 = reinterpret_cast<const __half2*>(&rcur[k]);
-#pragma unroll
-                                for (int e = 0; e < 4; ++e) {
-                                    const float2 f = __half22float2(h2[e]);
-                                    v[k * 8 + 2 * e] += f.x;
-                                    v[k * 8 + 2 * e + 1] += f.y;
-                                }
+                    for (int j = 0; j < BN / 8; ++j) {
+                        const int c = 8 * j + 2 * quad;
+                        const int col = ocol0 + c;
+                        if (col >= nvalid) continue;
+                        const bool two = col + 1 < nvalid;
+                        float v0 = affine(acc[4 * j + 2 * h], col);
+                        float v1 = two ? affine(acc[4 * j + 2 * h + 1], col + 1) : 0.f;
+                        if (res_row != nullptr) {
+                            if (two && pair_ok) {
+                                const float2 f = __half22float2(__ldg(reinterpret_cast<const __half2*>(res_row + c)));
+                                v0 += f.x;
+                                v1 += f.y;
+                            } else {
+                                v0 += __half2float(res_row[c]);
+                                if (two) v1 += __half2float(res_row[c + 1]);
                             }
                         }
-                    }
-                    const uint32_t my_stage = my_stage0 + (kStage2 ? stage_bank * 16384u : 0u);
-                    // bulk async-groups belong to the committing THREAD: issue, commit and wait all sit behind elect.sync (same
-                    // membermask -> same lane every time), which also keeps the UTMASTG free of a waterfall loop
-                    if constexpr (kStage2) {
-                        if (elect_one()) bulk_wait_read1();        // the store before the previous one has finished READING this bank
-                        stage_bank ^= 1u;
-                    } else {
-                        if (elect_one()) bulk_wait_read0();        // the previous chunk's store has finished READING the buffer
-                    }
-                    TRACE(8);
-                    __syncwarp();
-                    const uint32_t rowb = my_stage + static_cast<uint32_t>(lane) * 64u;
-                    const int sw = (lane >> 1) & 3;                // SWIZZLE_64B: 16-byte chunk ^= address bits [7,9)
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        uint32_t w4[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const __half2 hh = __floats2half2_rn(v[k * 8 + 2 * e], v[k * 8 + 2 * e + 1]);
-                            w4[e] = *reinterpret_cast<const uint32_t*>(&hh);
-                        }
-                        sts_128(rowb + static_cast<uint32_t>((k ^ sw) << 4), w4[0], w4[1], w4[2], w4[3]);
-                    }
-                    fence_proxy_async();
-                    TRACE(9);
-                    __syncwarp();
-                    if (!(g.flags & GEMM_DBG_NO_STORE) && tmi < g.tiles_m && elect_one()) {
-                        const int c1 = torg[0] + g.st_off[q][0], c2 = torg[1] + g.st_off[q][1];
-                        const int c3 = torg[2] + g.st_off[q][2], c4 = torg[3] + g.st_off[q][3];
-                        switch (g.nd) {
-                            case 1: tma_store_2d(&g.map_out, my_stage, ocol, c1); break;
-                            case 2: tma_store_3d(&g.map_out, my_stage, ocol, c1, c2); break;
-                            case 3: tma_store_4d(&g.map_out, my_stage, ocol, c1, c2, c3); break;
-                            default: tma_store_5d(&g.map_out, my_stage, ocol, c1, c2, c3, c4); break;
-                        }
-                        bulk_commit();
-                    }
-                    if (kResLate && ci + kResDepth * CSTEP < nchunks) load_res(rq[kResDepth - 1], ci + kResDepth * CSTEP);
-                } else
-                if (valid && !(g.flags & GEMM_DBG_NO_STORE)) {
-                    if (res_row != nullptr) {
-                        if (vec_ok) {
-#pragma unroll
-                            for (int k = 0; k < NV; ++k) {
-                                if (ocol + k * 8 < nvalid) {
-                                    const __half2* h2 = reinterpret_cast<const __half2*>(&rcur[k]);
-#pragma unroll
-                                    for (int e = 0; e < 4; ++e) {
-                                        const float2 f = __half22float2(h2[e]);
-                                        v[k * 8 + 2 * e] += f.x;
-                                        v[k * 8 + 2 * e + 1] += f.y;
-                                    }
-                                }
+                        if (out_f32) {
+                            float* op = reinterpret_cast<float*>(g.out) + sp * g.split_stride + grow * g.ldo + col;
+                            if (two && pair_ok) {
+                                *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+                            } else {
+                                op[0] = v0;
+                                if (two) op[1] = v1;
                             }
                         } else {
-#pragma unroll
-                            for (int j = 0; j < CW; ++j)
-                                if (ocol + j < nvalid) v[j] += __half2float(res_row[c0 + j]);
-                        }
-                    }
-                    if (out_f32) {
-                        float* op = reinterpret_cast<float*>(g.out) + sp * g.split_stride + grow * g.ldo + ocol;
-                        if (((g.ldo & 7) == 0) && ((nvalid & 7) == 0) && ((g.split_stride & 7) == 0) &&
-                            ((reinterpret_cast<uintptr_t>(g.out) & 31) == 0)) {
-#pragma unroll
-                            for (int j = 0; j < CW; j += 8) {
-                                if (ocol + j < nvalid) {
-                                    U32x8 ov;
-#pragma unroll
-                                    for (int e = 0; e < 8; ++e) ov.v[e] = __float_as_uint(v[j + e]);
-                                    stg_256(op + j, ov);
-                                }
+                            __half* op = reinterpret_cast<__half*>(g.out) + grow * g.ldo + col;
+                            if (two && pair_ok) {
+                                *reinterpret_cast<__half2*>(op) = __floats2half2_rn(v0, v1);
+                            } else {
+                                op[0] = __float2half_rn(v0);
+                                if (two) op[1] = __float2half_rn(v1);
                             }
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < CW; ++j)
-                                if (ocol + j < nvalid) op[j] = v[j];
-                        }
-                    } else {
-                        __half* op = reinterpret_cast<__half*>(g.out) + grow * g.ldo + ocol;
-                        if (vec32) {
-#pragma unroll
-                            for (int k = 0; k < NV; k += 2) {
-                                if (ocol + k * 8 < nvalid) {
-                                    U32x8 ov;
-#pragma unroll
-                                    for (int e = 0; e < 8; ++e) {
-                                        const __half2 hh = __floats2half2_rn(v[k * 8 + 2 * e], v[k * 8 + 2 * e + 1]);
-                                        ov.v[e] = *reinterpret_cast<const uint32_t*>(&hh);
-                                    }
-                                    stg_256(op + k * 8, ov);
-                                }
-                            }
-                        } else if (vec_ok) {
-#pragma unroll
-                            for (int k = 0; k < NV; ++k) {
-                                if (ocol + k * 8 < nvalid) {
-                                    uint4 ov;
-                                    __half2* h2 = reinterpret_cast<__half2*>(&ov);
-#pragma unroll
-                                    for (int e = 0; e < 4; ++e) h2[e] = __floats2half2_rn(v[k * 8 + 2 * e], v[k * 8 + 2 * e + 1]);
-                                    *reinterpret_cast<uint4*>(op + k * 8) = ov;
-                                }
-                            }
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < CW; ++j)
-                                if (ocol + j < nvalid) op[j] = __float2half_rn(v[j]);
                         }
                     }
                 }
-                }   // !GEGLU
             }
-            tc_fence_before();
-            __syncwarp();
-            TRACE(10);
-            if (lane == 0) {
-                if (CG == 2 && !leader) mbar_arrive_cluster(&tempty[acc], 0);   // the MMA issuer lives in the leader CTA
-                else mbar_arrive(&tempty[acc]);
-            }
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1u;
         }
     }
-
-    if (warp >= 2) {
-        if (elect_one()) bulk_wait0();            // TMA stores issued by this (elected) thread have left the staging buffer
-    }
-    tc_fence_before();
-    if constexpr (CG == 2) cluster_sync_all();    // no CTA may exit (or free TMEM) while its peer can still signal it
-    else __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        if constexpr (CG == 2) tmem_dealloc_2sm(tmem_base, 512);
-        else tmem_dealloc(tmem_base, 512);
-    }
+    if constexpr (CG == 2) cluster_sync_all();    // no CTA may exit while its peer can still multicast into it or signal it
 }
 
 // ------------------------------------------------------------------------------------------ host side
@@ -797,7 +402,7 @@ int encode_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dim
                           dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
-        fprintf(stderr, "[t2v_b200] cuTensorMapEncodeTiled failed: %d (rank %d, dims %llu %llu %llu %llu %llu)\n",
+        fprintf(stderr, "[t2v] cuTensorMapEncodeTiled failed: %d (rank %d, dims %llu %llu %llu %llu %llu)\n",
                 static_cast<int>(r), rank, (unsigned long long)dims[0], (unsigned long long)(rank > 1 ? dims[1] : 0),
                 (unsigned long long)(rank > 2 ? dims[2] : 0), (unsigned long long)(rank > 3 ? dims[3] : 0),
                 (unsigned long long)(rank > 4 ? dims[4] : 0));
@@ -812,10 +417,9 @@ struct Variant {
     const void* fn;
     int bs;
 };
-constexpr int kBsSmemBytes = kBsRing + 1024 + 256 + 4096 + 256 + 8 * 2048 * (T2V_EPI_STAGE2 ? 2 : 1);   // Cfg's map, ring at its budget
 template <int BN, bool G, int CG>
 Variant variant() {
-    return Variant{BN, G ? 1 : 0, CG, Cfg<BN, CG>::kSmemBytes, reinterpret_cast<const void*>(&gemm_tc_kernel<BN, G, CG>), 0};
+    return Variant{BN, G ? 1 : 0, CG, Cfg<BN>::kSmemBytes, reinterpret_cast<const void*>(&gemm_tc_kernel<BN, G, CG>), 0};
 }
 template <int BN, bool G>
 Variant variant_bs() {
@@ -849,7 +453,7 @@ int gemm_init() {
     cudaDriverEntryPointQueryResult qres;
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess ||
         fn == nullptr) {
-        fprintf(stderr, "[t2v_b200] cuTensorMapEncodeTiled entry point not found\n");
+        fprintf(stderr, "[t2v] cuTensorMapEncodeTiled entry point not found\n");
         return -1;
     }
     g_encode = reinterpret_cast<EncodeTiledFn>(fn);
@@ -859,7 +463,7 @@ int gemm_init() {
     for (int i = 0; i < nv; ++i)
         if (cudaFuncSetAttribute(vs[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, vs[i].smem) != cudaSuccess) attr_fail = true;
     if (attr_fail) {
-        fprintf(stderr, "[t2v_b200] cudaFuncSetAttribute(max dynamic smem) failed: %s\n",
+        fprintf(stderr, "[t2v] cudaFuncSetAttribute(max dynamic smem) failed: %s\n",
                 cudaGetErrorString(cudaGetLastError()));
         return -1;
     }
@@ -882,9 +486,8 @@ int tma_encode_f16(CUtensorMap* m, const void* base, int rank, const unsigned lo
 
 int gemm_bs_bn(long long tiles_m, int N, int K, int ntaps, bool geglu, int num_sms, int force_bn, bool any_k, int* stages_out) {
     static const bool bs_off = getenv("T2V_NO_BSTAT") != nullptr;
-    // measured on B200 (profiles/r02_gemm_epilogue_ab.txt): bit-identical results, no gain on the K = 320 layers (33.5 vs 33.6 us
-    // +res, 23.2 vs 24.4 us without) nor on the forward (23.27 vs 23.35 ms) -- those layers are not bound by the operand stream
-    // after all.  Kept as an opt-in (T2V_BSTAT_KMAX=<max K chunks>, e.g. 5) and for the op-level tests (GEMM_DBG_FORCE_BS).
+    // Off by default (not measured faster on the model's layers); opt-in with T2V_BSTAT_KMAX=<max K chunks>, e.g. 5, and taken
+    // by the op-level tests (GEMM_DBG_FORCE_BS).
     static const int bs_kmax = getenv("T2V_BSTAT_KMAX") ? atoi(getenv("T2V_BSTAT_KMAX")) : 0;
     const int kt = ntaps * ((K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K);
     if (bs_off || N <= 16 || (kt > bs_kmax && !any_k)) return 0;
@@ -896,10 +499,9 @@ int gemm_bs_bn(long long tiles_m, int N, int K, int ntaps, bool geglu, int num_s
         const int tn = (N + c - 1) / c;
         if (static_cast<double>(N) / (static_cast<double>(tn) * c) < 0.9) continue;
         const long long b_bytes = static_cast<long long>(kt) * c * GEMM_BLOCK_K * 2;
-        if (geglu) continue;      // measured: the GEGLU epilogue (MUFU / issue bound) gains nothing from resident weights and loses
-                                  // with the 128-wide tiles they need (512 vs 678 TFLOP/s on the level-0 feed-forward)
-        if (b_bytes > kBsRing - 4 * kABytes || tn > num_sms) continue;
-        const int stages = static_cast<int>(std::min<long long>(8, (kBsRing - b_bytes) / kABytes));
+        if (geglu) continue;      // the GEGLU epilogue gains nothing from resident weights and loses with the 128-wide tiles they need
+        if (b_bytes > kSmemBudget - 4 * kABytes || tn > num_sms) continue;
+        const int stages = static_cast<int>(std::min<long long>(8, (kSmemBudget - b_bytes) / kABytes));
         const int group = num_sms / tn;                               // CTAs per N-tile
         if (tiles_m < 3LL * group) continue;                          // too few M-tiles per CTA to amortise the resident load
         if (stages_out) *stages_out = stages;
@@ -913,7 +515,7 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
     if (p.nd < 1 || p.nd > GEMM_MAX_RDIMS || p.ntaps < 1 || p.ntaps > GEMM_MAX_TAPS) return -2;
     if ((p.lda & 7) != 0 || (p.K & 7) != 0 || (reinterpret_cast<uintptr_t>(p.a) & 15) != 0 ||
         (reinterpret_cast<uintptr_t>(p.b) & 15) != 0) {
-        fprintf(stderr, "[t2v_b200] gemm_plan: operands must be 16-byte aligned (lda %lld K %d)\n", p.lda, p.K);
+        fprintf(stderr, "[t2v] gemm_plan: operands must be 16-byte aligned (lda %lld K %d)\n", p.lda, p.K);
         return -3;
     }
     GemmDesc& g = plan->desc;
@@ -971,18 +573,14 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
     g.splits = p.splits > 1 ? p.splits : 1;
     g.split_stride = p.split_stride;
 
-    // ---- N tiling: the tile width with the shortest modelled kernel time.  The in-kernel timeline (profiles/r02_gemm_timeline.md)
-    // shows a K step costing the issuing threads ~600 clk whatever the tile width (the tensor pipe itself needs 2 clk per
-    // column: 512 clk at BN = 256), and a tile's epilogue ~1000 clk per 32-column chunk per warp (2 warps share a quadrant's
-    // chunks; twice that with a residual to fetch).  A persistent CTA walks ceil(tiles / CTAs) tiles whose MMA and epilogue
-    // overlap (double-buffered accumulator), plus one exposed epilogue at the end.  So: as few K steps per CTA as possible --
+    // ---- N tiling: the tile width with the shortest modelled kernel time.  A persistent CTA walks ceil(tiles / CTAs) tiles
+    // whose main loop (K steps) and epilogue add up, plus the fill of the last wave.  So: as few K steps per CTA as possible --
     // wide tiles, even slightly padded ones (N = 1920 -> 9 x 224 instead of 12 x 160), unless the epilogue is the longer leg.
     int bn = p.force_bn;
     const int k_total_sel = p.ntaps * g.k_chunks;
     static const int model_min_k = getenv("T2V_BN_MODEL_MINK") ? atoi(getenv("T2V_BN_MODEL_MINK")) : 10;      // A/B switch
     if (bn == 0 && k_total_sel >= model_min_k) {
-        // K-heavy tiles (>= 10 K steps): the MMA leg dominates -> time model, padded wide tiles allowed.  Measured (B200,
-        // profiles/r02_gemm_tile_widths.txt): N = 1920, K = 640: 12 x 160 -> 9 x 224 columns 34.7 -> 30.2 us.
+        // K-heavy tiles (>= 10 K steps): the MMA leg dominates -> time model, padded wide tiles allowed.
         const int cands[7] = {256, 224, 192, 160, 128, 64, 16};
         double best = 1e30;
         for (int i = 0; i < 7; ++i) {
@@ -1043,20 +641,18 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
         }
     }
     plan->bn = bn;
-    // CTA pairs (cta_group::2, M = 256 per pair, each CTA stages half of B).  Measured on B200 (profiles/r01_ncu_gemm.md):
-    // no gain over one CTA per tile for this kernel's shapes (69 % vs 66 % tensor-pipe at 24576x2560x1280, slightly slower
-    // on the K = 320 layers), so pairs are opt-in (T2V_2CTA=1 or force_cg) until the pair path gets TMA multicast.
+    // Clusters of two CTAs (two M-tiles, B halves multicast into both): opt-in (T2V_2CTA=1 or force_cg), not measured faster.
     static const bool use_pairs = getenv("T2V_2CTA") != nullptr;
     plan->cg = p.force_cg ? p.force_cg : ((g.tiles_m >= 2 && bn >= 64 && use_pairs) ? 2 : 1);
-    if (bn < 64 || p.b_batch_dim >= 0 || plan->bs || bn == 192 || bn == 224) plan->cg = 1;     // a pair shares ONE B tile: never across B batches
+    if (bn < 64 || p.b_batch_dim >= 0 || plan->bs || bn == 192 || bn == 224) plan->cg = 1;     // a cluster shares ONE B tile: never across B batches
     g.tiles_n = (p.N + bn - 1) / bn;
     if ((p.flags & GEMM_GEGLU) && (p.N % bn) != 0) {
-        fprintf(stderr, "[t2v_b200] gemm_plan: GEGLU needs N %% BN == 0 (N %d BN %d)\n", p.N, bn);
+        fprintf(stderr, "[t2v] gemm_plan: GEGLU needs N %% BN == 0 (N %d BN %d)\n", p.N, bn);
         return -4;
     }
     if ((p.flags & GEMM_GEGLU) && ((p.ldo & 15) != 0 || (reinterpret_cast<uintptr_t>(p.out) & 31) != 0 || p.residual != nullptr ||
                                    (p.flags & GEMM_OUT_F32) || p.bias_rows != 0 || p.splits > 1)) {
-        fprintf(stderr, "[t2v_b200] gemm_plan: GEGLU epilogue needs 32-byte aligned fp16 output rows (ldo %lld), no residual, "
+        fprintf(stderr, "[t2v] gemm_plan: GEGLU epilogue needs 32-byte aligned fp16 output rows (ldo %lld), no residual, "
                         "no per-sample bias, no split-K\n", p.ldo);
         return -4;
     }
@@ -1082,47 +678,8 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
                               static_cast<cuuint64_t>(nb)};
         const cuuint64_t ldb = static_cast<cuuint64_t>(p.ldb > 0 ? p.ldb : p.K);
         cuuint64_t strides[2] = {ldb * 2, ldb * 2 * static_cast<cuuint64_t>(p.n_alloc)};
-        cuuint32_t box[3] = {GEMM_BLOCK_K, static_cast<cuuint32_t>(bn / plan->cg), 1};   // a CTA of a pair stages half of B
+        cuuint32_t box[3] = {GEMM_BLOCK_K, static_cast<cuuint32_t>(bn / plan->cg), 1};   // a CTA of a cluster fetches half of B
         if (encode_map(&g.map_b, p.b, 3, dims, strides, box) != 0) return -6;
-    }
-    // ---- TMA-store epilogue (T2V_NO_TMA_STORE=1 disables): fp16 output, full 128-row boxes whose 32-row quadrants are sub-boxes
-    //      of the row grid.  Measured: 49.8 -> 46.6 us on the level-0 QKV projection (N = 960, K = 320), 1.6 % on the forward.
-    static const bool want_tma_store = getenv("T2V_NO_TMA_STORE") == nullptr;
-    if (want_tma_store && !(p.flags & (GEMM_GEGLU | GEMM_OUT_F32)) && p.splits <= 1 && bn >= 32 && (p.ldo & 7) == 0 && (p.N & 7) == 0 &&
-        (reinterpret_cast<uintptr_t>(p.out) & 15) == 0 && (p.residual == nullptr || (p.ldr & 7) == 0)) {
-        int sub[GEMM_MAX_RDIMS];
-        int rem = 32, prod = 1;
-        bool ok = true;
-        for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
-            prod *= g.box[d];
-            sub[d] = std::min(g.box[d], rem);
-            if (sub[d] < 1 || g.box[d] % sub[d] != 0 || rem % sub[d] != 0) ok = false;
-            else rem /= sub[d];
-        }
-        if (ok && rem == 1 && prod == GEMM_BLOCK_M) {
-            for (int q = 0; q < 4; ++q) {
-                int off = q * 32;
-                for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
-                    g.st_off[q][d] = static_cast<int8_t>(off % g.box[d]);
-                    off /= g.box[d];
-                }
-            }
-            cuuint64_t dims[5], strides[4];
-            cuuint32_t box[5], estr[5] = {1, 1, 1, 1, 1};
-            dims[0] = static_cast<cuuint64_t>(p.N);
-            box[0] = 32;
-            cuuint64_t pitch = static_cast<cuuint64_t>(p.ldo) * 2;
-            for (int d = 0; d < p.nd; ++d) {
-                dims[d + 1] = static_cast<cuuint64_t>(g.dim[d]);
-                box[d + 1] = static_cast<cuuint32_t>(sub[d]);
-                strides[d] = pitch;
-                pitch *= static_cast<cuuint64_t>(g.dim[d]);
-            }
-            const CUresult r = g_encode(&g.map_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, static_cast<cuuint32_t>(p.nd + 1), p.out, dims,
-                                        strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r == CUDA_SUCCESS) g.flags |= GEMM_TMA_STORE;
-        }
     }
     const Variant* var = find_variant(bn, (p.flags & GEMM_GEGLU) != 0, plan->cg, plan->bs);
     if (var == nullptr) return -7;
@@ -1143,7 +700,7 @@ int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(static_cast<unsigned>(plan.grid));
-    cfg.blockDim = dim3(static_cast<unsigned>(n_threads((plan.desc.flags & GEMM_GEGLU) != 0)));
+    cfg.blockDim = dim3(static_cast<unsigned>(kThreads));
     cfg.dynamicSmemBytes = static_cast<size_t>(plan.smem);
     cfg.stream = stream;
     cudaLaunchAttribute attr[2];
@@ -1167,11 +724,3 @@ int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
 }
 
 }  // namespace t2v
-
-#if T2V_GEMM_TRACE
-// trace builds only (scripts/gemm_trace.py): device buffer of 2 * 4 * 4096 u64, or null to stop recording
-extern "C" int t2v_debug_gemm_trace(void* buf) {
-    unsigned long long* p = reinterpret_cast<unsigned long long*>(buf);
-    return cudaMemcpyToSymbol(t2v::g_trace_buf, &p, sizeof(p)) == cudaSuccess ? 0 : -1;
-}
-#endif

@@ -1,4 +1,4 @@
-// Implicit-GEMM engine on tcgen05: every dense contraction of the denoiser / VAE (Linear, Conv1d k=1,
+// Implicit-GEMM engine on wgmma + TMA: every dense contraction of the denoiser / VAE (Linear, Conv1d k=1,
 // Conv2d 1x1 / 3x3, Conv3d (3,1,1)) is one launch of gemm_tc_kernel.
 //
 //   D[row, n] = sum_{tap} sum_{k} A[row + tap_offset(tap), k] * W[tap][n][k]   (+ bias, + residual, GEGLU ...)
@@ -25,11 +25,7 @@ enum GemmFlags : int {
     GEMM_OUT_F32 = 2,      // store fp32 instead of fp16
     GEMM_LN = 4,           // LayerNorm of the A rows folded into the epilogue: out = rstd_r * (acc - mean_r * colsum_n) + bias32_n
                            //   (weights pre-scaled by gamma; colsum_n = sum_k W'[n,k]; bias32_n = sum_k W[n,k] beta_k + bias_n)
-    GEMM_TMA_STORE = 8,    // set by gemm_plan: fp16 tile rows go through a swizzled smem staging buffer and cp.async.bulk.tensor stores
-    // bring-up / performance-isolation switches (never set by the model code)
-    GEMM_DBG_NO_STORE = 256,   // epilogue skips the global stores
-    GEMM_DBG_NO_EPI = 512,     // epilogue releases the accumulator without reading it
-    GEMM_DBG_NO_MMA = 1024,    // MMA warp commits without issuing tcgen05.mma (pure TMA pipeline)
+    // switches of t2v_op_gemm (never set by the model code)
     GEMM_DBG_FORCE_BS = 2048,  // t2v_op_gemm only: take the B-stationary variant whenever it is eligible (any K chunk count)
     GEMM_DBG_NO_BS = 4096,     // t2v_op_gemm only: never take it
 };
@@ -59,8 +55,6 @@ struct GemmDesc {
     const float2* rowstat;           // GEMM_LN: (mean, rstd) per global row
     const float* colsum;             // GEMM_LN: per packed column
     const float* bias32;             // GEMM_LN: per packed column (replaces `bias`)
-    CUtensorMap map_out;             // GEMM_TMA_STORE: rank 1 + nd view of the output, box = (32 columns, 32 rows of a tile quadrant)
-    int8_t st_off[4][GEMM_MAX_RDIMS]; //   origin of quadrant q (rows 32q..32q+31 of the tile) inside the tile box
     int splits;                      // split-K: work item = (tile, split); each split owns k_per_split k-iterations and
     int k_per_split;                 //   stores its fp32 partial tile at out + split * split_stride (reduced by splitk_reduce)
     long long split_stride;
@@ -90,7 +84,7 @@ struct GemmProblem {
     long long ldr;
     float alpha;
     int force_bn;                    // 0 = auto
-    int force_cg;                    // 0 = auto, 1 / 2
+    int force_cg;                    // 0 = auto, 1 / 2 (2: cluster of two M-tiles sharing each B box through TMA multicast)
     const float2* rowstat;           // GEMM_LN operands (see GemmFlags)
     const float* colsum;
     const float* bias32;
@@ -102,7 +96,7 @@ struct GemmProblem {
 struct GemmPlan {
     GemmDesc desc;
     int bn;
-    int cg;                          // 1 = one CTA per tile, 2 = CTA pair (tcgen05 cta_group::2) per two M-tiles
+    int cg;                          // 1 = one CTA per tile, 2 = cluster of two CTAs (two M-tiles) that multicast halves of B
     int bs;                          // 1 = B-stationary variant (CTA = one N-tile, walks M-tiles; weights resident in smem)
     int grid;
     int smem;

@@ -59,7 +59,7 @@ struct RelposParams {
 };
 int attention_relpos(const RelposParams& p, cudaStream_t stream);
 
-// attention_tc.cu: tcgen05 / TMEM / TMA kernel for long self-attention sequences (sq >= 256, skv >= 128, one-level batch).
+// attention_tc.cu: wgmma / TMA kernel for long self-attention sequences (sq >= 256, skv >= 128, one-level batch).
 // The plan holds the three tensor maps (encoded once per UNet plan, the launch itself is host-side free of driver calls).
 struct AttnTcPlan {
     CUtensorMap map_q, map_k, map_v;   // rank 3: (heads*64, sequence, batch)

@@ -4,7 +4,7 @@
 //   * spatial modules (ResBlock convs, SpatialTransformer, Down/Upsample) see rows grouped per frame,
 //   * temporal modules (TemporalConvBlock_v2, TemporalTransformer) address the SAME buffer with a frame stride,
 // so none of the reference's `(b f) c h w <-> b c f h w <-> (b h w) f c` rearrange copies exist here.
-// Every contraction goes through the tcgen05 implicit-GEMM engine (gemm_tc.cu); norms / attention / glue are the
+// Every contraction goes through the wgmma implicit-GEMM engine (gemm_tc.cu); norms / attention / glue are the
 // kernels in norm.cu, attention.cu, elementwise.cu.
 #include "../../include/t2v_b200.h"
 #include "runtime.cuh"
@@ -491,7 +491,7 @@ Tok transformer_block(Ctx& c, Tok x, const std::string& p, int heads, long long 
             AttnTcPlan tcp;
             if (!c.b->dry() && attention_tc_eligible(apc) && !getenv("T2V_ATTN_WARP_MMA") &&
                 attention_tc_plan(apc, &tcp) == 0) {
-                // long sequences: tcgen05 kernel, tensor maps encoded once here
+                // long sequences: wgmma kernel, tensor maps encoded once here
                 c.b->step([tcp](cudaStream_t s) { return attention_tc_launch(tcp, s); }, 1, STEP_ATTN, fl, label);
             } else {
                 c.b->step([apc](cudaStream_t s) { return attention(apc, s); }, 1, STEP_ATTN, fl, label);

@@ -3,7 +3,7 @@
 // Replaces modelscope/t2v_model.py:1646-1649 + ldm.modules.diffusionmodules.model.Decoder (vendored twin:
 // videocrafter/lvdm/models/modules/autoencoder_modules.py:484-596) and batches ALL frames of the clip instead of the
 // reference's one-frame-per-call loop with a D2H sync per frame (t2v_pipeline.py:329-355).
-// Same channels-last token layout and the same tcgen05 implicit-GEMM engine as the denoiser.
+// Same channels-last token layout and the same wgmma implicit-GEMM engine as the denoiser.
 #include "../../include/t2v_b200.h"
 #include "runtime.cuh"
 

@@ -1,6 +1,6 @@
 """ctypes binding of libt2v_b200.so (the C ABI declared in include/t2v_b200.h).
 
-There is deliberately NO fallback: if the shared library is missing or the device is not sm_100 the import of
+There is deliberately NO fallback: if the shared library is missing or the device is not sm_90 the import of
 the product path fails loudly (RuntimeError) -- a silent PyTorch path would void every parity/perf claim.
 """
 import ctypes as C
@@ -121,12 +121,12 @@ def load_library():
 
 
 def lib():
-    """The library, initialised on the current CUDA device.  Raises if there is no sm_100 GPU."""
+    """The library, initialised on the current CUDA device.  Raises if there is no sm_90 GPU."""
     global _inited_device
     import torch
     l = load_library()
     if not torch.cuda.is_available():
-        raise RuntimeError('t2v_b200 needs a CUDA device (sm_100a); no CPU fallback exists')
+        raise RuntimeError('t2v_b200 needs a CUDA device (sm_90a); no CPU fallback exists')
     dev = torch.cuda.current_device()
     if _inited_device != dev:
         torch.cuda.init()

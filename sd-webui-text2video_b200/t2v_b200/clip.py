@@ -1,5 +1,5 @@
 """`FrozenOpenCLIPEmbedder` -- the text conditioning step in front of the denoising loop (reference:
-scripts/modelscope/clip_hardcode.py:59-422), with the OpenCLIP ViT-H-14 text transformer on the B200-native library.
+scripts/modelscope/clip_hardcode.py:59-422), with the OpenCLIP ViT-H-14 text transformer on the GPU-native library.
 
 Kept from the reference: the class name, `.model` holding open_clip's parameter tree (`model.token_embedding`,
 `model.positional_embedding`, `model.transformer.resblocks[i].{ln_1, attn, ln_2, mlp.c_fc, mlp.c_proj}`, `model.ln_final`,

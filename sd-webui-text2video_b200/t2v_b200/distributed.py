@@ -1,7 +1,7 @@
 """Sample-parallel sharding of clips over the GPUs of one node -- the only parallelism the reference has
 (videocrafter/sample_text2video.py:174-188 + lvdm/utils/dist_utils.py:4-19): every rank owns the full weights, draws its
 own noise from `seed + rank`, and ONE all-gather collects the decoded clips.  No collective touches the denoising
-loop, so scaling is weak.  Backend-agnostic (NCCL over NVLink on the B200 box, gloo in the CPU tests).
+loop, so scaling is weak.  Backend-agnostic (NCCL over NVLink on a multi-GPU node, gloo in the CPU tests).
 
 Opt-in second mode (T2V_CFG_SPLIT=1, even world size): the classifier-free-guidance pair of every step -- two independent
 forwards, gaussian_sampler.py:161-162 / ddim/sampler.py:176-179 / ddim.py:216-217 -- is split over a PAIR of GPUs (even

@@ -1,4 +1,4 @@
-"""Stable-LoRA merging for the B200-native denoiser -- the arithmetic of `StableLoraProcessor.process_lora`
+"""Stable-LoRA merging for the GPU-native denoiser -- the arithmetic of `StableLoraProcessor.process_lora`
 (scripts/stable_lora/stable_utils/lora_processor.py:202-246 and :50-96) done on the library's packed weights.
 
 The reference walks `model.named_modules()`, and for every `<name>.lora_A` / `<name>.lora_B` pair in a LoRA file replaces

@@ -1,5 +1,5 @@
 """`TextToVideoSynthesis` -- the pipeline object behind the reference's `process_modelscope` entry point
-(scripts/modelscope/t2v_pipeline.py:45-385), with the denoising loop and the VAE decode on the B200-native library.
+(scripts/modelscope/t2v_pipeline.py:45-385), with the denoising loop and the VAE decode on the GPU-native library.
 
 Same public surface: `TextToVideoSynthesis(model_dir)`, attributes `.sd_model .autoencoder .clip_encoder .diffusion
 .model_dir .keep_in_vram`, and `infer(prompt, n_prompt, steps, frames, seed, scale, width, height, eta, cpu_vae,

@@ -1,5 +1,5 @@
 """`process_modelscope(args_dict, extra_args)` -- the entry point `t2v_helpers.render.run` dispatches to
-(reference: scripts/modelscope/process_modelscope.py:34-266), backed by the B200-native pipeline.
+(reference: scripts/modelscope/process_modelscope.py:34-266), backed by the GPU-native pipeline.
 
 Kept: the name, the signature, the return type (`list[str]` of data-URL videos, process_modelscope.py:34,:256-262), the
 module-global `pipe` cache (reset by render.py:41 through `pipe = None`), the batch loop with `seed + batch`

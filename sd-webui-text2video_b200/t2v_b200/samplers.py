@@ -5,7 +5,7 @@
     each with `.sample(S=, conditioning=, unconditional_conditioning=, unconditional_guidance_scale=, x_T=, shape=,
     eta=, mask=, callback=, strength=, t_start=, ...)`            (samplers_common.py:77-207)
 
-What changed underneath (B200-first):
+What changed underneath (GPU-first):
   * the conditional and unconditional denoiser evaluations of a step are ONE batched forward (B = 2) when the
     denoiser is our UNetSD -- the reference runs two sequential B = 1 forwards (gaussian_sampler.py:161-162);
   * classifier-free guidance + the latent update of a step are ONE fused CUDA kernel (t2v_ddim_step / t2v_cfg_x0 +

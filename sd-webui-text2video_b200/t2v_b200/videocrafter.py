@@ -1,4 +1,4 @@
-"""VideoCrafter text2video path (SURVEY.md section 8 rows a19-a20) on the B200-native kernels.
+"""VideoCrafter text2video path (SURVEY.md section 8 rows a19-a20) on the GPU-native kernels.
 
 Mirrors, with the reference's names / signatures for the calls on the path:
   * `LatentDiffusion`      videocrafter/lvdm/models/ddpm3d.py: `apply_model` :849-865 (DiffusionWrapper 'crossattn' :1378-1380),

@@ -16,6 +16,11 @@ def errs(a, b):
            ((a - b).pow(2).mean().sqrt() / (b.pow(2).mean().sqrt() + 1e-9)).item()
 
 
+def on_fixture_frames(t, g):
+    """`t` [B, C, F, h, w] restricted to the frames a fixture stores (fixtures of large clips keep a fixed subset, `frames`)."""
+    return t[:, :, g['frames']] if 'frames' in g else t
+
+
 def pass_rate(a, b, rtol=1e-3, atol=1e-4):
     """Fraction of elements inside BASELINE.json's element-wise gate |a-b| <= atol + rtol*|b|."""
     a, b = a.float().cpu(), b.float().cpu()
@@ -34,7 +39,7 @@ def report(name, **kv):
 class AutocastOracle(object):
     """The reference's GPU numerics contract (SURVEY.md appendix B): the SAME torch ops as the reference module tree, fp16
     weights, under torch.autocast('cuda') (t2v_pipeline.py:271: `with amp.autocast(enabled=True)`), attention through
-    F.scaled_dot_product_attention (t2v_model.py:566-569, the backend reachable on sm_100).  It is the honest yardstick for
+    F.scaled_dot_product_attention (t2v_model.py:566-569, the backend the reference takes without xformers).  It is the honest yardstick for
     "matches the reference PyTorch path": our error against the fp32 fixture is gated against THIS path's error against
     the same fixture."""
 

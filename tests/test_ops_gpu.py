@@ -27,7 +27,7 @@ def ops():
     (1, 64, 64, 0, True, False), (129, 72, 200, 0, True, True)])
 def test_linear(ops, M, K, N, bn, bias, res, cg):
     if cg == 2 and (bn == 16 or N <= 16):
-        pytest.skip('CTA pairs need BN >= 64')
+        pytest.skip('two-CTA clusters need BN >= 64')
     a = torch.randn(M, K, device=dev).half()
     w = (torch.randn(N, K, device=dev) / K ** 0.5).half()
     b = torch.randn(N, device=dev).half() if bias else None
@@ -51,7 +51,7 @@ def test_linear(ops, M, K, N, bn, bias, res, cg):
 @pytest.mark.parametrize('cg', [1, 2])
 def test_conv3x3_implicit_gemm(ops, NF, h, w, Cin, Cout, cg):
     if cg == 2 and Cout < 64:
-        pytest.skip('CTA pairs need BN >= 64')
+        pytest.skip('two-CTA clusters need BN >= 64')
     x = torch.randn(NF, h, w, Cin, device=dev).half()
     wt = (torch.randn(Cout, Cin, 3, 3, device=dev) / (9 * Cin) ** 0.5).half()
     b = torch.randn(Cout, device=dev).half()
@@ -216,7 +216,7 @@ def test_attention_dense_layout(ops, batch, heads, sq, skv):
 
 @pytest.mark.parametrize('batch,heads,S', [(2, 5, 1024), (3, 2, 320), (1, 2, 9216), (2, 3, 256), (1, 1, 1000)])
 def test_attention_tcgen05_fused_qkv(ops, batch, heads, S):
-    """Long spatial sequences take the tcgen05/TMEM kernel (csrc/attention_tc.cu): Q, K, V are column slices of the fused
+    """Long spatial sequences take the wgmma kernel (csrc/attention_tc.cu): Q, K, V are column slices of the fused
     [tokens, 3C] matrix, the head is a tensor-map column offset, ragged tails (S % 128 != 0) are TMA zero fill + masking."""
     C = heads * 64
     qkv = torch.randn(batch * S, 3 * C, device=dev).half()
@@ -231,7 +231,8 @@ def test_attention_tcgen05_fused_qkv(ops, batch, heads, S):
 
 def test_attention_tcgen05_shared_kv_and_peaked_scores(ops):
     """kv_batch_div (frames sharing K/V), skv != sq with a ragged last key tile, and scores large enough that the running
-    max actually moves between key tiles (exercises the exp2 rescale of the running output)."""
+    max actually moves between key tiles (exercises the exp2 rescale of the running output).  Kept under its original name:
+    the kernel is the wgmma one in csrc/attention_tc.cu."""
     batch, heads, sq, skv, div = 4, 2, 384, 200, 2
     C = heads * 64
     q = (torch.randn(batch, sq, C, device=dev) * 3).half()

@@ -1,13 +1,11 @@
 """CPU: the oracle restatement reproduces the committed reference outputs (tests/golden/*.pt, produced by
-oracle/make_golden.py from the UNMODIFIED reference).  When /root/reference is mounted, the restatement is also
-re-checked live against the reference modules."""
+oracle/make_golden.py from the UNMODIFIED reference)."""
 import os
 
 import pytest
 import torch
 
 from oracle import unet_oracle as UO, vae_oracle as VO, samplers_oracle as SO
-from oracle import ref_shim
 from oracle.make_golden import analytic_model, _SchedModel, synth_inputs
 
 
@@ -81,20 +79,15 @@ def test_ddim_timestep_grids():
     assert dts[0] == 1 and dts[-1] == 981
 
 
-@pytest.mark.skipif(not ref_shim.reference_available(), reason='reference tree not mounted')
-def test_oracle_unet_live_against_reference():
-    m = ref_shim.load_modelscope()
+def test_oracle_unet_live_against_reference(gold_dir):
+    """The oracle UNetSD vs the reference UNetSD's output for the same weights and inputs (tests/golden/reference_live.pt)."""
+    ref = torch.load(os.path.join(gold_dir, 'reference_live.pt'))['unet_out']
     cfg = UO.UNetConfig(dim=64)
-    net = m.UNetSD(in_dim=4, dim=64, y_dim=768, context_dim=1024, out_dim=4, dim_mult=[1, 2, 4, 4], num_heads=8,
-                   head_dim=64, num_res_blocks=2, attn_scales=[1, 0.5, 0.25], dropout=0.1, temporal_attention=True).eval()
     W = UO.make_weights(UO.param_specs(cfg), seed=5)
-    net.load_state_dict(W, strict=True)
     g = torch.Generator().manual_seed(9)
     x = torch.randn(2, 4, 3, 8, 8, generator=g)
     y = torch.randn(2, 77, 1024, generator=g)
     t = torch.tensor([500, 20])
-    with torch.no_grad():
-        ref = net(x, t, y)
     assert torch.allclose(UO.unet_forward(W, cfg, x, t, y), ref, rtol=0, atol=3e-5)
 
 
@@ -162,8 +155,10 @@ def test_full_size_fixtures_are_consistent(gold_dir):
     (make_golden.py asserted oracle == reference when it wrote them); check their shapes and that the single-step latents
     follow from the stored eps through the pinned scheduler restatement (DDIM_Gaussian: no model call needed)."""
     g = torch.load(os.path.join(gold_dir, 'unet_cfg2.pt'))
-    assert (g['F'], g['h'], g['w']) == (24, 32, 32) and g['eps_cond'].shape == (1, 4, 24, 32, 32)
+    nf = len(g['frames'])                   # the fixture keeps a fixed subset of the 24 frames (DDIM_Gaussian is per element)
+    assert (g['F'], g['h'], g['w']) == (24, 32, 32) and g['eps_cond'].shape == (1, 4, nf, 32, 32)
     x, c, uc = synth_inputs(24, 32, 32)
+    x = x[:, :, g['frames']]
     calls = []
 
     def model(xx, tt, cc):

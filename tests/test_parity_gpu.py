@@ -2,8 +2,8 @@
 
 Three yardsticks per case (all printed as `[parity] {...}` lines; T2V_PARITY_REPORT=<file> records them):
   1. the REFERENCE's fp32 CPU output committed in tests/golden (written by oracle/make_golden.py from the unmodified
-     reference modules) -- relative RMS and max error of our fp16 path against it, gated at the measured value x 1.5
-     (the constants below were measured on B200 and are listed in DESIGN.md section 5);
+     reference modules) -- relative RMS and max error of our fp16 path against it, gated by the constants below (the
+     values measured on H100 are listed beside them and in DESIGN.md section 5);
   2. the reference's GPU numerics contract: the same torch ops under fp16 autocast + SDPA on the same GPU
      (parity_util.AutocastOracle).  Gate: err(ours, fp32 fixture) <= 1.5 x err(autocast path, fp32 fixture) -- i.e. we are
      at least as close to the fp32 truth as the reference's own fp16 path is (up to the stated slack);
@@ -17,21 +17,21 @@ import torch
 
 from oracle import unet_oracle as UO, samplers_oracle as SO, vc_oracle as VC
 from oracle.make_golden import synth_inputs
-from parity_util import AutocastOracle, errs, first_update, pass_rate, report
+from parity_util import AutocastOracle, errs, first_update, on_fixture_frames, pass_rate, report
 
 pytestmark = pytest.mark.gpu
 
 SLACK = 1.5
-# measured relative-RMS error of eps vs the reference's fp32 output x 1.5 (B200, round 2; see DESIGN.md section 5)
-# measured (profiles/r02_parity_report.jsonl): tiny 2.63e-3, cfg1 2.90e-3, cfg2 2.86e-3, cfg3 slice 2.68e-3, 125 frames 3.01e-3, VC cfg5 2.04e-3
+# relative-RMS error of eps vs the reference's fp32 output, measured on H100 (T2V_PARITY_REPORT): tiny 2.45e-3, cfg1 2.88e-3,
+# cfg2 2.85e-3, cfg3 slice 2.68e-3, 125 frames 2.99e-3, VC cfg5 2.07e-3
 GATE_RMS = {'unet_tiny': 4.0e-3, 'unet_cfg1': 4.4e-3, 'unet_cfg2': 4.3e-3, 'unet_cfg3_slice': 4.0e-3, 'unet_f125': 4.5e-3,
             'vc_unet_cfg5': 3.1e-3}
-# max |err| / max |ref|, measured 2.4e-3 / 2.9e-3 / 3.1e-3 / 2.7e-3 / 3.5e-3 / 2.2e-3
+# max |err| / max |ref|, measured on H100 2.4e-3 / 3.4e-3 / 2.7e-3 / 2.9e-3 / 3.7e-3 / 2.2e-3
 GATE_MAX = {'unet_tiny': 3.6e-3, 'unet_cfg1': 4.4e-3, 'unet_cfg2': 4.7e-3, 'unet_cfg3_slice': 4.1e-3, 'unet_f125': 5.3e-3,
             'vc_unet_cfg5': 3.3e-3}
-# latent after ONE scheduler update vs the reference sampler's: measured DDIM_Gaussian 1.76e-3 rms / 2.9e-3 max (x 1.5)
-# DDIM 2.5e-3 / 3.1e-3; UniPC (the latent handed to the 5th model call: corrector of update 1 + predictor of update 2, i.e.
-# differences of x0-predictions at sigma/alpha ~ 15) 7.1e-3 / 6.8e-3.  Its scheduler arithmetic is pinned on the CPU
+# latent after ONE scheduler update vs the reference sampler's, measured on H100 (cfg1 / cfg2): DDIM_Gaussian 1.75e-3 rms /
+# 2.8e-3 max, DDIM 2.4e-3 / 2.8e-3; UniPC (the latent handed to the 5th model call: corrector of update 1 + predictor of update 2, i.e.
+# differences of x0-predictions at sigma/alpha ~ 15) 7.2e-3 / 8.5e-3.  Its scheduler arithmetic is pinned on the CPU
 # (tests/test_samplers_host_cpu.py: product host algebra == oracle to 1e-7 with fp16 eps); the rest is fp16 rounding noise of the
 # denoiser re-rolled by the UniPC update (scripts/diag_unipc.py: a 3.5e-8 change of x moves the fp16 eps by 2.4e-3)
 GATE_STEP = {'ddim_gaussian_x1': (2.7e-3, 4.5e-3), 'ddim_x1': (3.8e-3, 4.7e-3), 'unipc_x1': (1.07e-2, 1.03e-2)}
@@ -93,11 +93,11 @@ def _gate_step(case, g, net, betas, ac):
     for key, (sname, S, stop_at, oracle_run) in runs.items():
         if key not in g:
             continue
-        ours = first_update(lambda m: _sampler(sname, m, betas).sample(S=S, **kw), net, stop_at)
+        ours = on_fixture_frames(first_update(lambda m: _sampler(sname, m, betas).sample(S=S, **kw), net, stop_at), g)
         e = errs(ours, g[key])
         rec = dict(ours_max=e[0], ours_rms=e[1], ours_pass_1e3=pass_rate(ours, g[key]))
         if oracle_run is not None:
-            auto = first_update(oracle_run, acm, stop_at)
+            auto = on_fixture_frames(first_update(oracle_run, acm, stop_at), g)
             a = errs(auto, g[key])
             rec.update(autocast_max=a[0], autocast_rms=a[1], autocast_pass_1e3=pass_rate(auto, g[key]))
         report(f'{case}:{key}', **rec)
@@ -123,7 +123,7 @@ def _gate_step(case, g, net, betas, ac):
         pass
     finally:
         S_._step_kernel = orig
-    eb = errs(seen['x1'], g['ddim_gaussian_x1'])
+    eb = errs(on_fixture_frames(seen['x1'], g), g['ddim_gaussian_x1'])
     report(f'{case}:ddim_gaussian_x1:batched_B2', ours_max=eb[0], ours_rms=eb[1])
     assert eb[1] <= GATE_STEP['ddim_gaussian_x1'][0] and eb[0] <= GATE_STEP['ddim_gaussian_x1'][1], eb
 
@@ -141,17 +141,18 @@ def test_config1_forward_and_single_step(full, gold_dir):
 
 def test_config2_forward_and_single_step(full, gold_dir):
     """BASELINE config 2's shape -- 24 frames x 256^2, the shape every bench number is quoted on (different tile counts,
-    split-K decisions, attention_tc at S = 1024, TMA-store eligibility than config 1)."""
+    split-K decisions, attention_tc at S = 1024 than config 1).  The fixture keeps a fixed subset of the 24 frames; the
+    network still runs all of them."""
     cfg, W, net, betas, ac = full
     g = torch.load(os.path.join(gold_dir, 'unet_cfg2.pt'))
     x, c, uc = synth_inputs(g['F'], g['h'], g['w'])
     t = torch.tensor([g['t']])
     outs = {}
     for tag, ctx, key in (('cond', c, 'eps_cond'), ('uncond', uc, 'eps_uncond')):
-        outs[tag] = net(x.cuda(), t.cuda(), ctx.cuda())
-        _gate_forward(f'unet_cfg2:{tag}', outs[tag], ac(x, t, ctx), g[key])
+        outs[tag] = on_fixture_frames(net(x.cuda(), t.cuda(), ctx.cuda()), g)
+        _gate_forward(f'unet_cfg2:{tag}', outs[tag], on_fixture_frames(ac(x, t, ctx), g), g[key])
     # the production B = 2 forward (cond + uncond in one call) against the two B = 1 forwards
-    both = net(x.cuda().expand(2, -1, -1, -1, -1), t.cuda().expand(2), torch.cat([c, uc]).cuda())
+    both = on_fixture_frames(net(x.cuda().expand(2, -1, -1, -1, -1), t.cuda().expand(2), torch.cat([c, uc]).cuda()), g)
     eb = errs(both[0:1], g['eps_cond']), errs(both[1:2], g['eps_uncond'])
     report('unet_cfg2:B2', cond_rms=eb[0][1], uncond_rms=eb[1][1], b2_vs_b1_rms=errs(both[0:1], outs['cond'])[1])
     assert max(eb[0][1], eb[1][1]) <= GATE_RMS['unet_cfg2']
