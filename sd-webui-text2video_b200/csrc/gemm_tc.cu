@@ -5,7 +5,8 @@
 //                                  coordinates, OOB = zero padding) + one B box (BN x 64 K) into a SWIZZLE_128B smem ring
 //   warpgroups 1, 2 consumers    : each owns 64 rows of the 128-row tile; per ring stage 4 k-steps of wgmma m64 x BN x 16
 //                                  (both operands from shared memory) into fp32 registers, then the epilogue (alpha, bias,
-//                                  LayerNorm fold, residual, GEGLU) straight from the accumulator registers to global memory.
+//                                  LayerNorm fold, residual, GEGLU) through a per-warp shared-memory staging slab, so that
+//                                  global loads and stores are 16 B per thread over whole 128 B row segments.
 // The producer runs ahead into the next tile while the consumers are in the epilogue.
 // CG = 2: a cluster of two CTAs owns two consecutive M-tiles of the same N-tile; each CTA fetches half of the B box and
 // TMA-multicasts it into both CTAs, so B crosses L2 -> SM once per pair.
@@ -29,15 +30,22 @@ constexpr int kRegsConsumer = 232;
 constexpr int kABytes = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;     // 16 KB
 constexpr int kSmemBudget = 216 * 1024;                      // ring (barriers + alignment slack on top; 227 KB per block)
 constexpr int kMaxStages = 8;
+// Epilogue staging, per consumer warp: 8 rows x 128 B (half of the warp's 16 rows at a time) + the global row index of each of
+// its 16 rows.  It sits outside the ring budget, in what the 227 KB per block leaves over, so no ring loses a stage.
+constexpr int kEpiRowBytes = 128;
+constexpr int kEpiWarpBytes = 8 * kEpiRowBytes + 16 * 8;
+constexpr int kEpiBytes = 8 * kEpiWarpBytes;
 
 template <int BN>
 struct Cfg {
     static constexpr int kBBytes = BN * GEMM_BLOCK_K * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
     static constexpr int kStages = (kSmemBudget / kStageBytes) > kMaxStages ? kMaxStages : (kSmemBudget / kStageBytes);
-    static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + kEpiBytes;
+    static_assert(kSmemBytes <= 227 * 1024, "shared memory per block");
 };
-constexpr int kBsSmemBytes = kSmemBudget + 1024 + 256;      // B-stationary: resident weights + A ring fill the budget
+constexpr int kBsSmemBytes = kSmemBudget + 1024 + 256 + kEpiBytes;      // B-stationary: resident weights + A ring fill the budget
+static_assert(kBsSmemBytes <= 227 * 1024, "shared memory per block");
 
 // erf-form GELU x * Phi(x) (F.gelu default, t2v_model.py:821).  Phi(x) = 1/2 erfc(-x / sqrt 2); for z = |x| / sqrt 2
 // erfc(z) = t (a1 + t (a2 + t (a3 + t (a4 + t a5)))) exp(-z^2), t = 1 / (1 + p z) (Abramowitz-Stegun 7.1.26, |error| <=
@@ -55,20 +63,163 @@ __device__ __forceinline__ float gelu_erf(float x) {
     return x * (x < 0.f ? q : 1.0f - q);
 }
 
-// One K = 16 step of a 64 x BN tile: BN is split into wgmma widths of 256 / 128 / 64 / 32 / 16.  Chunk n0 reads B rows
-// n0.. (n0 * 128 B further, a whole number of 1024 B swizzle atoms) and accumulates into registers acc[n0 / 2 ..].
-template <int BN>
-__device__ __forceinline__ void mma_k16(float* acc, uint64_t da, uint64_t db, uint32_t scale_d) {
-    if constexpr (BN == 256 || BN == 128 || BN == 64 || BN == 32 || BN == 16) {
-        wgmma_ss<BN>(acc, da, db, scale_d);
-    } else if constexpr (BN > 128) {
-        wgmma_ss<128>(acc, da, db, scale_d);
-        mma_k16<BN - 128>(acc + 64, da, db + static_cast<uint64_t>((128 * 128) >> 4), scale_d);
-    } else if constexpr (BN > 64) {
-        wgmma_ss<64>(acc, da, db, scale_d);
-        mma_k16<BN - 64>(acc + 32, da, db + static_cast<uint64_t>((64 * 128) >> 4), scale_d);
-    } else {
-        static_assert(BN < 0, "unsupported tile width");
+// Byte offset of (row r, byte b of the row) in a staging slab of 8 rows x `segs` 16 B segments.  The segment index
+// L = r * segs + b / 16 is XOR-swizzled with L / 8, so that the fragment side (8 rows, the same 16 B column of each) and the
+// row side (8 consecutive segments per quarter-warp) both touch 8 distinct 16 B bank groups.
+__device__ __forceinline__ uint32_t stg_off(int r, int b, int segs) {
+    const int L = r * segs + (b >> 4);
+    return static_cast<uint32_t>(((L ^ ((L >> 3) & 7)) << 4) | (b & 15));
+}
+
+// Epilogue of one warp: its 16 rows x BN accumulator columns (fragment layout, ptx.cuh) -> global memory.
+//   1. in place on the accumulators: alpha + bias, or the LayerNorm fold; bias / colsum / bias32 loaded once per column
+//   2. per unit (chunk of 128 B of output per row, half h = rows 8h .. 8h + 7): the residual slice is loaded with 16 B reads
+//      (issued one unit ahead) into the staging slab; each thread adds it to its fragment values, rounds, and writes the
+//      result back to the same place; then the rows leave with 16 B stores.
+// Per element the arithmetic is that of a direct store: fp32 affine, + residual in fp32, one rounding (GEGLU: fp16 value,
+// fp16 gate, fp16 gelu, fp16 product).  fp32 output (split-K partials) stages 32 columns per unit and has no residual
+// (gemm_plan).  A segment that is cut by N, or an unaligned output / residual, goes element-wise.
+// rowg[16]: global row of each of the warp's rows, -1 for rows outside the problem.
+template <int BN, bool GEGLU, bool F32>
+__device__ __forceinline__ void epilogue_warp(const GemmDesc& g, float (&acc)[BN / 2], uint8_t* stg, const long long* rowg,
+                                              int tn, int sp, int lane) {
+    static_assert(!(GEGLU && F32), "GEGLU stores fp16");
+    constexpr int ES = F32 ? 4 : 2;                      // output element bytes
+    constexpr int EPS = 16 / ES;                         // elements per 16 B segment
+    constexpr int OUTW = GEGLU ? BN / 2 : BN;            // output columns of the tile
+    constexpr int CW = kEpiRowBytes / ES;                // output columns per unit
+    constexpr int NCH = (OUTW + CW - 1) / CW;
+    constexpr int NU = 2 * NCH;                          // units: (chunk u / 2, half u % 2)
+    const int quad = lane & 3, fr = lane >> 2;           // fragment: rows fr, fr + 8; columns 8j + 2 quad + {0, 1}
+    const int nvalid = GEGLU ? g.N / 2 : g.N;
+    const int ocol0 = tn * OUTW;
+    const bool ln = (g.flags & GEMM_LN) != 0;
+    const bool has_res = g.residual != nullptr;
+    const bool vec_out = (g.ldo % EPS) == 0 && (reinterpret_cast<uintptr_t>(g.out) & 15) == 0 && (!F32 || (g.split_stride % EPS) == 0);
+    const bool vec_res = has_res && (g.ldr & 7) == 0 && (reinterpret_cast<uintptr_t>(g.residual) & 15) == 0;
+
+    // ---- 1. affine, in place
+    long long fg[2];
+    float2 rs[2];
+    const __half* brow[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        fg[h] = rowg[fr + 8 * h];
+        rs[h] = (ln && fg[h] >= 0) ? __ldg(g.rowstat + fg[h]) : make_float2(0.f, 1.f);      // (mean, rstd) of the row
+        brow[h] = g.bias;
+        if (g.bias != nullptr && g.bias_rows > 0 && fg[h] >= 0) brow[h] += (fg[h] / g.bias_rows) * g.bias_stride;
+    }
+    const bool row_bias = g.bias != nullptr && g.bias_rows > 0;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int col = tn * BN + 8 * j + 2 * quad + e;                  // packed accumulator column
+            if (!GEGLU && col >= nvalid) continue;
+            float& v0 = acc[4 * j + e];
+            float& v1 = acc[4 * j + 2 + e];
+            if (ln) {
+                const float cs = __ldg(g.colsum + col), b32 = __ldg(g.bias32 + col);
+                v0 = fmaf(rs[0].y, fmaf(-rs[0].x, cs, v0), b32);
+                v1 = fmaf(rs[1].y, fmaf(-rs[1].x, cs, v1), b32);
+            } else {
+                const float b0 = brow[0] != nullptr ? __half2float(__ldg(brow[0] + col)) : 0.f;
+                const float b1 = row_bias ? __half2float(__ldg(brow[1] + col)) : b0;
+                v0 = fmaf(v0, g.alpha, b0);
+                v1 = fmaf(v1, g.alpha, b1);
+            }
+        }
+    }
+
+    // ---- 2. staged stores
+    auto segs_of = [](int c) { return (min(CW, OUTW - c * CW) * ES) / 16; };
+    auto load_res = [&](int u, uint4 (&rb)[2]) {          // fp16 residual of unit u, row-side layout
+        const int c = u >> 1, h = u & 1, segs = segs_of(c);
+#pragma unroll
+        for (int p = 0; p < 2; ++p) {
+            const int idx = lane + 32 * p;
+            rb[p] = make_uint4(0u, 0u, 0u, 0u);
+            if (idx >= 8 * segs) continue;
+            const long long gr = rowg[8 * h + idx / segs];
+            const int col = ocol0 + c * CW + 8 * (idx % segs);
+            if (gr < 0) continue;
+            const __half* src = g.residual + gr * g.ldr + col;
+            if (vec_res && col + 8 <= nvalid) {
+                rb[p] = __ldg(reinterpret_cast<const uint4*>(src));
+            } else {
+                uint32_t w[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const __half2 v = __halves2half2(col + 2 * e < nvalid ? src[2 * e] : __ushort_as_half(0),
+                                                     col + 2 * e + 1 < nvalid ? src[2 * e + 1] : __ushort_as_half(0));
+                    w[e] = *reinterpret_cast<const uint32_t*>(&v);
+                }
+                rb[p] = make_uint4(w[0], w[1], w[2], w[3]);
+            }
+        }
+    };
+    uint4 rbuf[2][2];
+    if (!F32 && has_res) load_res(0, rbuf[0]);
+#pragma unroll
+    for (int u = 0; u < NU; ++u) {
+        const int c = u >> 1, h = u & 1, segs = segs_of(c);
+        if (!F32 && has_res) {
+#pragma unroll
+            for (int p = 0; p < 2; ++p) {
+                const int idx = lane + 32 * p;
+                if (idx < 8 * segs) *reinterpret_cast<uint4*>(stg + stg_off(idx / segs, 16 * (idx % segs), segs)) = rbuf[u & 1][p];
+            }
+            if (u + 1 < NU) load_res(u + 1, rbuf[(u + 1) & 1]);
+            __syncwarp();
+        }
+        // fragment side: row fr of this half, the chunk's columns
+#pragma unroll
+        for (int jj = 0; jj < CW / 8; ++jj) {
+            if (jj >= segs * EPS / 8) break;
+            const int j = c * (CW / 8) + jj;
+            uint8_t* sp_ = stg + stg_off(fr, (8 * jj + 2 * quad) * ES, segs);
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if constexpr (GEGLU) {
+                // out = fp16(value) * fp16(gelu(fp16(gate))): the reference's rounding points under autocast (t2v_model.py:819-821)
+                const __half2 xh = __floats2half2_rn(v0, v1);
+                const float2 gf = __half22float2(__floats2half2_rn(acc[BN / 4 + 4 * j + 2 * h], acc[BN / 4 + 4 * j + 2 * h + 1]));
+                const __half2 ge = __floats2half2_rn(gelu_erf(gf.x), gelu_erf(gf.y));
+                *reinterpret_cast<__half2*>(sp_) = __hmul2(xh, ge);          // fp16 x fp16 -> fp16 (RN)
+            } else if constexpr (F32) {
+                *reinterpret_cast<float2*>(sp_) = make_float2(v0, v1);
+            } else {
+                if (has_res) {
+                    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(sp_));
+                    v0 += f.x;
+                    v1 += f.y;
+                }
+                *reinterpret_cast<__half2*>(sp_) = __floats2half2_rn(v0, v1);
+            }
+        }
+        __syncwarp();
+        // row side: 16 B per thread, whole row segments
+#pragma unroll
+        for (int p = 0; p < 2; ++p) {
+            const int idx = lane + 32 * p;
+            if (idx >= 8 * segs) continue;
+            const long long gr = rowg[8 * h + idx / segs];
+            if (gr < 0) continue;
+            const int col = ocol0 + c * CW + EPS * (idx % segs);
+            const uint4 val = *reinterpret_cast<const uint4*>(stg + stg_off(idx / segs, 16 * (idx % segs), segs));
+            uint8_t* dst = static_cast<uint8_t*>(g.out) + ((F32 ? sp * g.split_stride : 0) + gr * g.ldo + col) * ES;
+            if (vec_out && col + EPS <= nvalid) {
+                *reinterpret_cast<uint4*>(dst) = val;
+            } else {
+                const uint32_t w[4] = {val.x, val.y, val.z, val.w};
+#pragma unroll
+                for (int e = 0; e < EPS; ++e)
+                    if (col + e < nvalid) {
+                        if constexpr (F32) reinterpret_cast<uint32_t*>(dst)[e] = w[e];
+                        else reinterpret_cast<uint16_t*>(dst)[e] = static_cast<uint16_t>(w[e >> 1] >> (16 * (e & 1)));
+                    }
+            }
+        }
+        __syncwarp();
     }
 }
 
@@ -87,6 +238,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     uint64_t* full = bars;                       // [kStages] TMA -> consumers
     uint64_t* empty = bars + kBarStages;         // [kStages] consumers (of both CTAs of a cluster) -> TMA
     uint64_t* bfull = empty + kBarStages;        // BS: the resident weight slice has landed
+    uint8_t* const epi = reinterpret_cast<uint8_t*>(bars) + 256;       // epilogue staging, kEpiBytes
     // BS smem map: [resident B: k_total chunks of BN x 64][A ring: bs_stages x 16 KB] ... barriers at the fixed ring budget
     const int nst = BS ? g.bs_stages : Cf::kStages;
     uint8_t* const sB_res = smem;
@@ -224,19 +376,14 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         const int cw = wg - 1;                        // rows 64 cw .. 64 cw + 63 of the tile
         const int lt = threadIdx.x & 127;
         const int wr = lt >> 5, lane = lt & 31;
-        const int quad = lane & 3;
         int stage = 0;
         uint32_t phase = 0;
         if constexpr (BS) {
             if (first_pair < total_items) mbar_wait(bfull, 0u);
         }
         const bool out_f32 = (g.flags & GEMM_OUT_F32) != 0;
-        const bool ln = (g.flags & GEMM_LN) != 0;
-        const int nvalid = GEGLU ? g.N / 2 : g.N;
-        // column pairs as one 4 / 8-byte access when every row segment starts at an even element
-        const bool pair_ok = ((g.ldo & 1) == 0) && ((reinterpret_cast<uintptr_t>(g.out) & (out_f32 ? 7 : 3)) == 0) &&
-                             ((g.split_stride & 1) == 0) &&
-                             (g.residual == nullptr || (((g.ldr & 1) == 0) && ((reinterpret_cast<uintptr_t>(g.residual) & 3) == 0)));
+        uint8_t* const stg = epi + (cw * 4 + wr) * kEpiWarpBytes;          // this warp's staging slab and row table
+        long long* const rowg = reinterpret_cast<long long*>(stg + 8 * kEpiRowBytes);
         float acc[BN / 2];
         for (int wi = first_pair; wi < total_items; wi += pair_stride) {
             const int sp = BS ? 0 : wi % nsplit;
@@ -259,7 +406,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < GEMM_BLOCK_K / 16; ++k)          // +32 B per K = 16 step (start address in 16 B units)
-                    mma_k16<BN>(acc, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), (it | k) != 0 ? 1u : 0u);
+                    wgmma_ss<BN>(acc, da + static_cast<uint64_t>(k * 2), db + static_cast<uint64_t>(k * 2), (it | k) != 0 ? 1u : 0u);
                 wgmma_commit();
                 wgmma_wait<1>();                                      // the previous stage's group has retired
                 if (prev >= 0 && lt == 0) {
@@ -280,109 +427,37 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 if constexpr (CG == 2) mbar_arrive_cluster(&empty[prev], rank ^ 1u);
             }
 
-            // ---- epilogue: this thread holds rows r0, r0 + 8 and, per 8-column group j, columns 8j + 2 quad + {0, 1}
-            const int r0 = cw * 64 + wr * 16 + (lane >> 2);
-            int tm_org[GEMM_MAX_RDIMS] = {0, 0, 0, 0};
-            if (g.nd > 1) {
-                int tm = tmi;
+            // ---- epilogue: global row of each of this warp's 16 rows (-1: outside the problem), then the staged stores
+            if (lane < 16) {
+                const int r = cw * 64 + wr * 16 + lane;
+                long long grow = -1;
+                if (tmi < g.tiles_m) {
+                    if (g.nd == 1) {                       // plain row matrix: no div/mod chain
+                        const int o = tmi * g.box[0];
+                        if (r < g.box[0] && o + r < g.dim[0]) grow = o + r;
+                    } else {
+                        int tm = tmi, rr = r;
+                        long long mul = 1, gr = 0;
+                        bool valid = true;
 #pragma unroll
-                for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
-                    const int td = g.tdim[d];
-                    tm_org[d] = (tm % td) * g.box[d];
-                    tm /= td;
-                }
-            }
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int r = r0 + 8 * h;
-                long long grow = 0;
-                bool valid = tmi < g.tiles_m;
-                if (g.nd == 1) {                       // plain row matrix: no div/mod chain
-                    const int o = tmi * g.box[0];
-                    valid = valid && (r < g.box[0]) && (o + r < g.dim[0]);
-                    grow = o + r;
-                } else {
-                    int rr = r;
-                    long long mul = 1;
-#pragma unroll
-                    for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
-                        const int i = rr % g.box[d];
-                        rr /= g.box[d];
-                        const int c = tm_org[d] + i;
-                        valid = valid && (c < g.dim[d]);
-                        grow += mul * c;
-                        mul *= g.dim[d];
-                    }
-                    valid = valid && (rr == 0);
-                }
-                if (!valid) continue;
-                const __half* bias = g.bias;
-                if (bias != nullptr && g.bias_rows > 0) bias += (grow / g.bias_rows) * g.bias_stride;
-                float2 rs = make_float2(0.f, 1.f);                    // (mean, rstd) of this row
-                if (ln) rs = __ldg(g.rowstat + grow);
-                // accumulator -> alpha / LayerNorm fold -> + bias, for packed column pcol
-                auto affine = [&](float v, int pcol) {
-                    if (ln) return fmaf(rs.y, fmaf(-rs.x, __ldg(g.colsum + pcol), v), __ldg(g.bias32 + pcol));
-                    return fmaf(v, g.alpha, bias != nullptr ? __half2float(__ldg(bias + pcol)) : 0.f);
-                };
-                if constexpr (GEGLU) {
-                    // out = fp16(value) * fp16(gelu(fp16(gate))) with the reference's fp16 rounding points (t2v_model.py:819-821
-                    // under autocast: proj output, gelu output, product).  Value column c and gate column BN/2 + c of the tile
-                    // sit BN/4 registers apart; gemm_plan guarantees N % BN == 0 and 32 B aligned fp16 rows.
-                    __half* orow = reinterpret_cast<__half*>(g.out) + grow * g.ldo + tn * (BN / 2);
-#pragma unroll
-                    for (int j = 0; j < BN / 16; ++j) {
-                        const int c = 8 * j + 2 * quad;
-                        const int pc = tn * BN + c;
-                        const float x0 = affine(acc[4 * j + 2 * h], pc), x1 = affine(acc[4 * j + 2 * h + 1], pc + 1);
-                        const float g0 = affine(acc[BN / 4 + 4 * j + 2 * h], pc + BN / 2);
-                        const float g1 = affine(acc[BN / 4 + 4 * j + 2 * h + 1], pc + BN / 2 + 1);
-                        const __half2 xh = __floats2half2_rn(x0, x1);
-                        const float2 gf = __half22float2(__floats2half2_rn(g0, g1));
-                        const __half2 ge = __floats2half2_rn(gelu_erf(gf.x), gelu_erf(gf.y));
-                        *reinterpret_cast<__half2*>(orow + c) = __hmul2(xh, ge);     // fp16 x fp16 -> fp16 (RN)
-                    }
-                } else {
-                    const int ocol0 = tn * BN;
-                    const __half* res_row = g.residual != nullptr ? g.residual + grow * g.ldr + ocol0 : nullptr;
-#pragma unroll
-                    for (int j = 0; j < BN / 8; ++j) {
-                        const int c = 8 * j + 2 * quad;
-                        const int col = ocol0 + c;
-                        if (col >= nvalid) continue;
-                        const bool two = col + 1 < nvalid;
-                        float v0 = affine(acc[4 * j + 2 * h], col);
-                        float v1 = two ? affine(acc[4 * j + 2 * h + 1], col + 1) : 0.f;
-                        if (res_row != nullptr) {
-                            if (two && pair_ok) {
-                                const float2 f = __half22float2(__ldg(reinterpret_cast<const __half2*>(res_row + c)));
-                                v0 += f.x;
-                                v1 += f.y;
-                            } else {
-                                v0 += __half2float(res_row[c]);
-                                if (two) v1 += __half2float(res_row[c + 1]);
-                            }
+                        for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
+                            const int td = g.tdim[d];
+                            const int c = (tm % td) * g.box[d] + rr % g.box[d];
+                            tm /= td;
+                            rr /= g.box[d];
+                            valid = valid && (c < g.dim[d]);
+                            gr += mul * c;
+                            mul *= g.dim[d];
                         }
-                        if (out_f32) {
-                            float* op = reinterpret_cast<float*>(g.out) + sp * g.split_stride + grow * g.ldo + col;
-                            if (two && pair_ok) {
-                                *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
-                            } else {
-                                op[0] = v0;
-                                if (two) op[1] = v1;
-                            }
-                        } else {
-                            __half* op = reinterpret_cast<__half*>(g.out) + grow * g.ldo + col;
-                            if (two && pair_ok) {
-                                *reinterpret_cast<__half2*>(op) = __floats2half2_rn(v0, v1);
-                            } else {
-                                op[0] = __float2half_rn(v0);
-                                if (two) op[1] = __float2half_rn(v1);
-                            }
-                        }
+                        if (valid && rr == 0) grow = gr;
                     }
                 }
+                rowg[lane] = grow;
             }
+            __syncwarp();
+            if constexpr (GEGLU) epilogue_warp<BN, true, false>(g, acc, stg, rowg, tn, sp, lane);
+            else if (out_f32) epilogue_warp<BN, false, true>(g, acc, stg, rowg, tn, sp, lane);
+            else epilogue_warp<BN, false, false>(g, acc, stg, rowg, tn, sp, lane);
         }
     }
     if constexpr (CG == 2) cluster_sync_all();    // no CTA may exit while its peer can still multicast into it or signal it
@@ -646,6 +721,10 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
     plan->cg = p.force_cg ? p.force_cg : ((g.tiles_m >= 2 && bn >= 64 && use_pairs) ? 2 : 1);
     if (bn < 64 || p.b_batch_dim >= 0 || plan->bs || bn == 192 || bn == 224) plan->cg = 1;     // a cluster shares ONE B tile: never across B batches
     g.tiles_n = (p.N + bn - 1) / bn;
+    if ((p.flags & GEMM_OUT_F32) && p.residual != nullptr) {
+        fprintf(stderr, "[t2v] gemm_plan: fp32 output takes no residual\n");
+        return -4;
+    }
     if ((p.flags & GEMM_GEGLU) && (p.N % bn) != 0) {
         fprintf(stderr, "[t2v] gemm_plan: GEGLU needs N %% BN == 0 (N %d BN %d)\n", p.N, bn);
         return -4;

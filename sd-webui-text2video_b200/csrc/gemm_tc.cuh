@@ -22,7 +22,7 @@ constexpr int GEMM_MAX_RDIMS = 4;
 
 enum GemmFlags : int {
     GEMM_GEGLU = 1,        // epilogue: out[:, j] = (acc[:, j] + b) * gelu(acc[:, BN/2 + j] + b)  (weights interleaved per tile)
-    GEMM_OUT_F32 = 2,      // store fp32 instead of fp16
+    GEMM_OUT_F32 = 2,      // store fp32 instead of fp16 (no residual)
     GEMM_LN = 4,           // LayerNorm of the A rows folded into the epilogue: out = rstd_r * (acc - mean_r * colsum_n) + bias32_n
                            //   (weights pre-scaled by gamma; colsum_n = sum_k W'[n,k]; bias32_n = sum_k W[n,k] beta_k + bias_n)
     // switches of t2v_op_gemm (never set by the model code)
