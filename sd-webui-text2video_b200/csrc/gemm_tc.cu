@@ -2,12 +2,16 @@
 //
 // Per CTA (persistent, 384 threads = 3 warpgroups, 1 CTA/SM):
 //   warpgroup 0     TMA producer : one elected thread issues, per k-iteration, one A box (128 rows x 64 K, tap-shifted
-//                                  coordinates, OOB = zero padding) + one B box (BN x 64 K) into a SWIZZLE_128B smem ring
+//                                  coordinates, OOB = zero padding) + one B box (BN x 64 K) into a SWIZZLE_128B smem ring;
+//                                  warp 1 copies each tile's per-column epilogue operands (bias, or the LayerNorm fold's
+//                                  colsum / bias32) into shared memory
 //   warpgroups 1, 2 consumers    : each owns 64 rows of the 128-row tile; per ring stage 4 k-steps of wgmma m64 x BN x 16
 //                                  (both operands from shared memory) into fp32 registers, then the epilogue (alpha, bias,
 //                                  LayerNorm fold, residual, GEGLU) through a per-warp shared-memory staging slab, so that
 //                                  global loads and stores are 16 B per thread over whole 128 B row segments.
-// The producer runs ahead into the next tile while the consumers are in the epilogue.
+// The producer runs ahead into the next tile while the consumers are in the epilogue.  What the epilogue needs besides the
+// accumulators is fetched before they are ready: the row table and LayerNorm row statistics at tile start, the column
+// operands by warp 1, the first residual units while the tile's last MMAs run.
 // CG = 2: a cluster of two CTAs owns two consecutive M-tiles of the same N-tile; each CTA fetches half of the B box and
 // TMA-multicasts it into both CTAs, so B crosses L2 -> SM once per pair.
 // Roofline: tensor-bound (2*M*N*K*taps flop per launch) whenever K*taps is large; see DESIGN.md.
@@ -31,9 +35,11 @@ constexpr int kABytes = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;     // 16 KB
 constexpr int kSmemBudget = 216 * 1024;                      // ring (barriers + alignment slack on top; 227 KB per block)
 constexpr int kMaxStages = 8;
 // Epilogue staging, per consumer warp: 8 rows x 128 B (half of the warp's 16 rows at a time) + the global row index of each of
-// its 16 rows.  It sits outside the ring budget, in what the 227 KB per block leaves over, so no ring loses a stage.
+// its 16 rows (32-bit: gemm_plan rejects problems of 2^31 rows or more).  Behind the 8 slabs, the tile's per-column epilogue
+// operands, BN x 8 B.  All of it sits outside the ring budget, in what the 227 KB per block leaves over, so no ring loses a
+// stage (BN = 160: 768 B spare before the column buffer, which the 32-bit row table makes room for).
 constexpr int kEpiRowBytes = 128;
-constexpr int kEpiWarpBytes = 8 * kEpiRowBytes + 16 * 8;
+constexpr int kEpiWarpBytes = 8 * kEpiRowBytes + 16 * 4;
 constexpr int kEpiBytes = 8 * kEpiWarpBytes;
 
 template <int BN>
@@ -41,11 +47,12 @@ struct Cfg {
     static constexpr int kBBytes = BN * GEMM_BLOCK_K * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
     static constexpr int kStages = (kSmemBudget / kStageBytes) > kMaxStages ? kMaxStages : (kSmemBudget / kStageBytes);
-    static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + kEpiBytes;
+    static constexpr int kColBytes = BN * 8;      // (colsum, bias32) fp32 pairs, or the fp16 bias
+    static constexpr int kTailBytes = 1024 /*align slack*/ + 256 /*barriers*/ + kEpiBytes + kColBytes;
+    static constexpr int kSmemBytes = kStages * kStageBytes + kTailBytes;
+    static constexpr int kBsSmemBytes = kSmemBudget + kTailBytes;      // B-stationary: resident weights + A ring fill the budget
     static_assert(kSmemBytes <= 227 * 1024, "shared memory per block");
 };
-constexpr int kBsSmemBytes = kSmemBudget + 1024 + 256 + kEpiBytes;      // B-stationary: resident weights + A ring fill the budget
-static_assert(kBsSmemBytes <= 227 * 1024, "shared memory per block");
 
 // erf-form GELU x * Phi(x) (F.gelu default, t2v_model.py:821).  Phi(x) = 1/2 erfc(-x / sqrt 2); for z = |x| / sqrt 2
 // erfc(z) = t (a1 + t (a2 + t (a3 + t (a4 + t a5)))) exp(-z^2), t = 1 / (1 + p z) (Abramowitz-Stegun 7.1.26, |error| <=
@@ -71,105 +78,128 @@ __device__ __forceinline__ uint32_t stg_off(int r, int b, int segs) {
     return static_cast<uint32_t>(((L ^ ((L >> 3) & 7)) << 4) | (b & 15));
 }
 
-// Epilogue of one warp: its 16 rows x BN accumulator columns (fragment layout, ptx.cuh) -> global memory.
-//   1. in place on the accumulators: alpha + bias, or the LayerNorm fold; bias / colsum / bias32 loaded once per column
-//   2. per unit (chunk of 128 B of output per row, half h = rows 8h .. 8h + 7): the residual slice is loaded with 16 B reads
-//      (issued one unit ahead) into the staging slab; each thread adds it to its fragment values, rounds, and writes the
-//      result back to the same place; then the rows leave with 16 B stores.
+// Step 1 of a warp's epilogue, in place on its accumulators (fragment layout, ptx.cuh): alpha + bias, or the LayerNorm fold
+// (rs: (mean, rstd) of rows fr and fr + 8).  The tile's per-column operands come from `cols`, which the producer warpgroup
+// filled (zero past N): (colsum, bias32) fp32 pairs with the fold, else the fp16 bias.  A per-sample bias (bias_rows > 0,
+// where one tile's rows may fall into two samples) is read from global memory instead.
+template <int BN, bool GEGLU>
+__device__ __forceinline__ void epilogue_affine(const GemmDesc& g, float (&acc)[BN / 2], const uint8_t* cols, const int* rowg,
+                                                const float2 (&rs)[2], int tn, int lane) {
+    const int quad = lane & 3, fr = lane >> 2;           // fragment: rows fr, fr + 8; columns 8j + 2 quad + {0, 1}
+    if (g.bias != nullptr && g.bias_rows > 0 && (g.flags & GEMM_LN) == 0) {
+        const int nvalid = GEGLU ? g.N / 2 : g.N;
+        const __half* brow[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int fg = rowg[fr + 8 * h];
+            brow[h] = g.bias + (fg >= 0 ? (fg / g.bias_rows) * g.bias_stride : 0);
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int col = tn * BN + 8 * j + 2 * quad + e;              // packed accumulator column
+                if (!GEGLU && col >= nvalid) continue;
+                acc[4 * j + e] = fmaf(acc[4 * j + e], g.alpha, __half2float(__ldg(brow[0] + col)));
+                acc[4 * j + 2 + e] = fmaf(acc[4 * j + 2 + e], g.alpha, __half2float(__ldg(brow[1] + col)));
+            }
+        }
+        return;
+    }
+    const bool ln = (g.flags & GEMM_LN) != 0;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + 2 * quad;                      // tile column of acc[4j], acc[4j + 2]; c + 1: acc[4j + 1], acc[4j + 3]
+        if (ln) {
+            const float4 p = *reinterpret_cast<const float4*>(cols + 8 * c);      // colsum, bias32 of c; colsum, bias32 of c + 1
+            acc[4 * j] = fmaf(rs[0].y, fmaf(-rs[0].x, p.x, acc[4 * j]), p.y);
+            acc[4 * j + 2] = fmaf(rs[1].y, fmaf(-rs[1].x, p.x, acc[4 * j + 2]), p.y);
+            acc[4 * j + 1] = fmaf(rs[0].y, fmaf(-rs[0].x, p.z, acc[4 * j + 1]), p.w);
+            acc[4 * j + 3] = fmaf(rs[1].y, fmaf(-rs[1].x, p.z, acc[4 * j + 3]), p.w);
+        } else {
+            const float2 b = __half22float2(*reinterpret_cast<const __half2*>(cols + 2 * c));
+            acc[4 * j] = fmaf(acc[4 * j], g.alpha, b.x);
+            acc[4 * j + 2] = fmaf(acc[4 * j + 2], g.alpha, b.x);
+            acc[4 * j + 1] = fmaf(acc[4 * j + 1], g.alpha, b.y);
+            acc[4 * j + 3] = fmaf(acc[4 * j + 3], g.alpha, b.y);
+        }
+    }
+}
+
+// Residual of the fp16 epilogue, unit by unit (a unit = 128 B of output per row for 8 rows: chunk u / 2, rows 8 (u % 2) ..
+// 8 (u % 2) + 7), in the row-side layout of the staging slab: 16 B per thread.  kResUnits units of a tile are in flight at
+// a time; the first ones are issued while the tile's last MMAs run.  BN <= 192: the warp's whole slice (<= 12 x 16 B per
+// thread); wider tiles keep four units in flight, which fits their register budget without spills.
+template <int BN>
+struct ResQ {
+    static constexpr int kCW = kEpiRowBytes / 2;                       // output columns per unit
+    static constexpr int kUnits = 2 * ((BN + kCW - 1) / kCW);
+    static constexpr int kDepth = BN <= 192 ? kUnits : 4;
+    static __device__ __forceinline__ int segs(int c) { return (min(kCW, BN - c * kCW) * 2) / 16; }
+    static __device__ __forceinline__ void load(const GemmDesc& g, const int* rowg, int tn, int u, int lane, uint4 (&rb)[2]) {
+        const int c = u >> 1, h = u & 1, sg = segs(c);
+        const bool vec_res = (g.ldr & 7) == 0 && (reinterpret_cast<uintptr_t>(g.residual) & 15) == 0;
+#pragma unroll
+        for (int p = 0; p < 2; ++p) {
+            const int idx = lane + 32 * p;
+            rb[p] = make_uint4(0u, 0u, 0u, 0u);
+            if (idx >= 8 * sg) continue;
+            const int gr = rowg[8 * h + idx / sg];
+            const int col = tn * BN + c * kCW + 8 * (idx % sg);
+            if (gr < 0) continue;
+            const __half* src = g.residual + gr * g.ldr + col;
+            if (vec_res && col + 8 <= g.N) {
+                rb[p] = __ldg(reinterpret_cast<const uint4*>(src));
+            } else {
+                uint32_t w[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const __half2 v = __halves2half2(col + 2 * e < g.N ? src[2 * e] : __ushort_as_half(0),
+                                                     col + 2 * e + 1 < g.N ? src[2 * e + 1] : __ushort_as_half(0));
+                    w[e] = *reinterpret_cast<const uint32_t*>(&v);
+                }
+                rb[p] = make_uint4(w[0], w[1], w[2], w[3]);
+            }
+        }
+    }
+};
+
+// Step 2 of a warp's epilogue: its 16 rows x BN accumulator columns -> global memory, per unit (chunk of 128 B of output per
+// row, half h = rows 8h .. 8h + 7).  The residual slice (queued in rq, ResQ) goes into the staging slab; each thread adds it
+// to its fragment values, rounds, and writes the result back to the same place; then the rows leave with 16 B stores.
 // Per element the arithmetic is that of a direct store: fp32 affine, + residual in fp32, one rounding (GEGLU: fp16 value,
 // fp16 gate, fp16 gelu, fp16 product).  fp32 output (split-K partials) stages 32 columns per unit and has no residual
-// (gemm_plan).  A segment that is cut by N, or an unaligned output / residual, goes element-wise.
+// (gemm_plan), nor has GEGLU.  A segment that is cut by N, or an unaligned output / residual, goes element-wise.
 // rowg[16]: global row of each of the warp's rows, -1 for rows outside the problem.
 template <int BN, bool GEGLU, bool F32>
-__device__ __forceinline__ void epilogue_warp(const GemmDesc& g, float (&acc)[BN / 2], uint8_t* stg, const long long* rowg,
-                                              int tn, int sp, int lane) {
+__device__ __forceinline__ void epilogue_warp(const GemmDesc& g, float (&acc)[BN / 2], uint4 (&rq)[ResQ<BN>::kDepth][2],
+                                              uint8_t* stg, const int* rowg, int tn, int sp, int lane) {
     static_assert(!(GEGLU && F32), "GEGLU stores fp16");
+    constexpr bool RES = !GEGLU && !F32;                 // the variants that may add a residual
     constexpr int ES = F32 ? 4 : 2;                      // output element bytes
     constexpr int EPS = 16 / ES;                         // elements per 16 B segment
     constexpr int OUTW = GEGLU ? BN / 2 : BN;            // output columns of the tile
     constexpr int CW = kEpiRowBytes / ES;                // output columns per unit
     constexpr int NCH = (OUTW + CW - 1) / CW;
     constexpr int NU = 2 * NCH;                          // units: (chunk u / 2, half u % 2)
+    constexpr int QD = ResQ<BN>::kDepth;
     const int quad = lane & 3, fr = lane >> 2;           // fragment: rows fr, fr + 8; columns 8j + 2 quad + {0, 1}
     const int nvalid = GEGLU ? g.N / 2 : g.N;
     const int ocol0 = tn * OUTW;
-    const bool ln = (g.flags & GEMM_LN) != 0;
-    const bool has_res = g.residual != nullptr;
+    const bool has_res = RES && g.residual != nullptr;
     const bool vec_out = (g.ldo % EPS) == 0 && (reinterpret_cast<uintptr_t>(g.out) & 15) == 0 && (!F32 || (g.split_stride % EPS) == 0);
-    const bool vec_res = has_res && (g.ldr & 7) == 0 && (reinterpret_cast<uintptr_t>(g.residual) & 15) == 0;
 
-    // ---- 1. affine, in place
-    long long fg[2];
-    float2 rs[2];
-    const __half* brow[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        fg[h] = rowg[fr + 8 * h];
-        rs[h] = (ln && fg[h] >= 0) ? __ldg(g.rowstat + fg[h]) : make_float2(0.f, 1.f);      // (mean, rstd) of the row
-        brow[h] = g.bias;
-        if (g.bias != nullptr && g.bias_rows > 0 && fg[h] >= 0) brow[h] += (fg[h] / g.bias_rows) * g.bias_stride;
-    }
-    const bool row_bias = g.bias != nullptr && g.bias_rows > 0;
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            const int col = tn * BN + 8 * j + 2 * quad + e;                  // packed accumulator column
-            if (!GEGLU && col >= nvalid) continue;
-            float& v0 = acc[4 * j + e];
-            float& v1 = acc[4 * j + 2 + e];
-            if (ln) {
-                const float cs = __ldg(g.colsum + col), b32 = __ldg(g.bias32 + col);
-                v0 = fmaf(rs[0].y, fmaf(-rs[0].x, cs, v0), b32);
-                v1 = fmaf(rs[1].y, fmaf(-rs[1].x, cs, v1), b32);
-            } else {
-                const float b0 = brow[0] != nullptr ? __half2float(__ldg(brow[0] + col)) : 0.f;
-                const float b1 = row_bias ? __half2float(__ldg(brow[1] + col)) : b0;
-                v0 = fmaf(v0, g.alpha, b0);
-                v1 = fmaf(v1, g.alpha, b1);
-            }
-        }
-    }
-
-    // ---- 2. staged stores
     auto segs_of = [](int c) { return (min(CW, OUTW - c * CW) * ES) / 16; };
-    auto load_res = [&](int u, uint4 (&rb)[2]) {          // fp16 residual of unit u, row-side layout
-        const int c = u >> 1, h = u & 1, segs = segs_of(c);
-#pragma unroll
-        for (int p = 0; p < 2; ++p) {
-            const int idx = lane + 32 * p;
-            rb[p] = make_uint4(0u, 0u, 0u, 0u);
-            if (idx >= 8 * segs) continue;
-            const long long gr = rowg[8 * h + idx / segs];
-            const int col = ocol0 + c * CW + 8 * (idx % segs);
-            if (gr < 0) continue;
-            const __half* src = g.residual + gr * g.ldr + col;
-            if (vec_res && col + 8 <= nvalid) {
-                rb[p] = __ldg(reinterpret_cast<const uint4*>(src));
-            } else {
-                uint32_t w[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const __half2 v = __halves2half2(col + 2 * e < nvalid ? src[2 * e] : __ushort_as_half(0),
-                                                     col + 2 * e + 1 < nvalid ? src[2 * e + 1] : __ushort_as_half(0));
-                    w[e] = *reinterpret_cast<const uint32_t*>(&v);
-                }
-                rb[p] = make_uint4(w[0], w[1], w[2], w[3]);
-            }
-        }
-    };
-    uint4 rbuf[2][2];
-    if (!F32 && has_res) load_res(0, rbuf[0]);
 #pragma unroll
     for (int u = 0; u < NU; ++u) {
         const int c = u >> 1, h = u & 1, segs = segs_of(c);
-        if (!F32 && has_res) {
+        if (RES && has_res) {
 #pragma unroll
             for (int p = 0; p < 2; ++p) {
                 const int idx = lane + 32 * p;
-                if (idx < 8 * segs) *reinterpret_cast<uint4*>(stg + stg_off(idx / segs, 16 * (idx % segs), segs)) = rbuf[u & 1][p];
+                if (idx < 8 * segs) *reinterpret_cast<uint4*>(stg + stg_off(idx / segs, 16 * (idx % segs), segs)) = rq[u % QD][p];
             }
-            if (u + 1 < NU) load_res(u + 1, rbuf[(u + 1) & 1]);
+            if (u + QD < NU) ResQ<BN>::load(g, rowg, tn, u + QD, lane, rq[u % QD]);
             __syncwarp();
         }
         // fragment side: row fr of this half, the chunk's columns
@@ -202,7 +232,7 @@ __device__ __forceinline__ void epilogue_warp(const GemmDesc& g, float (&acc)[BN
         for (int p = 0; p < 2; ++p) {
             const int idx = lane + 32 * p;
             if (idx >= 8 * segs) continue;
-            const long long gr = rowg[8 * h + idx / segs];
+            const int gr = rowg[8 * h + idx / segs];
             if (gr < 0) continue;
             const int col = ocol0 + c * CW + EPS * (idx % segs);
             const uint4 val = *reinterpret_cast<const uint4*>(stg + stg_off(idx / segs, 16 * (idx % segs), segs));
@@ -229,6 +259,7 @@ template <int BN, bool GEGLU, int CG, bool BS = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmDesc g) {
     using Cf = Cfg<BN>;
     static_assert(!BS || CG == 1, "B-stationary tiles are single-CTA");
+    static_assert(!BS || Cf::kBsSmemBytes <= 227 * 1024, "shared memory per block");
     constexpr int kBarStages = BS ? kMaxStages : Cf::kStages;      // barrier slots (BS: ring depth is a run-time value <= 8)
     const uint32_t rank = CG == 2 ? cluster_ctarank() : 0u;       // position in the cluster
     extern __shared__ uint8_t smem_raw[];
@@ -238,7 +269,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     uint64_t* full = bars;                       // [kStages] TMA -> consumers
     uint64_t* empty = bars + kBarStages;         // [kStages] consumers (of both CTAs of a cluster) -> TMA
     uint64_t* bfull = empty + kBarStages;        // BS: the resident weight slice has landed
+    uint64_t* colfull = bfull + 1;               // column operands of the next tile are in `cols` (warp 1 -> consumers)
+    uint64_t* colempty = bfull + 2;              // every consumer warp has read them (consumers -> warp 1)
     uint8_t* const epi = reinterpret_cast<uint8_t*>(bars) + 256;       // epilogue staging, kEpiBytes
+    uint8_t* const cols = epi + kEpiBytes;                             // per-column epilogue operands, Cf::kColBytes
     // BS smem map: [resident B: k_total chunks of BN x 64][A ring: bs_stages x 16 KB] ... barriers at the fixed ring budget
     const int nst = BS ? g.bs_stages : Cf::kStages;
     uint8_t* const sB_res = smem;
@@ -254,6 +288,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             mbar_init(&empty[i], 2 * CG);         // one arrival per consumer warpgroup of every CTA that writes this stage
         }
         if constexpr (BS) mbar_init(bfull, 1);
+        mbar_init(colfull, 1);
+        mbar_init(colempty, 8);                   // one arrival per consumer warp
         fence_barrier_init();
     }
     if constexpr (CG == 2) cluster_sync_all();    // peer barriers are initialised before any multicast / remote arrive
@@ -271,6 +307,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     const int first_pair = BS ? static_cast<int>(blockIdx.x) / g.tiles_n : static_cast<int>(blockIdx.x) / CG;
     const int pair_stride = BS ? (static_cast<int>(gridDim.x) - bs_tn + g.tiles_n - 1) / g.tiles_n : static_cast<int>(gridDim.x) / CG;
     const int total_items = BS ? g.tiles_m : total_pairs;
+    // the per-column epilogue operands go through shared memory unless the bias is per sample (epilogue_affine)
+    const bool col_operands = (g.flags & GEMM_LN) != 0 || g.bias == nullptr || g.bias_rows == 0;
 
     if (wg == 0) {
         // ------------------------------------------------------------------ TMA producer
@@ -368,6 +406,30 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             }
             // nothing left to fetch: let the next kernel's CTAs be scheduled as SMs drain (PDL)
             griddep_launch();
+        } else if (threadIdx.x >= 32 && threadIdx.x < 64 && col_operands) {
+            // Warp 1: the per-column epilogue operands of each tile into `cols`, zero past N.  The consumers release the buffer
+            // after step 1 of their epilogue, so the next tile's columns load during the rest of that epilogue and the next
+            // main loop, off the consumers' path.
+            const int lane = threadIdx.x & 31;
+            const bool ln = (g.flags & GEMM_LN) != 0;
+            uint32_t cphase = 0;
+            for (int wi = first_pair; wi < total_items; wi += pair_stride) {
+                const int col0 = (BS ? bs_tn : (wi / nsplit) % g.tiles_n) * BN;
+                mbar_wait(colempty, cphase ^ 1u);
+#pragma unroll
+                for (int c = lane; c < BN; c += 32) {
+                    const int col = col0 + c;
+                    if (ln) {
+                        reinterpret_cast<float2*>(cols)[c] =
+                            col < g.N ? make_float2(__ldg(g.colsum + col), __ldg(g.bias32 + col)) : make_float2(0.f, 0.f);
+                    } else {
+                        reinterpret_cast<__half*>(cols)[c] = g.bias != nullptr && col < g.N ? __ldg(g.bias + col) : __ushort_as_half(0);
+                    }
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(colfull);
+                cphase ^= 1u;
+            }
         }
         __syncwarp();
     } else {
@@ -382,9 +444,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             if (first_pair < total_items) mbar_wait(bfull, 0u);
         }
         const bool out_f32 = (g.flags & GEMM_OUT_F32) != 0;
+        const bool ln = (g.flags & GEMM_LN) != 0;
         uint8_t* const stg = epi + (cw * 4 + wr) * kEpiWarpBytes;          // this warp's staging slab and row table
-        long long* const rowg = reinterpret_cast<long long*>(stg + 8 * kEpiRowBytes);
+        int* const rowg = reinterpret_cast<int*>(stg + 8 * kEpiRowBytes);
+        uint32_t cphase = 0;
         float acc[BN / 2];
+        uint4 rq[ResQ<BN>::kDepth][2];
         for (int wi = first_pair; wi < total_items; wi += pair_stride) {
             const int sp = BS ? 0 : wi % nsplit;
             const int pt = wi / nsplit;
@@ -392,6 +457,43 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             const int tmi = BS ? wi : (pt / g.tiles_n) * CG + static_cast<int>(rank);
             const int it0s = BS ? 0 : sp * k_per;
             const int k_iters = min(k_total, it0s + k_per) - it0s;
+
+            // ---- global row of each of this warp's 16 rows (-1: outside the problem) and the LayerNorm (mean, rstd) of the
+            // thread's two fragment rows.  Both depend on the tile index only, so they are fetched before the main loop (the
+            // previous tile's epilogue, which read the table, ended with __syncwarp).
+            if (lane < 16) {
+                const int r = cw * 64 + wr * 16 + lane;
+                int grow = -1;
+                if (tmi < g.tiles_m) {
+                    if (g.nd == 1) {                       // plain row matrix: no div/mod chain
+                        const int o = tmi * g.box[0];
+                        if (r < g.box[0] && o + r < g.dim[0]) grow = o + r;
+                    } else {
+                        int tm = tmi, rr = r;
+                        long long mul = 1, gr = 0;
+                        bool valid = true;
+#pragma unroll
+                        for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
+                            const int td = g.tdim[d];
+                            const int c = (tm % td) * g.box[d] + rr % g.box[d];
+                            tm /= td;
+                            rr /= g.box[d];
+                            valid = valid && (c < g.dim[d]);
+                            gr += mul * c;
+                            mul *= g.dim[d];
+                        }
+                        if (valid && rr == 0) grow = static_cast<int>(gr);
+                    }
+                }
+                rowg[lane] = grow;
+            }
+            __syncwarp();
+            float2 rs[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int fg = rowg[(lane >> 2) + 8 * h];
+                rs[h] = ln && fg >= 0 ? __ldg(g.rowstat + fg) : make_float2(0.f, 1.f);
+            }
 
             // ---- main loop: one ring stage per iteration, one wgmma group kept in flight
             int prev = -1;
@@ -419,6 +521,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                     phase ^= 1u;
                 }
             }
+            // the first residual units are in flight while the last MMAs run
+            if constexpr (!GEGLU) {
+                if (g.residual != nullptr) {
+#pragma unroll
+                    for (int u = 0; u < ResQ<BN>::kDepth; ++u) ResQ<BN>::load(g, rowg, tn, u, lane, rq[u]);
+                }
+            }
             wgmma_wait<0>();
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);       // epilogue reads stay behind the wait
@@ -427,37 +536,17 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 if constexpr (CG == 2) mbar_arrive_cluster(&empty[prev], rank ^ 1u);
             }
 
-            // ---- epilogue: global row of each of this warp's 16 rows (-1: outside the problem), then the staged stores
-            if (lane < 16) {
-                const int r = cw * 64 + wr * 16 + lane;
-                long long grow = -1;
-                if (tmi < g.tiles_m) {
-                    if (g.nd == 1) {                       // plain row matrix: no div/mod chain
-                        const int o = tmi * g.box[0];
-                        if (r < g.box[0] && o + r < g.dim[0]) grow = o + r;
-                    } else {
-                        int tm = tmi, rr = r;
-                        long long mul = 1, gr = 0;
-                        bool valid = true;
-#pragma unroll
-                        for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
-                            const int td = g.tdim[d];
-                            const int c = (tm % td) * g.box[d] + rr % g.box[d];
-                            tm /= td;
-                            rr /= g.box[d];
-                            valid = valid && (c < g.dim[d]);
-                            gr += mul * c;
-                            mul *= g.dim[d];
-                        }
-                        if (valid && rr == 0) grow = gr;
-                    }
-                }
-                rowg[lane] = grow;
+            // ---- epilogue: affine (column operands from `cols`, then the buffer goes back to warp 1), staged stores
+            if (col_operands) mbar_wait(colfull, cphase);
+            epilogue_affine<BN, GEGLU>(g, acc, cols, rowg, rs, tn, lane);
+            if (col_operands) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(colempty);
+                cphase ^= 1u;
             }
-            __syncwarp();
-            if constexpr (GEGLU) epilogue_warp<BN, true, false>(g, acc, stg, rowg, tn, sp, lane);
-            else if (out_f32) epilogue_warp<BN, false, true>(g, acc, stg, rowg, tn, sp, lane);
-            else epilogue_warp<BN, false, false>(g, acc, stg, rowg, tn, sp, lane);
+            if constexpr (GEGLU) epilogue_warp<BN, true, false>(g, acc, rq, stg, rowg, tn, sp, lane);
+            else if (out_f32) epilogue_warp<BN, false, true>(g, acc, rq, stg, rowg, tn, sp, lane);
+            else epilogue_warp<BN, false, false>(g, acc, rq, stg, rowg, tn, sp, lane);
         }
     }
     if constexpr (CG == 2) cluster_sync_all();    // no CTA may exit while its peer can still multicast into it or signal it
@@ -498,7 +587,7 @@ Variant variant() {
 }
 template <int BN, bool G>
 Variant variant_bs() {
-    return Variant{BN, G ? 1 : 0, 1, kBsSmemBytes, reinterpret_cast<const void*>(&gemm_tc_kernel<BN, G, 1, true>), 1};
+    return Variant{BN, G ? 1 : 0, 1, Cfg<BN>::kBsSmemBytes, reinterpret_cast<const void*>(&gemm_tc_kernel<BN, G, 1, true>), 1};
 }
 const Variant* variants(int* n) {
     static const Variant v[] = {
@@ -611,6 +700,10 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
         remaining = b >= ext ? remaining / b : 1;     // only grow into the next dim when this one is fully covered
         boxrows *= b;
         rows *= ext;
+    }
+    if (rows >= (1LL << 31)) {          // the epilogue's row table holds 32-bit row indices
+        fprintf(stderr, "[t2v] gemm_plan: %lld rows, at most 2^31 - 1\n", rows);
+        return -4;
     }
     if (p.b_batch_dim >= 0 && g.box[p.b_batch_dim] != 1) {
         // a tile may not straddle two B batches: shrink that dim's box to 1
