@@ -175,20 +175,30 @@ double t2v_vae_flops(t2v_vae* v, int nframes, int h, int w);
  * 23 of the 24 for layer = 'penultimate' -- then ln_final; no text projection).  Parameter names are open_clip's
  * (`token_embedding.weight`, `positional_embedding`, `transformer.resblocks.N.{ln_1,attn.in_proj_weight,attn.in_proj_bias,
  * attn.out_proj,ln_2,mlp.c_fc,mlp.c_proj}`, `ln_final`), i.e. the keys of open_clip_pytorch_model.bin without `visual.*`.
- * Prompt parsing / chunking / emphasis weights stay host Python (clip_hardcode.py:146-395).                      */
+ * Prompt parsing / chunking / emphasis weights stay host Python (clip_hardcode.py:146-395).
+ * arch = 1 is VideoCrafter's FrozenCLIPEmbedder (videocrafter/lvdm/models/modules/condition_modules.py:15-40): the
+ * OpenAI CLIP ViT-L/14 text model as transformers' CLIPTextModel computes `last_hidden_state` (all layers, then
+ * final_layer_norm; quick_gelu MLP; causal mask only, no padding mask).                                          */
 typedef struct t2v_clip t2v_clip;
 typedef struct {
-    int width;          /* 1024 */
-    int heads;          /* 16 (head width must be 64) */
-    int layers_run;     /* 23 = 24 resblocks, 'penultimate' */
+    int width;          /* 1024 (arch 1: 768) */
+    int heads;          /* 16 (head width must be 64; arch 1: 12) */
+    int layers_run;     /* 23 = 24 resblocks, 'penultimate' (arch 1: 12, every layer) */
     int context;        /* 77 */
     int vocab;          /* 49408 */
+    int arch;           /* 0: OpenCLIP ViT-H-14 text tower, names above
+                         * 1: transformers CLIPTextModel (ViT-L/14), state_dict keys relative to the CLIPTextModel:
+                         *    `text_model.embeddings.{token_embedding,position_embedding}.weight`,
+                         *    `text_model.encoder.layers.N.{layer_norm1,self_attn.{q,k,v,out}_proj,layer_norm2,mlp.fc1,
+                         *    mlp.fc2}.{weight,bias}`, `text_model.final_layer_norm.{weight,bias}`; q / k / v are fused into
+                         *    one projection inside the library.  A zero-initialised config is arch 0. */
 } t2v_clip_config;
 int t2v_clip_create(const t2v_clip_config* cfg, t2v_clip** out);
 void t2v_clip_destroy(t2v_clip* m);
 int t2v_clip_set_param(t2v_clip* m, const char* name, const void* data, int dtype, int ndim, const int64_t* shape, void* stream);
 int t2v_clip_param_info(t2v_clip* m, int index, char* name_out, size_t name_cap, int64_t* shape_out, int* ndim_out);
-/* tokens [B, context] int32 (device) -> out [B, context, width] fp16 (out_is_f32 = 0) or fp32: ln_final(transformer(...)) */
+/* tokens [B, context] int32 (device) -> out [B, context, width] fp16 (out_is_f32 = 0) or fp32: ln_final(transformer(...))
+ * (arch 1: final_layer_norm(encoder(...)) = last_hidden_state) */
 int t2v_clip_encode(t2v_clip* m, const int* tokens, void* out, int out_is_f32, int B, void* stream);
 
 /* ------------------------------------------------------------------------------------------ sampler steps

@@ -8,6 +8,11 @@
 //
 // Same engine as the denoiser: LayerNorm folded into the consuming wgmma GEMM, residual adds in the GEMM epilogue; the
 // 77-token causal attention and the GELU are small dedicated kernels (the tower runs once per prompt: 2 x 77 rows).
+//
+// arch = 1 is the OpenAI CLIP ViT-L/14 text model of VideoCrafter's FrozenCLIPEmbedder (videocrafter/lvdm/models/modules/
+// condition_modules.py:15-40: transformers' CLIPTextModel, `last_hidden_state`).  Same block structure with transformers'
+// parameter names, separate q / k / v projections (fused here into one [q|k|v] weight and bias, so the block keeps one
+// LayerNorm-folded projection GEMM), quick_gelu instead of GELU, every layer, then final_layer_norm.
 #include "../../include/t2v_b200.h"
 #include "runtime.cuh"
 
@@ -66,6 +71,22 @@ __global__ void gelu_kernel(__half* __restrict__ x, long long n8) {
             const float2 f = __half22float2(h[k]);
             h[k] = __floats2half2_rn(0.5f * f.x * (1.0f + erff(f.x * 0.70710678118654752440f)),
                                      0.5f * f.y * (1.0f + erff(f.y * 0.70710678118654752440f)));
+        }
+        reinterpret_cast<uint4*>(x)[i] = v;
+    }
+}
+
+// y = x * sigmoid(1.702 x) (transformers' quick_gelu, CLIP ViT-L/14), in place on [rows, C] fp16; fp32 math, one rounding
+__global__ void quick_gelu_kernel(__half* __restrict__ x, long long n8) {
+    griddep_wait();
+    griddep_launch_small();
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n8; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        uint4 v = reinterpret_cast<uint4*>(x)[i];
+        __half2* h = reinterpret_cast<__half2*>(&v);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float2 f = __half22float2(h[k]);
+            h[k] = __floats2half2_rn(f.x / (1.0f + expf(-1.702f * f.x)), f.y / (1.0f + expf(-1.702f * f.y)));
         }
         reinterpret_cast<uint4*>(x)[i] = v;
     }
@@ -143,7 +164,41 @@ __global__ void __launch_bounds__(128) clip_attention_kernel(const __half* __res
     }
 }
 
+// arch 1: transformers CLIPTextModel names (relative to the CLIPTextModel)
+const char* const kHfEmb = "text_model.embeddings.token_embedding.weight";
+const char* const kHfPos = "text_model.embeddings.position_embedding.weight";
+const char* const kHfFinal = "text_model.final_layer_norm";
+std::string hf_layer(int i) { return "text_model.encoder.layers." + std::to_string(i); }
+
+void expect_params_hf(t2v_clip* m) {
+    ParamStore& P = m->params;
+    const t2v_clip_config& c = m->cfg;
+    P.expect(kHfEmb, {c.vocab, c.width});
+    P.expect(kHfPos, {c.context, c.width});
+    for (int i = 0; i < c.layers_run; ++i) {
+        const std::string p = hf_layer(i);
+        for (const char* ln : {".layer_norm1", ".layer_norm2"}) {
+            P.expect(p + ln + ".weight", {c.width});
+            P.expect(p + ln + ".bias", {c.width});
+        }
+        for (const char* proj : {".self_attn.q_proj", ".self_attn.k_proj", ".self_attn.v_proj", ".self_attn.out_proj"}) {
+            P.expect(p + proj + ".weight", {c.width, c.width});
+            P.expect(p + proj + ".bias", {c.width});
+        }
+        P.expect(p + ".mlp.fc1.weight", {4 * c.width, c.width});
+        P.expect(p + ".mlp.fc1.bias", {4 * c.width});
+        P.expect(p + ".mlp.fc2.weight", {c.width, 4 * c.width});
+        P.expect(p + ".mlp.fc2.bias", {c.width});
+    }
+    P.expect(std::string(kHfFinal) + ".weight", {c.width});
+    P.expect(std::string(kHfFinal) + ".bias", {c.width});
+}
+
 void expect_params(t2v_clip* m) {
+    if (m->cfg.arch == 1) {
+        expect_params_hf(m);
+        return;
+    }
     ParamStore& P = m->params;
     const t2v_clip_config& c = m->cfg;
     P.expect("token_embedding.weight", {c.vocab, c.width});
@@ -171,14 +226,15 @@ int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     Builder bld(plan, arena, dry, num_sms());
     NetCtx c{&m->params, &bld, stream, nullptr};
     const t2v_clip_config& cfg = m->cfg;
+    const bool hf = cfg.arch == 1;
     const int L = cfg.context, W = cfg.width, heads = cfg.heads;
     const long long R = static_cast<long long>(B) * L;
     int* tokens = reinterpret_cast<int*>(bld.alloc_bytes(static_cast<size_t>(R) * sizeof(int)));
     *tok_out = tokens;
     Tok x = bld.alloc(R, W);
     {
-        const __half* emb = prm(c, "token_embedding.weight");
-        const __half* pos = prm(c, "positional_embedding");
+        const __half* emb = prm(c, hf ? kHfEmb : "token_embedding.weight");
+        const __half* pos = prm(c, hf ? kHfPos : "positional_embedding");
         const Tok xx = x;
         const int vocab = cfg.vocab;
         bld.step([=](cudaStream_t s) {
@@ -187,11 +243,24 @@ int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
             return launch_status("clip launch");
         }, 1, STEP_OTHER, 0.0, "clip embed");
     }
+    // per-layer names: open_clip's ResidualAttentionBlock (arch 0) or transformers' CLIPEncoderLayer (arch 1)
+    const std::string out_proj = hf ? ".self_attn.out_proj" : ".attn.out_proj";
+    const std::string ln2 = hf ? ".layer_norm2" : ".ln_2", fc1 = hf ? ".mlp.fc1" : ".mlp.c_fc", fc2 = hf ? ".mlp.fc2" : ".mlp.c_proj";
+    void (*act)(__half*, long long) = hf ? quick_gelu_kernel : gelu_kernel;
+    const char* act_label = hf ? "clip quick_gelu" : "clip gelu";
     for (int i = 0; i < cfg.layers_run; ++i) {
-        const std::string p = "transformer.resblocks." + std::to_string(i);
+        const std::string p = hf ? hf_layer(i) : "transformer.resblocks." + std::to_string(i);
         // x = x + out_proj(attention(in_proj(ln_1(x))))
-        Tok qkv = ln_linear(c, x, p + ".ln_1", p + ".attn.in_proj", prm(c, p + ".attn.in_proj_weight"), prm(c, p + ".attn.in_proj_bias"),
+        Tok qkv;
+        if (hf) {       // q / k / v with their biases, concatenated once into one [3W, W] weight and one [3W] bias (cached)
+            const std::string a = p + ".self_attn.";
+            const __half* wqkv = w_cat(c, {a + "q_proj.weight", a + "k_proj.weight", a + "v_proj.weight"});
+            const __half* bqkv = w_cat(c, {a + "q_proj.bias", a + "k_proj.bias", a + "v_proj.bias"});
+            qkv = ln_linear(c, x, p + ".layer_norm1", a + "qkv", wqkv, bqkv, 3 * W, nullptr);
+        } else {
+            qkv = ln_linear(c, x, p + ".ln_1", p + ".attn.in_proj", prm(c, p + ".attn.in_proj_weight"), prm(c, p + ".attn.in_proj_bias"),
                             3 * W, nullptr);
+        }
         Tok o = bld.alloc(R, W);
         {
             const Tok q = qkv, oo = o;
@@ -202,26 +271,26 @@ int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
             }, 1, STEP_ATTN, 4.0 * B * heads * static_cast<double>(L) * L * kClipD / 2, "clip causal attention");
         }
         bld.free(qkv);
-        Tok y = linear(c, o, prm(c, p + ".attn.out_proj.weight"), W, prm(c, p + ".attn.out_proj.bias"), &x);
+        Tok y = linear(c, o, prm(c, p + out_proj + ".weight"), W, prm(c, p + out_proj + ".bias"), &x);
         bld.free(o);
         bld.free(x);
         x = y;
-        // x = x + c_proj(gelu(c_fc(ln_2(x))))
-        Tok h = ln_linear(c, x, p + ".ln_2", p + ".mlp.c_fc", prm(c, p + ".mlp.c_fc.weight"), prm(c, p + ".mlp.c_fc.bias"), 4 * W, nullptr);
+        // x = x + c_proj(gelu(c_fc(ln_2(x))))       (arch 1: x + fc2(quick_gelu(fc1(layer_norm2(x)))))
+        Tok h = ln_linear(c, x, p + ln2, p + fc1, prm(c, p + fc1 + ".weight"), prm(c, p + fc1 + ".bias"), 4 * W, nullptr);
         {
             const Tok hh = h;
             const long long n8 = R * (4 * W) / 8;
             bld.step([=](cudaStream_t s) {
-                launch_pdl(gelu_kernel, dim3(static_cast<unsigned>((n8 + 255) / 256)), dim3(256), 0, s, hh.p, n8);
+                launch_pdl(act, dim3(static_cast<unsigned>((n8 + 255) / 256)), dim3(256), 0, s, hh.p, n8);
                 return launch_status("clip launch");
-            }, 1, STEP_OTHER, 0.0, "clip gelu");
+            }, 1, STEP_OTHER, 0.0, act_label);
         }
-        Tok y2 = linear(c, h, prm(c, p + ".mlp.c_proj.weight"), W, prm(c, p + ".mlp.c_proj.bias"), &x);
+        Tok y2 = linear(c, h, prm(c, p + fc2 + ".weight"), W, prm(c, p + fc2 + ".bias"), &x);
         bld.free(h);
         bld.free(x);
         x = y2;
     }
-    Tok z = layer_norm(c, x, "ln_final");
+    Tok z = layer_norm(c, x, hf ? kHfFinal : "ln_final");
     bld.free(x);
     *out_tok = z.p;
     return bld.error;
@@ -279,6 +348,10 @@ int t2v_clip_create(const t2v_clip_config* cfg, t2v_clip** out) {
     if (!cfg || !out) return -1;
     if (cfg->width % 64 != 0 || cfg->width / cfg->heads != 64 || cfg->context > 128 || cfg->layers_run < 1 || cfg->vocab < 1) {
         set_error("CLIP text tower: head width must be 64 (width / heads), context <= 128");
+        return -2;
+    }
+    if (cfg->arch != 0 && cfg->arch != 1) {
+        set_error("CLIP text tower: arch %d (0: OpenCLIP ViT-H-14, 1: transformers CLIPTextModel)", cfg->arch);
         return -2;
     }
     t2v_clip* m = new t2v_clip();

@@ -90,7 +90,7 @@ class ShardExportC(C.Structure):
 
 
 class ClipConfigC(C.Structure):
-    _fields_ = [('width', c_int), ('heads', c_int), ('layers_run', c_int), ('context', c_int), ('vocab', c_int)]
+    _fields_ = [('width', c_int), ('heads', c_int), ('layers_run', c_int), ('context', c_int), ('vocab', c_int), ('arch', c_int)]
 
 
 class VAEConfigC(C.Structure):

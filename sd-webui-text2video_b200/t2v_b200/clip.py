@@ -11,9 +11,13 @@ so `load_state_dict` of the text side of open_clip_pytorch_model.bin works and t
 Not here: the BPE vocabulary (open_clip ships it; there is no copy offline) -- pass `tokenizer` (anything with
 `.encode(str) -> list[int]`; `open_clip.tokenizer._tokenizer` when the package is installed) -- and the webui's prompt-attention
 syntax parser (`modules.prompt_parser`, used when importable; otherwise every token has weight 1).
+
+`FrozenCLIPEmbedder` is VideoCrafter's text conditioning (videocrafter/lvdm/models/modules/condition_modules.py:15-40): the
+OpenAI CLIP ViT-L/14 text model with transformers' parameter names, on the same library tower (arch 1).
 """
 import ctypes as C
 import math
+import os
 
 import torch
 import torch.nn as nn
@@ -32,18 +36,59 @@ class _InProj(nn.Module):
         self.out_proj = nn.Linear(width, width)
 
 
-class _TextTower(_NativeModule):
-    """`model` of the embedder: open_clip's text-side module tree; arithmetic in libt2v_b200.so (csrc/clip.cu)."""
+class _NativeTextTower(_NativeModule):
+    """A CLIP text transformer whose arithmetic runs in libt2v_b200.so (csrc/clip.cu); subclasses build the parameter tree."""
     _set_fn = 't2v_clip_set_param'
 
-    def __init__(self, width=1024, heads=16, layers=24, layers_run=23, context=77, vocab=49408):
-        super().__init__()
-        cfg = _lib.ClipConfigC(width, heads, layers_run, context, vocab)
+    def _create(self, width, heads, layers, layers_run, context, vocab, arch):
+        cfg = _lib.ClipConfigC(width, heads, layers_run, context, vocab, arch)
         self.width, self.heads, self.layers, self.layers_run, self.context, self.vocab = width, heads, layers, layers_run, context, vocab
         h = C.c_void_p()
         _lib.check(_lib.load_library().t2v_clip_create(C.byref(cfg), C.byref(h)), 'clip_create')
         object.__setattr__(self, '_handle', h)
         self._native_names = set(_param_table('t2v_clip_param_info', h))
+
+    def __del__(self):
+        h = self.__dict__.get('_handle')
+        if h:
+            try:
+                _lib.load_library().t2v_clip_destroy(h)
+            except Exception:
+                pass
+
+    def named_parameters(self, *a, **kw):
+        for name, p in super().named_parameters(*a, **kw):
+            if name in self._native_names:
+                yield name, p
+
+    def state_dict(self, *a, **kw):
+        return nn.Module.state_dict(self, *a, **kw)
+
+    def _load_from_state_dict(self, *a, **kw):
+        # also reached when a parent module (e.g. LatentDiffusion) loads a state dict: its in-place copies must reship
+        self._dirty = True
+        super()._load_from_state_dict(*a, **kw)
+
+    @torch.no_grad()
+    def encode_tokens(self, tokens, out_dtype=torch.float32):
+        """tokens [B, context] integer tensor -> ln_final(transformer(...)) [B, context, width]."""
+        self.sync_weights()
+        tokens = tokens.to('cuda', torch.int32).contiguous()
+        B, L = tokens.shape
+        if L != self.context:
+            raise ValueError(f'expected {self.context} tokens per chunk, got {L}')
+        out = torch.empty((B, L, self.width), device='cuda', dtype=out_dtype)
+        _lib.check(_lib.lib().t2v_clip_encode(self._handle, _lib.ptr(tokens), _lib.ptr(out), int(out_dtype == torch.float32), B,
+                                              _lib.stream_ptr()), 'clip_encode')
+        return out
+
+
+class _TextTower(_NativeTextTower):
+    """`model` of the embedder: open_clip's text-side module tree; arithmetic in libt2v_b200.so (csrc/clip.cu)."""
+
+    def __init__(self, width=1024, heads=16, layers=24, layers_run=23, context=77, vocab=49408):
+        super().__init__()
+        self._create(width, heads, layers, layers_run, context, vocab, arch=0)
         self.token_embedding = nn.Embedding(vocab, width)
         self.positional_embedding = nn.Parameter(torch.zeros(context, width))
         self.transformer = _Holder()
@@ -63,34 +108,52 @@ class _TextTower(_NativeModule):
         self.logit_scale = nn.Parameter(torch.zeros(()))
         self._init_native()
 
-    def __del__(self):
-        h = self.__dict__.get('_handle')
-        if h:
-            try:
-                _lib.load_library().t2v_clip_destroy(h)
-            except Exception:
-                pass
 
-    def named_parameters(self, *a, **kw):
-        for name, p in super().named_parameters(*a, **kw):
-            if name in self._native_names:
-                yield name, p
+class _HFEmbeddings(_Holder):
+    """`text_model.embeddings` of transformers' CLIPTextModel.  Older transformers releases saved the `position_ids`
+    buffer (arange(77)) in checkpoints; it carries no weight, so a state dict that has it loads and the entry is dropped."""
 
-    def state_dict(self, *a, **kw):
-        return nn.Module.state_dict(self, *a, **kw)
+    def __init__(self, vocab, context, width):
+        super().__init__()
+        self.token_embedding = nn.Embedding(vocab, width)
+        self.position_embedding = nn.Embedding(context, width)
 
-    @torch.no_grad()
-    def encode_tokens(self, tokens, out_dtype=torch.float32):
-        """tokens [B, context] integer tensor -> ln_final(transformer(...)) [B, context, width]."""
-        self.sync_weights()
-        tokens = tokens.to('cuda', torch.int32).contiguous()
-        B, L = tokens.shape
-        if L != self.context:
-            raise ValueError(f'expected {self.context} tokens per chunk, got {L}')
-        out = torch.empty((B, L, self.width), device='cuda', dtype=out_dtype)
-        _lib.check(_lib.lib().t2v_clip_encode(self._handle, _lib.ptr(tokens), _lib.ptr(out), int(out_dtype == torch.float32), B,
-                                              _lib.stream_ptr()), 'clip_encode')
-        return out
+    def _load_from_state_dict(self, state_dict, prefix, *a, **kw):
+        state_dict.pop(prefix + 'position_ids', None)
+        super()._load_from_state_dict(state_dict, prefix, *a, **kw)
+
+
+class _CLIPTextModel(_NativeTextTower):
+    """`transformer` of FrozenCLIPEmbedder: transformers' CLIPTextModel module tree (`text_model.embeddings`,
+    `text_model.encoder.layers[i].{layer_norm1, self_attn.{q,k,v,out}_proj, layer_norm2, mlp.fc1, mlp.fc2}`,
+    `text_model.final_layer_norm`); arithmetic in libt2v_b200.so (csrc/clip.cu, arch 1)."""
+
+    def __init__(self, width=768, heads=12, layers=12, context=77, vocab=49408):
+        super().__init__()
+        self._create(width, heads, layers, layers, context, vocab, arch=1)
+        tm = _Holder()
+        tm.embeddings = _HFEmbeddings(vocab, context, width)
+        blocks = []
+        for _ in range(layers):
+            b = _Holder()
+            b.self_attn = _Holder()
+            for n in ('k_proj', 'v_proj', 'q_proj', 'out_proj'):
+                setattr(b.self_attn, n, nn.Linear(width, width))
+            b.layer_norm1 = nn.LayerNorm(width)
+            b.mlp = _Holder()
+            b.mlp.fc1 = nn.Linear(width, 4 * width)
+            b.mlp.fc2 = nn.Linear(4 * width, width)
+            b.layer_norm2 = nn.LayerNorm(width)
+            blocks.append(b)
+        tm.encoder = _Holder()
+        tm.encoder.layers = nn.ModuleList(blocks)
+        tm.final_layer_norm = nn.LayerNorm(width)
+        self.text_model = tm
+        self._init_native()
+
+    def forward(self, input_ids):
+        """input_ids [B, context] -> last_hidden_state [B, context, width] fp32 (no attention mask: causal only)."""
+        return self.encode_tokens(input_ids)
 
 
 class PromptChunk(object):
@@ -201,3 +264,92 @@ class FrozenOpenCLIPEmbedder(nn.Module):
 
     def get_learned_conditioning(self, text):
         return self.encode(text)
+
+
+def _is_hf_tokenizer(tok):
+    return any(c.__module__.startswith('transformers.') for c in type(tok).__mro__)
+
+
+class FrozenCLIPEmbedder(nn.Module):
+    """VideoCrafter's text conditioning (videocrafter/lvdm/models/modules/condition_modules.py:15-40): the OpenAI CLIP
+    ViT-L/14 text model, `forward(list of str) -> last_hidden_state [B, 77, 768]` fp32, on the library (csrc/clip.cu, arch 1).
+
+    `transformer` holds transformers' CLIPTextModel parameter tree, so the `cond_stage_model.transformer.text_model.*` keys
+    of a VideoCrafter `model.ckpt` load into it.  Prompts are framed as the reference's `tokenizer(text, truncation=True,
+    max_length=77, padding='max_length')`: <|startoftext|>, at most 75 BPE ids, <|endoftext|>, then <|endoftext|> (the
+    ViT-L/14 tokenizer's pad token) up to 77.
+
+    tokenizer: a transformers CLIPTokenizer (called exactly as the reference calls it), or any object with
+    `.encode(str) -> list of int` over the OpenAI CLIP BPE vocabulary (e.g. open_clip's SimpleTokenizer; the framing is
+    then done here).  `version` names the model; when it is a local directory (a Hugging Face snapshot of
+    openai/clip-vit-large-patch14) the tokenizer and the text weights are read from it.  Nothing is downloaded."""
+    ID_START, ID_END = 49406, 49407
+
+    def __init__(self, version='openai/clip-vit-large-patch14', device='cuda', max_length=77, tokenizer=None, width=768, heads=12,
+                 layers=12, vocab=49408):
+        super().__init__()
+        self.transformer = _CLIPTextModel(width, heads, layers, max_length, vocab)
+        self.version, self.device, self.max_length = version, device, max_length
+        local = isinstance(version, str) and os.path.isdir(version)
+        if tokenizer is None and local:
+            from transformers import CLIPTokenizer                      # type: ignore
+            tokenizer = CLIPTokenizer.from_pretrained(version, local_files_only=True)
+        self.tokenizer = tokenizer
+        if local:
+            self.transformer.load_state_dict(_text_weights(version), strict=True)
+        self.freeze()
+
+    def freeze(self):
+        self.transformer = self.transformer.eval()
+        for param in self.parameters():
+            param.requires_grad = False
+
+    # read from the tokenizer when used, so a tokenizer attached after construction frames prompts with its own ids
+    @property
+    def id_start(self):
+        enc = getattr(self.tokenizer, 'encoder', None) or {}
+        return enc.get('<|startoftext|>', enc.get('<start_of_text>', self.ID_START))
+
+    @property
+    def id_end(self):
+        enc = getattr(self.tokenizer, 'encoder', None) or {}
+        return enc.get('<|endoftext|>', enc.get('<end_of_text>', self.ID_END))
+
+    def tokenize(self, text):
+        """list of str (or one str) -> input_ids [B, max_length] int64 on the CPU."""
+        texts = [text] if isinstance(text, str) else list(text)
+        tok = self.tokenizer
+        if tok is None:
+            raise RuntimeError('FrozenCLIPEmbedder needs the CLIP BPE tokenizer to encode strings: pass tokenizer= (a '
+                               'transformers CLIPTokenizer, or an object with .encode(str) -> list of int such as open_clip\'s '
+                               'SimpleTokenizer), or version= a local openai/clip-vit-large-patch14 snapshot directory')
+        if _is_hf_tokenizer(tok):
+            be = tok(texts, truncation=True, max_length=self.max_length, return_length=True, return_overflowing_tokens=False,
+                     padding='max_length', return_tensors='pt')
+            return be['input_ids']
+        rows = []
+        for t in texts:
+            ids = [self.id_start] + list(tok.encode(t))[:self.max_length - 2] + [self.id_end]
+            rows.append(ids + [self.id_end] * (self.max_length - len(ids)))
+        return torch.tensor(rows, dtype=torch.long)
+
+    def encode_with_transformer(self, tokens):
+        """Already tokenised input [B, max_length] -> last_hidden_state [B, max_length, width] fp32 on the GPU."""
+        return self.transformer.encode_tokens(torch.as_tensor(tokens))
+
+    def forward(self, text):
+        return self.encode_with_transformer(self.tokenize(text))
+
+    def encode(self, text):
+        return self(text)
+
+
+def _text_weights(directory):
+    """`text_model.*` tensors of a local Hugging Face CLIP snapshot (model.safetensors or pytorch_model.bin)."""
+    st = os.path.join(directory, 'model.safetensors')
+    if os.path.exists(st):
+        from safetensors.torch import load_file                           # type: ignore
+        sd = load_file(st)
+    else:
+        sd = torch.load(os.path.join(directory, 'pytorch_model.bin'), map_location='cpu')
+    return {k: v for k, v in sd.items() if k.startswith('text_model.') and not k.endswith('.position_ids')}
