@@ -71,6 +71,17 @@ int t2v_unet_param_info(t2v_unet* u, int index, char* name_out, size_t name_cap,
  *   out [B, out_dim, F, h, w] fp16 (out_is_f32 = 0) or fp32                                               */
 int t2v_unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, void* out,
                      int out_is_f32, int B, int F, int h, int w, int L, void* stream);
+/* eps = UNetModel.forward(x, t, context, features_adapter) (videocrafter/lvdm/models/modules/openaimodel3d.py:632-670), arch 1
+ * only: feature i is added to h after input block id with (id + 1) % 3 == 0 (the i-th such block, counting from 0), before h is
+ * pushed on the skip stack.  feats[i] is a device pointer to [feats_B, F, h_i, w_i, C_i] fp16, channels-last: the
+ * reference's `b c t h w` feature permuted to (b, t, h, w, c), with h_i, w_i, C_i those of h at that block.  Sample j of the
+ * forward reads feature sample j % feats_B (feats_B = 1: broadcast; B = 2 feats_B: a batched cond / uncond pair).
+ * n_feats must equal the number of such blocks and B a multiple of feats_B.  The features are staged per forward (copied
+ * device to device); the plan of a shape with features is separate from the plan without, which t2v_unet_forward keeps
+ * using unchanged.  Other arguments as t2v_unet_forward.                                                          */
+int t2v_unet_forward_adapter(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx,
+                             const void* const* feats, int n_feats, int feats_B, void* out, int out_is_f32, int B, int F, int h,
+                             int w, int L, void* stream);
 /* 2*MAC flop count of one forward at this shape (for roofline reporting). */
 double t2v_unet_flops(t2v_unet* u, int B, int F, int h, int w, int L);
 int t2v_unet_num_launches(t2v_unet* u);
@@ -200,6 +211,38 @@ int t2v_clip_param_info(t2v_clip* m, int index, char* name_out, size_t name_cap,
 /* tokens [B, context] int32 (device) -> out [B, context, width] fp16 (out_is_f32 = 0) or fp32: ln_final(transformer(...))
  * (arch 1: final_layer_norm(encoder(...)) = last_hidden_state) */
 int t2v_clip_encode(t2v_clip* m, const int* tokens, void* out, int out_is_f32, int B, void* stream);
+
+/* ------------------------------------------------------------------------------------------ depth adapter
+ * replaces VideoCrafter's T2I-Adapter (videocrafter/lvdm/models/modules/adapter.py: Adapter(channels, nums_rb, cin, ksize, sk,
+ * use_conv)) as T2VAdapterDepth.get_adapter_features runs it (videocrafter/lvdm/models/ddpm3d.py:1470-1484): PixelUnshuffle(8),
+ * conv_in, then nums_rb ResnetBlocks per level (the first block of every level after the first downsamples: 3x3 stride-2
+ * conv if use_conv, else 2x2 average pooling), one feature map per level.  Parameter names are the reference module's
+ * (`conv_in.*`, `body.{k}.{in_conv,block1,block2,skep,down_opt.op}.*`, k = level * nums_rb + block), so an adapter
+ * checkpoint loads as is.  create rejects what the reference cannot run: sk = 0 with differing level widths (its skep is
+ * built for the block's input width but applied to in_conv's output).  Also rejected: cin not a multiple of 64, ksize other
+ * than 1 or 3, level widths not multiples of 8.                                                                      */
+typedef struct t2v_adapter t2v_adapter;
+typedef struct {
+    int cin;              /* input channels after PixelUnshuffle(8): 64 * condition channels (64 for one depth channel) */
+    int channels[4];      /* per-level widths, e.g. 320, 640, 1280, 1280 */
+    int n_levels;         /* len(channels), 1..4 */
+    int nums_rb;          /* ResnetBlocks per level */
+    int ksize;            /* in_conv / block2 / skep kernel (1 or 3); block1 is always 3x3 */
+    int sk;               /* 1: identity skip (in_conv only where the width changes), 0: skep conv in every block */
+    int use_conv;         /* downsampling: 1 = 3x3 stride-2 conv (sizes round up), 0 = 2x2 average pooling (sizes round down) */
+} t2v_adapter_config;
+int t2v_adapter_create(const t2v_adapter_config* cfg, t2v_adapter** out);
+void t2v_adapter_destroy(t2v_adapter* a);
+int t2v_adapter_set_param(t2v_adapter* a, const char* name, const void* data, int dtype, int ndim, const int64_t* shape,
+                          void* stream);
+int t2v_adapter_missing_params(t2v_adapter* a, char* name_out, size_t name_cap);
+int t2v_adapter_param_info(t2v_adapter* a, int index, char* name_out, size_t name_cap, int64_t* shape_out, int* ndim_out);
+/* cond [N, cin/64, H, W] fp32 (cond_is_f32 = 1) or fp16 -> feats_out[i] [N, h_i, w_i, channels[i]] fp16 channels-last (the
+ * reference's feature i [N, C_i, h_i, w_i], permuted), h_0 = H/8 and each later level halved as the config downsamples.
+ * Errors: H or W not a multiple of 8, or a level that would be empty.  The first call at a shape builds its plan, the
+ * second and later ones replay it as one CUDA graph.                                                                */
+int t2v_adapter_encode(t2v_adapter* a, const void* cond, int cond_is_f32, void* const* feats_out, int N, int H, int W,
+                       void* stream);
 
 /* ------------------------------------------------------------------------------------------ sampler steps
  * replace the per-step tensor arithmetic of scripts/samplers (ddim/gaussian_sampler.py:125-136,:269-283;

@@ -224,6 +224,103 @@ __global__ void frames_to_u8_kernel(const __half* tok, long long ld, uint8_t* ou
     }
 }
 
+// nn.PixelUnshuffle(8) of NCHW frames straight into tokens: row (n, y, x), column c*64 + i*8 + j = x[n, c, 8y+i, 8x+j].
+// One thread per 8 consecutive columns (a fixed (c, i), j = 0..7): eight contiguous source pixels, one 16-byte store.
+__global__ void pixel_unshuffle_kernel(const void* x, int x_is_f32, __half* tok, int N, int Cc, int H, int W) {
+    griddep_wait();
+    griddep_launch_small();
+    const int h8 = H / 8, w8 = W / 8;
+    const int groups = Cc * 8;                  // 8-column groups per row
+    const long long n = static_cast<long long>(N) * h8 * w8 * groups;
+    GRID_STRIDE(i, n) {
+        const int g = static_cast<int>(i % groups);
+        long long t = i / groups;
+        const int xo = static_cast<int>(t % w8);
+        t /= w8;
+        const int yo = static_cast<int>(t % h8);
+        const long long f = t / h8;
+        const int c = g >> 3, ky = g & 7;
+        const long long src = ((f * Cc + c) * H + (8 * yo + ky)) * static_cast<long long>(W) + 8 * xo;
+        uint4 o;
+        __half* oh = reinterpret_cast<__half*>(&o);
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            oh[j] = x_is_f32 ? __float2half_rn(reinterpret_cast<const float*>(x)[src + j]) : reinterpret_cast<const __half*>(x)[src + j];
+        reinterpret_cast<uint4*>(tok)[i] = o;
+    }
+}
+
+// y = max(x, 0) in place on a token matrix (n8 16-byte vectors)
+__global__ void relu_kernel(uint4* x, long long n8) {
+    griddep_wait();
+    griddep_launch_small();
+    const __half2 z = __float2half2_rn(0.f);
+    GRID_STRIDE(i, n8) {
+        uint4 v = x[i];
+        __half2* h = reinterpret_cast<__half2*>(&v);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) h[k] = __hmax2(h[k], z);
+        x[i] = v;
+    }
+}
+
+// 2x2 average pooling, stride 2, floor sizes (nn.AvgPool2d(2, 2)): x [n, h, w, C] -> y [n, h/2, w/2, C]; fp32 sum of the four
+// taps, times 0.25, one fp16 rounding
+__global__ void avgpool2x2_kernel(const uint4* x, uint4* y, long long nframes, int h, int w, int C8) {
+    griddep_wait();
+    griddep_launch_small();
+    const int ho = h / 2, wo = w / 2;
+    GRID_STRIDE(i, nframes * ho * wo * C8) {
+        const int c = static_cast<int>(i % C8);
+        long long t = i / C8;
+        const int xo = static_cast<int>(t % wo);
+        t /= wo;
+        const int yo = static_cast<int>(t % ho);
+        const long long f = t / ho;
+        float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int tap = 0; tap < 4; ++tap) {
+            const uint4 v = __ldg(x + ((f * h + 2 * yo + (tap >> 1)) * w + 2 * xo + (tap & 1)) * C8 + c);
+            const __half2* hv = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float2 a = __half22float2(hv[k]);
+                acc[2 * k] += a.x;
+                acc[2 * k + 1] += a.y;
+            }
+        }
+        uint4 o;
+        __half2* oh = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) oh[k] = __floats2half2_rn(acc[2 * k] * 0.25f, acc[2 * k + 1] * 0.25f);
+        y[i] = o;
+    }
+}
+
+// x[r, :] += f[(r / rows_per_sample % f_samples) * rows_per_sample + r % rows_per_sample, :]  in place; fp32 add, one rounding
+__global__ void feature_add_kernel(__half* x, long long ldx, const __half* f, int C8, long long rows, long long rows_per_sample,
+                                   int f_samples) {
+    griddep_wait();
+    griddep_launch_small();
+    GRID_STRIDE(i, rows * C8) {
+        const long long r = i / C8;
+        const int c = static_cast<int>(i - r * C8);
+        const long long s = r / rows_per_sample;
+        const long long fr = (s % f_samples) * rows_per_sample + (r - s * rows_per_sample);
+        uint4* xp = reinterpret_cast<uint4*>(x + r * ldx) + c;
+        uint4 a = *xp;
+        const uint4 b = __ldg(reinterpret_cast<const uint4*>(f + fr * (static_cast<long long>(C8) * 8)) + c);
+        __half2* ah = reinterpret_cast<__half2*>(&a);
+        const __half2* bh = reinterpret_cast<const __half2*>(&b);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float2 u = __half22float2(ah[k]), v = __half22float2(bh[k]);
+            ah[k] = __floats2half2_rn(u.x + v.x, u.y + v.y);
+        }
+        *xp = a;
+    }
+}
+
 __global__ void frames_to_f32_kernel(const __half* tok, long long ld, float* out, int n, int H, int W) {
     griddep_wait();
     griddep_launch_small();
@@ -493,6 +590,32 @@ int im2col_s2(const __half* x, __half* col, int nframes, int h, int w, int C, cu
     const long long n = static_cast<long long>(nframes) * ((pad_lo ? (h + 1) / 2 : h / 2)) * ((pad_lo ? (w + 1) / 2 : w / 2)) * 9 * (C / 8);
     launch_pdl(im2col_s2_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(col),
                                                            nframes, h, w, C / 8, pad_lo);
+    return ok();
+}
+int pixel_unshuffle_ingest(const void* x, int x_is_f32, __half* tok, int N, int Cc, int H, int W, cudaStream_t stream) {
+    if (H % 8 || W % 8) return -1;
+    const long long n = static_cast<long long>(N) * (H / 8) * (W / 8) * Cc * 8;
+    launch_pdl(pixel_unshuffle_kernel, grid_for(n, 256), 256, 0, stream, x, x_is_f32, tok, N, Cc, H, W);
+    return ok();
+}
+int relu_inplace(__half* x, long long rows, int C, cudaStream_t stream) {
+    if (C % 8) return -1;
+    const long long n8 = rows * (C / 8);
+    launch_pdl(relu_kernel, grid_for(n8, 256), 256, 0, stream, reinterpret_cast<uint4*>(x), n8);
+    return ok();
+}
+int avgpool2x2(const __half* x, __half* y, int nframes, int h, int w, int C, cudaStream_t stream) {
+    if (C % 8) return -1;
+    const long long n = static_cast<long long>(nframes) * (h / 2) * (w / 2) * (C / 8);
+    launch_pdl(avgpool2x2_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y),
+               nframes, h, w, C / 8);
+    return ok();
+}
+int feature_add(__half* x, long long ldx, const __half* f, int C, long long rows, long long rows_per_sample, int f_samples,
+                cudaStream_t stream) {
+    if (C % 8 || ldx % 8 || rows_per_sample < 1 || f_samples < 1) return -1;
+    const long long n = rows * (C / 8);
+    launch_pdl(feature_add_kernel, grid_for(n, 256), 256, 0, stream, x, ldx, f, C / 8, rows, rows_per_sample, f_samples);
     return ok();
 }
 int concat_cols(const __half* a, long long lda, int Ca, const __half* b, long long ldb, int Cb, __half* out,

@@ -82,6 +82,17 @@ int egress_latent(const __half* tok, long long ld, void* out, int out_is_f32, in
 int upsample2x(const __half* x, __half* y, int nframes, int h, int w, int C, cudaStream_t stream);
 // 3x3 stride-2 pad-1 gather: x [n, h, w, C] -> col [n*ho*wo, 9*C] (tap-major, tap = ky*3+kx)
 int im2col_s2(const __half* x, __half* col, int nframes, int h, int w, int C, cudaStream_t stream, int pad_lo = 1);
+// T2I-Adapter glue (adapter.cu, unet.cu).  nn.PixelUnshuffle(8): x [N, Cc, H, W] (fp32 or fp16, H, W multiples of 8) ->
+// tokens [N*(H/8)*(W/8), 64*Cc] fp16, column c*64 + i*8 + j = x[n, c, 8y+i, 8x+j]
+int pixel_unshuffle_ingest(const void* x, int x_is_f32, __half* tok, int N, int Cc, int H, int W, cudaStream_t stream);
+// max(x, 0) in place on a dense token matrix [rows, C]
+int relu_inplace(__half* x, long long rows, int C, cudaStream_t stream);
+// nn.AvgPool2d(2, 2) (floor sizes): x [n, h, w, C] -> y [n, h/2, w/2, C]; fp32 sum, one fp16 rounding
+int avgpool2x2(const __half* x, __half* y, int nframes, int h, int w, int C, cudaStream_t stream);
+// x[r, :] += f[(sample % f_samples) * rows_per_sample + r % rows_per_sample, :], sample = r / rows_per_sample; f dense [., C];
+// fp16 + fp16 in fp32, one rounding (adding zeros leaves every value unchanged)
+int feature_add(__half* x, long long ldx, const __half* f, int C, long long rows, long long rows_per_sample, int f_samples,
+                cudaStream_t stream);
 int concat_cols(const __half* a, long long lda, int Ca, const __half* b, long long ldb, int Cb, __half* out,
                 long long ldo, long long rows, cudaStream_t stream);
 // sinusoidal_embedding(t, dim): out [B, dim] fp16 = [cos(t*f_i) | sin(t*f_i)], f_i = 10000^(-i/half)

@@ -771,15 +771,30 @@ Tok upsample(Ctx& c, const Tok& x, const Blk& blk, int hcur, int wcur) {
     return y;
 }
 
+constexpr int kMaxFeat = 8;
+
 struct IO {
     __half* x_tok;      // [R, 8]
     float* t;           // [B]
     __half* ctx;        // [B*L, context_dim]
     __half* out_tok;    // [R, 8]
+    // adapter features (plans built with feats_B > 0): staging [feats_B * F * h_i * w_i, C_i] per injection point
+    int n_feat = 0;
+    __half* feat[kMaxFeat] = {nullptr};
+    long long feat_elems[kMaxFeat] = {0};
 };
 
+// input blocks after which VideoCrafter's UNetModel adds an adapter feature (openaimodel3d.py:658): (id + 1) % 3 == 0
+bool feature_block(int id) { return (id + 1) % 3 == 0; }
+int n_feature_blocks(const t2v_unet* u) {
+    int n = 0;
+    for (size_t id = 0; id < u->ins.size(); ++id) n += feature_block(static_cast<int>(id)) ? 1 : 0;
+    return n;
+}
+
+// feats_B > 0: the plan variant with adapter features (VideoCrafter only), staged for feats_B samples
 int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, int B, int F, int h, int w, int L,
-          IO* io) {
+          IO* io, int feats_B = 0) {
     Builder bld(plan, arena, dry, num_sms());
     Ctx c;
     c.params = &u->params;
@@ -816,6 +831,27 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     Tok ctx_tok = bld.alloc(static_cast<long long>(B) * L, cfg.context_dim);
     c.ctx = ctx_tok.p;
     io->ctx = ctx_tok.p;
+    io->n_feat = 0;
+    if (feats_B > 0) {                   // feature staging, filled per forward like ctx; level sizes follow the input blocks
+        int hf = h, wf = w;
+        for (size_t id = 0; id < u->ins.size(); ++id) {
+            const Blk& b0 = u->ins[id][0];
+            if (b0.kind == Blk::DOWN) {
+                hf = (hf + 1) / 2;
+                wf = (wf + 1) / 2;
+            }
+            if (!feature_block(static_cast<int>(id))) continue;
+            if (io->n_feat >= kMaxFeat) {
+                set_error("more than %d adapter injection points", kMaxFeat);
+                return -7;
+            }
+            const int Cf = u->ins[id].back().cout;
+            Tok f = bld.alloc(static_cast<long long>(feats_B) * F * hf * wf, Cf);
+            io->feat[io->n_feat] = f.p;
+            io->feat_elems[io->n_feat] = f.rows * f.C;
+            io->n_feat += 1;
+        }
+    }
     // time embedding: sinusoid -> Linear -> SiLU -> Linear (t2v_model.py:154-156, :420)
     __half* sinus = reinterpret_cast<__half*>(bld.alloc_bytes(static_cast<size_t>(B) * cfg.dim * sizeof(__half)));
     __half* e1 = reinterpret_cast<__half*>(bld.alloc_bytes(static_cast<size_t>(B) * E * sizeof(__half)));
@@ -888,9 +924,18 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
             x = y;
         }
     };
-    for (auto& blk : u->ins) {
-        run_block(blk);
+    int feat_i = 0;
+    for (size_t id = 0; id < u->ins.size(); ++id) {
+        run_block(u->ins[id]);
         to_layout(false);                // skip connections (and the next block's ResBlock) are frame-sharded
+        if (feats_B > 0 && feature_block(static_cast<int>(id))) {       // h = h + features_adapter[i], before the push
+            const Tok xx = x;
+            const __half* f = io->feat[feat_i++];
+            const long long per_sample = static_cast<long long>(F) * hc * wc;
+            const int fb = feats_B;
+            bld.step([=](cudaStream_t s) { return feature_add(xx.p, xx.ld, f, xx.C, xx.rows, per_sample, fb, s); }, 1, STEP_OTHER,
+                     0.0, "adapter feature add");
+        }
         xs.push_back(x);
         xs_hw.push_back({hc, wc});
     }
@@ -929,10 +974,14 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
 
 std::map<Plan*, IO> g_io;
 
-Plan* get_plan(t2v_unet* u, int B, int F, int h, int w, int L, cudaStream_t stream) {
-    char key[96];
+Plan* get_plan(t2v_unet* u, int B, int F, int h, int w, int L, cudaStream_t stream, int feats_B = 0) {
+    char key[112];
     snprintf(key, sizeof(key), "%d,%d,%d,%d,%d,%d,%d/%d", B, F, h, w, L, u->taps_enabled ? 1 : 0, u->shard_on ? u->peers.rank : 0,
              u->shard_on ? u->peers.nranks : 1);
+    if (feats_B > 0) {                   // the adapter-feature variant (a forward without features keeps its plan and key)
+        const size_t n = strlen(key);
+        snprintf(key + n, sizeof(key) - n, ",a%d", feats_B);
+    }
     auto touch = [&](const std::string& k) {
         auto& l = u->plan_lru;
         l.erase(std::remove(l.begin(), l.end(), k), l.end());
@@ -1016,7 +1065,7 @@ Plan* get_plan(t2v_unet* u, int B, int F, int h, int w, int L, cudaStream_t stre
         Plan scratch;
         scratch.shard = plan->shard;
         arena.reset(nullptr, u->taps_enabled || getenv("T2V_ARENA_NO_REUSE") != nullptr);
-        if (build(u, &scratch, &arena, true, stream, B, F, h, w, L, &io) != 0) return nullptr;
+        if (build(u, &scratch, &arena, true, stream, B, F, h, w, L, &io, feats_B) != 0) return nullptr;
     }
     const size_t bytes = arena.peak() + (1 << 20);
     if (cudaMalloc(&plan->slab, bytes) != cudaSuccess) {
@@ -1025,7 +1074,7 @@ Plan* get_plan(t2v_unet* u, int B, int F, int h, int w, int L, cudaStream_t stre
     }
     plan->slab_bytes = bytes;
     arena.reset(plan->slab, u->taps_enabled || getenv("T2V_ARENA_NO_REUSE") != nullptr);
-    if (build(u, plan.get(), &arena, false, stream, B, F, h, w, L, &io) != 0) return nullptr;
+    if (build(u, plan.get(), &arena, false, stream, B, F, h, w, L, &io, feats_B) != 0) return nullptr;
     plan->weights_version = u->params.version();
     Plan* raw = plan.get();
     g_io[raw] = io;
@@ -1107,15 +1156,18 @@ int t2v_unet_param_info(t2v_unet* u, int index, char* name_out, size_t name_cap,
     return n;
 }
 
-int t2v_unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, void* out,
-                     int out_is_f32, int B, int F, int h, int w, int L, void* stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    clear_pending_error("t2v_unet_forward");
+}  // extern "C"
+
+namespace t2v {
+namespace {
+
+int unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, const void* const* feats, int feats_B,
+                 void* out, int out_is_f32, int B, int F, int h, int w, int L, cudaStream_t stream) {
     if (u->cfg.arch == 1 && F > 32) {
         set_error("VideoCrafter temporal attention kernel: at most 32 frames per clip (got %d)", F);
         return -4;
     }
-    Plan* plan = get_plan(u, B, F, h, w, L, stream);
+    Plan* plan = get_plan(u, B, F, h, w, L, stream, feats_B);
     if (!plan) return -1;
     auto io_it = g_io.find(plan);
     if (io_it == g_io.end()) {
@@ -1139,6 +1191,8 @@ int t2v_unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, c
     cudaMemcpyAsync(io.t, t, sizeof(float) * B, cudaMemcpyDeviceToDevice, stream);
     cudaMemcpyAsync(io.ctx, ctx, static_cast<size_t>(B) * L * cfg.context_dim * sizeof(__half), cudaMemcpyDeviceToDevice,
                     stream);
+    for (int i = 0; i < io.n_feat; ++i)
+        cudaMemcpyAsync(io.feat[i], feats[i], static_cast<size_t>(io.feat_elems[i]) * sizeof(__half), cudaMemcpyDeviceToDevice, stream);
     rc = run_plan(plan, stream, !u->taps_enabled);
     if (rc != 0) {
         set_error("UNet launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
@@ -1148,6 +1202,47 @@ int t2v_unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, c
     u->last_exchanges = plan->shard ? plan->shard->n_xchg : 0;
     const int out_ld = (cfg.out_dim % 8 == 0) ? cfg.out_dim : (cfg.out_dim + 7) / 8 * 8;
     return egress_latent(io.out_tok, out_ld, out, out_is_f32, B, cfg.out_dim, F, h, w, stream);
+}
+
+}  // namespace
+}  // namespace t2v
+
+extern "C" {
+
+int t2v_unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, void* out,
+                     int out_is_f32, int B, int F, int h, int w, int L, void* stream_) {
+    clear_pending_error("t2v_unet_forward");
+    return unet_forward(u, x, x_is_f32, t, ctx, nullptr, 0, out, out_is_f32, B, F, h, w, L, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+int t2v_unet_forward_adapter(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx,
+                             const void* const* feats, int n_feats, int feats_B, void* out, int out_is_f32, int B, int F, int h,
+                             int w, int L, void* stream_) {
+    clear_pending_error("t2v_unet_forward_adapter");
+    if (u->cfg.arch != 1) {
+        set_error("adapter features are a VideoCrafter UNetModel input (arch 1); this denoiser is arch %d", u->cfg.arch);
+        return -2;
+    }
+    const int want = n_feature_blocks(u);
+    if (n_feats != want) {
+        set_error("adapter features: got %d feature maps, the UNet adds one after each of its %d input blocks with (id + 1) %% 3 == 0",
+                  n_feats, want);
+        return -2;
+    }
+    if (feats_B < 1 || B % feats_B != 0) {
+        set_error("adapter features: feature batch %d does not divide the forward batch %d", feats_B, B);
+        return -2;
+    }
+    if (feats == nullptr) {
+        set_error("adapter features: null feature list");
+        return -2;
+    }
+    for (int i = 0; i < n_feats; ++i)
+        if (feats[i] == nullptr) {
+            set_error("adapter features: feature %d is a null pointer", i);
+            return -2;
+        }
+    return unet_forward(u, x, x_is_f32, t, ctx, feats, feats_B, out, out_is_f32, B, F, h, w, L, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 double t2v_unet_flops(t2v_unet* u, int B, int F, int h, int w, int L) {

@@ -24,6 +24,7 @@ SIGNATURES = {
     't2v_unet_missing_params': (c_int, [P, c_char_p, C.c_size_t]),
     't2v_unet_param_info': (c_int, [P, c_int, c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(c_int)]),
     't2v_unet_forward': (c_int, [P, P, c_int, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
+    't2v_unet_forward_adapter': (c_int, [P, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     't2v_unet_flops': (c_double, [P, c_int, c_int, c_int, c_int, c_int]),
     't2v_unet_num_launches': (c_int, [P]),
     't2v_unet_profile': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, C.POINTER(c_double)]),
@@ -52,6 +53,12 @@ SIGNATURES = {
     't2v_clip_set_param': (c_int, [P, c_char_p, P, c_int, c_int, C.POINTER(C.c_int64), P]),
     't2v_clip_param_info': (c_int, [P, c_int, c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(c_int)]),
     't2v_clip_encode': (c_int, [P, P, P, c_int, c_int, P]),
+    't2v_adapter_create': (c_int, [P, C.POINTER(P)]),
+    't2v_adapter_destroy': (None, [P]),
+    't2v_adapter_set_param': (c_int, [P, c_char_p, P, c_int, c_int, C.POINTER(C.c_int64), P]),
+    't2v_adapter_missing_params': (c_int, [P, c_char_p, C.c_size_t]),
+    't2v_adapter_param_info': (c_int, [P, c_int, c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(c_int)]),
+    't2v_adapter_encode': (c_int, [P, P, c_int, P, c_int, c_int, c_int, P]),
     't2v_ddim_step': (c_int, [P, P, P, c_int, P, c_ll, c_ll, c_int, c_int, c_float, c_int, c_float, c_float, c_float, c_float,
                               c_float, P, c_int, P]),
     't2v_cfg_x0': (c_int, [P, P, P, c_int, P, c_ll, c_float, c_float, c_float, c_int, P]),
@@ -91,6 +98,11 @@ class ShardExportC(C.Structure):
 
 class ClipConfigC(C.Structure):
     _fields_ = [('width', c_int), ('heads', c_int), ('layers_run', c_int), ('context', c_int), ('vocab', c_int), ('arch', c_int)]
+
+
+class AdapterConfigC(C.Structure):
+    _fields_ = [('cin', c_int), ('channels', c_int * 4), ('n_levels', c_int), ('nums_rb', c_int), ('ksize', c_int), ('sk', c_int),
+                ('use_conv', c_int)]
 
 
 class VAEConfigC(C.Structure):

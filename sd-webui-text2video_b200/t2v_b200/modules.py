@@ -356,7 +356,7 @@ class UNetSD(_NativeModule):
 class UNetModel(UNetSD):
     """Drop-in for videocrafter/lvdm/models/modules/openaimodel3d.py::UNetModel as configured by
     base_t2v/model_config.yaml:21-46 (constructor keywords of that file; state_dict keys of `model.diffusion_model.*`).
-    `forward(x, timesteps, context=...)` -> eps, x [B,4,T,h,w], T <= 32 frames."""
+    `forward(x, timesteps, context=..., features_adapter=None)` -> eps, x [B,4,T,h,w], T <= 32 frames."""
 
     def __init__(self, image_size=32, in_channels=4, model_channels=320, out_channels=4, num_res_blocks=2,
                  attention_resolutions=(4, 2, 1), dropout=0, channel_mult=(1, 2, 4, 4), conv_resample=True, dims=3,
@@ -398,10 +398,92 @@ class UNetModel(UNetSD):
         self._init_native()
 
     @torch.no_grad()
-    def forward(self, x, timesteps=None, time_emb_replace=None, context=None, features_adapter=None, y=None, **kwargs):
-        if time_emb_replace is not None or features_adapter is not None or y is not None:
-            raise NotImplementedError('time_emb_replace / features_adapter / class labels are not part of the base_t2v path')
-        return UNetSD.forward(self, x, timesteps, context)
+    def forward(self, x, timesteps=None, time_emb_replace=None, context=None, features_adapter=None, y=None,
+                features_adapter_tiled=False, **kwargs):
+        """`features_adapter`: the T2I-Adapter's feature maps, one `b c t h w` tensor per input block with (id + 1) % 3 == 0
+        (openaimodel3d.py:654-663), added to h there on the library.  Their batch is 1 or B (torch broadcasting);
+        `features_adapter_tiled=True` also accepts any batch b dividing B, sample j reading feature sample j % b (the DDIM
+        sampler's batched cond / uncond pair)."""
+        if time_emb_replace is not None or y is not None:
+            raise NotImplementedError('time_emb_replace / class labels are not part of the base_t2v path')
+        if features_adapter is None:
+            return UNetSD.forward(self, x, timesteps, context)
+        return self._forward_adapter(x, timesteps, context, list(features_adapter), features_adapter_tiled)
+
+    def feature_shapes(self, T, h, w):
+        """[(C, T, h_i, w_i)] the UNet expects of each adapter feature for a [., ., T, h, w] latent."""
+        out, ch, hh, ww, idx = [], self.model_channels, h, w, 1
+        for level, mult in enumerate(self.dim_mult):
+            for _ in range(self.num_res_blocks):
+                ch = self.model_channels * mult
+                if (idx + 1) % 3 == 0:
+                    out.append((ch, T, hh, ww))
+                idx += 1
+            if level != len(self.dim_mult) - 1:
+                hh, ww = (hh + 1) // 2, (ww + 1) // 2
+                if (idx + 1) % 3 == 0:
+                    out.append((ch, T, hh, ww))
+                idx += 1
+        return out
+
+    def _channels_last(self, f):
+        """f [b, C, T, h, w] -> fp16 [b, T, h, w, C] contiguous: a view when f already has that layout (the Adapter's output),
+        else one copy per distinct tensor, cached by (data_ptr, version, shape, dtype) so a sampling loop copies nothing."""
+        cl = f.permute(0, 2, 3, 4, 1)
+        if f.dtype == torch.float16 and cl.is_contiguous():
+            return cl
+        cache = self.__dict__.setdefault('_feature_cache', {})
+        key = (f.data_ptr(), f._version, tuple(f.shape), tuple(f.stride()), f.dtype, f.device)
+        hit = cache.get(key)
+        if hit is not None and hit[0] is f:
+            return hit[1]
+        if len(cache) >= 16:
+            cache.clear()
+        out = cl.to(torch.float16).contiguous()
+        cache[key] = (f, out)            # holds f: its storage cannot be reused by another tensor while the entry lives
+        return out
+
+    def _forward_adapter(self, x, t, context, feats, tiled):
+        if x.dim() != 5:
+            raise ValueError('x must be [B, C, T, h, w]')
+        B, _, T, h, w = x.shape
+        want = self.feature_shapes(T, h, w)
+        if len(feats) != len(want):
+            raise ValueError(f'features_adapter: got {len(feats)} feature maps, this UNet adds {len(want)} '
+                             f'(one after each input block with (id + 1) % 3 == 0)')
+        fb = None
+        for i, (f, (c, tt, hh, ww)) in enumerate(zip(feats, want)):
+            if f.dim() != 5 or tuple(f.shape[1:]) != (c, tt, hh, ww):
+                raise ValueError(f'features_adapter[{i}]: shape {tuple(f.shape)} does not match h there, [B, {c}, {tt}, {hh}, {ww}] '
+                                 f'(adapter levels must follow the UNet: a latent of odd size needs use_conv=True)')
+            if fb is None:
+                fb = f.shape[0]
+            elif f.shape[0] != fb:
+                raise ValueError(f'features_adapter: feature batches differ ({fb} vs {f.shape[0]})')
+        if not (fb == 1 or fb == B or (tiled and B % fb == 0)):
+            raise ValueError(f'features_adapter: feature batch {fb} does not broadcast to the batch {B}')
+        staged = [self._channels_last(f.to(x.device) if f.device != x.device else f) for f in feats]
+        self.sync_weights()
+        l = _lib.lib()
+        if x.dtype not in (torch.float32, torch.float16):
+            x = x.float()
+        x = x.contiguous()
+        t = torch.as_tensor(t, device=x.device).reshape(-1).to(torch.float32)
+        if t.numel() == 1 and B > 1:
+            t = t.expand(B)
+        t = t.contiguous()
+        y = context.to(device=x.device, dtype=torch.float16)
+        if y.shape[0] == 1 and B > 1:
+            y = y.expand(B, -1, -1)
+        y = y.contiguous()
+        if y.shape[2] != self.context_dim:
+            raise ValueError(f'context dim {y.shape[2]} != {self.context_dim}')
+        out = torch.empty((B, self.out_dim, T, h, w), device=x.device, dtype=torch.float16)
+        ptrs = (C.c_void_p * len(staged))(*[s.data_ptr() for s in staged])
+        rc = l.t2v_unet_forward_adapter(self._handle, _lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(t), _lib.ptr(y), ptrs,
+                                        len(staged), fb, _lib.ptr(out), 0, B, T, h, w, y.shape[1], _lib.stream_ptr())
+        _lib.check(rc, 'unet_forward_adapter')
+        return out
 
 
 def _encoder_table(ch, ch_mult, num_res_blocks, in_channels, z_channels):

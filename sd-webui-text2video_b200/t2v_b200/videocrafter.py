@@ -13,6 +13,9 @@ Mirrors, with the reference's names / signatures for the calls on the path:
                            `p_sample_ddim`; per-step noise from the sampler's CPU `noise_gen`, util.py:321-325).
   * `sample_text2video`    videocrafter/sample_text2video.py:75-131, `make_model_input_shape` sample_utils.py:77-84.
   * `process_videocrafter` videocrafter/process_videocrafter.py:13-98 (the webui entry point).
+  * `T2VAdapterDepth`      ddpm3d.py:1436-1484 (depth-guided mode: the T2I-Adapter on the library, t2v_b200/adapter.py; the
+                           depth model is the caller's), `adapter_guided_synthesis` / `load_model_checkpoint`
+                           sample_text2video_adapter.py:20-137; `DDIMSampler.sample(features_adapter=...)` ddim.py:219-229.
 
 Arithmetic: the UNet runs in fp16 storage / fp32 accumulate (the reference runs this path in fp32; tolerance in
 tests/test_model_gpu.py), CFG `e_u + g (e_c - e_u)` and the DDIM update in fp32 inside ONE fused kernel per step
@@ -177,14 +180,19 @@ class DDIMSampler(object):
     @torch.no_grad()
     def sample(self, S, batch_size, shape, conditioning=None, callback=None, img_callback=None, eta=0.0, mask=None, x0=None,
                temperature=1.0, noise_dropout=0.0, verbose=True, schedule_verbose=False, x_T=None, log_every_t=100,
-               unconditional_guidance_scale=1.0, unconditional_conditioning=None, sample_noise=None, **kwargs):
+               unconditional_guidance_scale=1.0, unconditional_conditioning=None, sample_noise=None, features_adapter=None,
+               **kwargs):
+        """`features_adapter` (T2VAdapterDepth.get_adapter_features) reaches every apply_model call, conditional and
+        unconditional, as in ddim.py:219-229.  Other keywords of adapter_guided_synthesis (`temporal_length`,
+        `conditional_guidance_scale_temporal`) reach modules that ignore them in the reference: accepted and ignored."""
         if mask is not None or noise_dropout > 0.0 or kwargs.get('score_corrector') is not None or kwargs.get('cond_fn'):
             raise NotImplementedError('mask blending / noise dropout / score correctors are not on the text2video path')
         self.make_schedule(ddim_num_steps=S, ddim_eta=eta, verbose=schedule_verbose)
         size = (batch_size, *shape)
         return self.ddim_sampling(conditioning, size, callback=callback, img_callback=img_callback, temperature=temperature,
                                   x_T=x_T, log_every_t=log_every_t, unconditional_guidance_scale=unconditional_guidance_scale,
-                                  unconditional_conditioning=unconditional_conditioning, sample_noise=sample_noise)
+                                  unconditional_conditioning=unconditional_conditioning, sample_noise=sample_noise,
+                                  features_adapter=features_adapter)
 
     @staticmethod
     def _ctx(c):
@@ -194,22 +202,27 @@ class DDIMSampler(object):
             c = torch.cat(list(c), 1)
         return c
 
-    def _eps_pair(self, x, ts, cond, uncond):
-        """(e_t, e_t_uncond) of ddim.py:212-221 as ONE batched forward (the two evaluations are independent samples)."""
+    def _eps_pair(self, x, ts, cond, uncond, features_adapter=None):
+        """(e_t, e_t_uncond) of ddim.py:212-221 as ONE batched forward (the two evaluations are independent samples).  Adapter
+        features of batch b serve both halves of the 2b batch (sample j reads feature sample j % b)."""
         c, uc = self._ctx(cond), self._ctx(uncond)
         b = x.shape[0]
+        fa = {} if features_adapter is None else {'features_adapter': features_adapter}
         if _dist.cfg_split_enabled():       # one branch per GPU of a pair, one all-gather of eps per step (distributed.py)
             _, role, grp = _dist.cfg_pair()
-            return _dist.exchange_eps(self.model.apply_model(x, ts, c if role == 0 else uc), grp)
+            return _dist.exchange_eps(self.model.apply_model(x, ts, c if role == 0 else uc, **fa), grp)
         if c.shape == uc.shape:
-            out = self.model.apply_model(torch.cat([x, x], 0), torch.cat([ts, ts], 0), torch.cat([c, uc], 0))
+            tiled = {} if features_adapter is None else {'features_adapter_tiled': True}
+            out = self.model.apply_model(torch.cat([x, x], 0), torch.cat([ts, ts], 0), torch.cat([c, uc], 0), **fa, **tiled)
             return out[:b], out[b:]
-        return self.model.apply_model(x, ts, c), self.model.apply_model(x, ts, uc)
+        return self.model.apply_model(x, ts, c, **fa), self.model.apply_model(x, ts, uc, **fa)
 
     @torch.no_grad()
     def ddim_sampling(self, cond, shape, x_T=None, callback=None, img_callback=None, log_every_t=100, temperature=1.0,
-                      unconditional_guidance_scale=1.0, unconditional_conditioning=None, sample_noise=None, **kwargs):
+                      unconditional_guidance_scale=1.0, unconditional_conditioning=None, sample_noise=None, features_adapter=None,
+                      **kwargs):
         device = self.model.device
+        fa = {} if features_adapter is None else {'features_adapter': features_adapter}
         # NB the reference draws x_T from the GLOBAL RNG when it is not given (ddim.py:148-149); kept
         img = torch.randn(shape, device=device) if x_T is None else x_T
         _need_cuda(img)
@@ -224,9 +237,9 @@ class DDIMSampler(object):
             ts = torch.full((b,), int(step), device=device, dtype=torch.long)
             unguided = unconditional_conditioning is None or g == 1.0
             if unguided:
-                e_c, e_u = self.model.apply_model(img, ts, self._ctx(cond)), None
+                e_c, e_u = self.model.apply_model(img, ts, self._ctx(cond), **fa), None
             else:
-                e_c, e_u = self._eps_pair(img, ts, cond, unconditional_conditioning)
+                e_c, e_u = self._eps_pair(img, ts, cond, unconditional_conditioning, features_adapter)
             a_t, a_prev = _f32(self.ddim_alphas[index]), _f32(self.ddim_alphas_prev[index])
             sigma, s1m = _f32(self.ddim_sigmas[index]), _f32(self.ddim_sqrt_one_minus_alphas[index])
             if sample_noise is None:        # util.py:321-325: CPU generator, then moved to the device
@@ -309,3 +322,115 @@ def process_videocrafter(args_dict, model=None):
                                     show_denoising_progress=False, num_frames=a.frames, x_T=getattr(a, 'x_T', None))
         outputs.append(video_encoder(samples[0:1], a) if video_encoder is not None else samples[0:1])
     return outputs
+
+
+# ------------------------------------------------------------------------------------------------- depth-guided synthesis
+_MIDAS_HINT = ('the MiDaS depth model that VideoCrafter\'s depth_stage_config names is not part of VideoCrafter\'s source tree '
+               'and is not shipped here: pass depth_stage_model=<callable mapping [N, 3, 384, 384] frames in [-1, 1] to '
+               '[N, 1, h, w] depth>, e.g. a MiDaS DPT model you load yourself')
+
+
+def _build_depth_stage(config):
+    """instantiate_from_config(depth_stage_config) (lvdm/utils/common_utils.py) when its target is importable; else an error
+    that says what to pass instead."""
+    if config is None:
+        raise RuntimeError('T2VAdapterDepth: no depth_stage_config and no depth_stage_model; ' + _MIDAS_HINT)
+    cfg = _plain(config)
+    target = str(cfg.get('target', ''))
+    try:
+        import importlib
+        mod, cls = target.rsplit('.', 1)
+        return getattr(importlib.import_module(mod), cls)(**dict(cfg.get('params', None) or {}))
+    except Exception as e:
+        raise RuntimeError(f'T2VAdapterDepth: depth_stage_config target {target!r} cannot be built here ({type(e).__name__}: {e}); '
+                           + _MIDAS_HINT) from None
+
+
+class T2VAdapterDepth(LatentDiffusion):
+    """ddpm3d.py:1436-1484: LatentDiffusion + the T2I-Adapter (`self.adapter`, on the library) + a depth estimator.
+
+    `adapter_config` is the reference's {target, params, cond_name} (dict or OmegaConf); `params` go to t2v_b200.adapter.Adapter.
+    `depth_stage_model` is any callable [N, 3, 384, 384] -> [N, 1, h', w'] (a torch module is registered as a submodule, as
+    the reference's is); it runs once per clip in get_batch_depth and is caller-side torch, not part of the library.  Without
+    it, `depth_stage_config` must name something importable."""
+
+    def __init__(self, depth_stage_config, adapter_config, *args, depth_stage_model=None, **kwargs):
+        super().__init__(*args, **kwargs)
+        from .adapter import Adapter
+        acfg = _plain(adapter_config)
+        self.adapter = Adapter(**dict(acfg.get('params', None) or {}))
+        self.condtype = acfg.get('cond_name', None)
+        self.depth_stage_model = depth_stage_model if depth_stage_model is not None else _build_depth_stage(depth_stage_config)
+
+    def prepare_midas_input(self, batch_x):
+        # input: b,c,h,w
+        return torch.nn.functional.interpolate(batch_x, size=(384, 384), mode='bicubic')
+
+    @torch.no_grad()
+    def get_batch_depth(self, batch_x, target_size, encode_bs=1):
+        """batch_x [b, c, t, h, w] -> depth [b, 1, t, *target_size] in [-1, 1] per frame (ddpm3d.py:1448-1468)."""
+        b, c, t, h, w = batch_x.shape
+        merge_x = batch_x.permute(0, 2, 1, 3, 4).reshape(b * t, c, h, w)
+        dtype = next((p.dtype for p in getattr(self.depth_stage_model, 'parameters', lambda: iter(()))()), None)
+        cond_depth_list = []
+        for x in torch.split(merge_x, encode_bs, dim=0):
+            x_midas = self.prepare_midas_input(x)
+            cond_depth = self.depth_stage_model(x_midas if dtype is None else x_midas.to(dtype))
+            cond_depth = torch.nn.functional.interpolate(cond_depth, size=target_size, mode='bicubic', align_corners=False)
+            depth_min = torch.amin(cond_depth, dim=[1, 2, 3], keepdim=True)
+            depth_max = torch.amax(cond_depth, dim=[1, 2, 3], keepdim=True)
+            cond_depth_list.append(2. * (cond_depth - depth_min) / (depth_max - depth_min + 1e-7) - 1.)
+        d = torch.cat(cond_depth_list, dim=0)
+        return d.reshape(b, t, *d.shape[1:]).permute(0, 2, 1, 3, 4)
+
+    def get_adapter_features(self, extra_cond, encode_bs=1):
+        """extra_cond [b, c, t, h, w] -> one [b, C_l, t, h_l, w_l] feature per adapter level (ddpm3d.py:1470-1484).  All b*t
+        frames go through ONE library call (`encode_bs` only splits the work in the reference); the results are views of the
+        library's channels-last output, which UNetModel stages without a copy."""
+        b, c, t, h, w = extra_cond.shape
+        x = extra_cond.permute(0, 2, 1, 3, 4).reshape(b * t, c, h, w)
+        feats = self.adapter(x)
+        return [f.permute(0, 2, 3, 1).reshape(b, t, f.shape[2], f.shape[3], f.shape[1]).permute(0, 4, 1, 2, 3) for f in feats]
+
+
+@torch.no_grad()
+def adapter_guided_synthesis(model, prompts, videos, noise_shape, n_samples=1, ddim_steps=50, ddim_eta=1.,
+                             unconditional_guidance_scale=1.0, unconditional_guidance_scale_temporal=None, **kwargs):
+    """sample_text2video_adapter.py:96-137: depth of `videos` [b, 3, t, H, W] -> adapter features -> `n_samples` DDIM runs
+    guided by them -> decoded clips.  Returns (samples [b, n_samples, 3, t, H', W'], extra_cond [b, 1, t, H, W])."""
+    ddim_sampler = DDIMSampler(model)
+    batch_size = noise_shape[0]
+    if isinstance(prompts, str):
+        prompts = [prompts]
+    cond = model.get_learned_conditioning(prompts)
+    if unconditional_guidance_scale != 1.0:
+        uc = model.get_learned_conditioning(batch_size * [""])
+    else:
+        uc = None
+    b, c, t, h, w = videos.shape
+    extra_cond = model.get_batch_depth(videos, (h, w))
+    features_adapter = model.get_adapter_features(extra_cond)
+    batch_variants = []
+    for _ in range(n_samples):
+        samples, _ = ddim_sampler.sample(S=ddim_steps, conditioning=cond, batch_size=noise_shape[0], shape=noise_shape[1:],
+                                         verbose=False, unconditional_guidance_scale=unconditional_guidance_scale,
+                                         unconditional_conditioning=uc, eta=ddim_eta, temporal_length=noise_shape[2],
+                                         conditional_guidance_scale_temporal=unconditional_guidance_scale_temporal,
+                                         features_adapter=features_adapter, **kwargs)
+        batch_variants.append(model.decode_first_stage(samples, decode_bs=1, return_cpu=False))
+    batch_variants = torch.stack(batch_variants)
+    return batch_variants.permute(1, 0, 2, 3, 4, 5), extra_cond
+
+
+def load_model_checkpoint(model, ckpt, adapter_ckpt=None):
+    """sample_text2video_adapter.py:20-41: with an adapter checkpoint, the main model loads with strict=False (it has no
+    adapter.* keys) and `model.adapter` with strict=True; without one, the whole model loads strictly."""
+    def _sd(path):
+        sd = torch.load(path, map_location='cpu')
+        return sd['state_dict'] if 'state_dict' in list(sd.keys()) else sd
+    if adapter_ckpt:
+        model.load_state_dict(_sd(ckpt), strict=False)
+        model.adapter.load_state_dict(_sd(adapter_ckpt), strict=True)
+    else:
+        model.load_state_dict(_sd(ckpt), strict=True)
+    return model
