@@ -37,8 +37,7 @@ struct AdapterIO {
 struct t2v_adapter {
     t2v_adapter_config cfg;
     ParamStore params;
-    std::map<std::string, std::unique_ptr<Plan>> plans;      // key: "N,H,W"
-    std::map<Plan*, AdapterIO> io;
+    PlanCache<AdapterIO> plans{4};      // key: "N,H,W"
 };
 
 namespace t2v {
@@ -166,42 +165,12 @@ int build(t2v_adapter* a, Plan* plan, Arena* arena, bool dry, cudaStream_t strea
     return bld.error;
 }
 
-Plan* get_plan(t2v_adapter* a, int N, int H, int W, cudaStream_t stream) {
-    char key[64];
-    snprintf(key, sizeof(key), "%d,%d,%d", N, H, W);
-    auto it = a->plans.find(key);
-    if (it != a->plans.end() && it->second->weights_version == a->params.version()) return it->second.get();
-    if (it != a->plans.end()) {
-        a->io.erase(it->second.get());
-        a->plans.erase(it);
-    }
-    std::string miss;
-    if (a->params.missing(&miss) > 0) {
-        set_error("Adapter parameters missing (e.g. '%s')", miss.c_str());
-        return nullptr;
-    }
-    std::unique_ptr<Plan> plan(new Plan());
-    Arena arena;
-    AdapterIO io;
-    {
-        Plan scratch;
-        arena.reset(nullptr, false);
-        if (build(a, &scratch, &arena, true, stream, N, H, W, &io) != 0) return nullptr;
-    }
-    const size_t bytes = arena.peak() + (1 << 20);
-    if (cudaMalloc(&plan->slab, bytes) != cudaSuccess) {
-        set_error("Adapter activation slab cudaMalloc(%zu MB) failed", bytes >> 20);
-        return nullptr;
-    }
-    plan->slab_bytes = bytes;
-    arena.reset(plan->slab, false);
-    io = AdapterIO();
-    if (build(a, plan.get(), &arena, false, stream, N, H, W, &io) != 0) return nullptr;
-    plan->weights_version = a->params.version();
-    Plan* raw = plan.get();
-    a->io[raw] = io;
-    a->plans[key] = std::move(plan);
-    return raw;
+PlanCache<AdapterIO>::Entry* get_plan(t2v_adapter* a, int N, int H, int W, cudaStream_t stream) {
+    const std::string key = std::to_string(N) + "," + std::to_string(H) + "," + std::to_string(W);
+    if (auto* e = a->plans.find(key, a->params.version())) return e;
+    if (!a->params.complete("Adapter")) return nullptr;
+    return a->plans.build(key, a->params.version(), stream, std::unique_ptr<Plan>(new Plan()), false, "Adapter",
+                          [&](Plan* p, Arena* ar, bool dry, AdapterIO* io) { return build(a, p, ar, dry, stream, N, H, W, io); });
 }
 
 }  // namespace
@@ -250,28 +219,11 @@ int t2v_adapter_set_param(t2v_adapter* a, const char* name, const void* data, in
 }
 
 int t2v_adapter_missing_params(t2v_adapter* a, char* name_out, size_t name_cap) {
-    std::string one;
-    const int n = a->params.missing(&one);
-    if (name_out && name_cap > 0) {
-        strncpy(name_out, one.c_str(), name_cap - 1);
-        name_out[name_cap - 1] = 0;
-    }
-    return n;
+    return missing_params_out(a->params, name_out, name_cap);
 }
 
 int t2v_adapter_param_info(t2v_adapter* a, int index, char* name_out, size_t name_cap, int64_t* shape_out, int* ndim_out) {
-    std::string name;
-    std::vector<long long> shape;
-    const int n = a->params.info(index, &name, &shape);
-    if (n < 0) return -1;
-    if (name_out && name_cap > 0) {
-        strncpy(name_out, name.c_str(), name_cap - 1);
-        name_out[name_cap - 1] = 0;
-    }
-    if (ndim_out) *ndim_out = static_cast<int>(shape.size());
-    if (shape_out)
-        for (size_t i = 0; i < shape.size() && i < 8; ++i) shape_out[i] = shape[i];
-    return n;
+    return param_info_out(a->params, index, name_out, name_cap, shape_out, ndim_out);
 }
 
 int t2v_adapter_encode(t2v_adapter* a, const void* cond, int cond_is_f32, void* const* feats_out, int N, int H, int W,
@@ -292,12 +244,12 @@ int t2v_adapter_encode(t2v_adapter* a, const void* cond, int cond_is_f32, void* 
                       cfg.use_conv ? "stride-2 convs" : "2x2 average pooling");
             return -3;
         }
-    Plan* plan = get_plan(a, N, H, W, stream);
-    if (!plan) return -1;
-    const AdapterIO& io = a->io[plan];
+    auto* entry = get_plan(a, N, H, W, stream);
+    if (!entry) return -1;
+    const AdapterIO& io = entry->io;
     int rc = pixel_unshuffle_ingest(cond, cond_is_f32, io.cond_tok, N, cfg.cin / 64, H, W, stream);
     if (rc != 0) return rc;
-    rc = run_plan(plan, stream, true);
+    rc = run_plan(entry->plan.get(), stream, true);
     if (rc != 0) {
         set_error("Adapter launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
         return rc;

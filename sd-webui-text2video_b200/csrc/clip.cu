@@ -21,13 +21,23 @@
 #include <cstring>
 #include <memory>
 
+namespace t2v {
+namespace {
+
+struct ClipIO {
+    int* tokens;        // token staging [B * L]
+    __half* out;        // output tokens [B * L, width]
+};
+
+}  // namespace
+}  // namespace t2v
+
 using namespace t2v;
 
 struct t2v_clip {
     t2v_clip_config cfg;
     ParamStore params;
-    std::map<int, std::unique_ptr<Plan>> plans;       // key: batch
-    std::map<Plan*, std::pair<int*, __half*>> io;      // plan -> (token staging, output tokens)
+    PlanCache<ClipIO> plans{4};       // key: batch
 };
 
 namespace t2v {
@@ -222,7 +232,7 @@ void expect_params(t2v_clip* m) {
     P.expect("ln_final.bias", {c.width});
 }
 
-int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, int B, int** tok_out, __half** out_tok) {
+int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, int B, ClipIO* io) {
     Builder bld(plan, arena, dry, num_sms());
     NetCtx c{&m->params, &bld, stream, nullptr};
     const t2v_clip_config& cfg = m->cfg;
@@ -230,7 +240,7 @@ int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     const int L = cfg.context, W = cfg.width, heads = cfg.heads;
     const long long R = static_cast<long long>(B) * L;
     int* tokens = reinterpret_cast<int*>(bld.alloc_bytes(static_cast<size_t>(R) * sizeof(int)));
-    *tok_out = tokens;
+    io->tokens = tokens;
     Tok x = bld.alloc(R, W);
     {
         const __half* emb = prm(c, hf ? kHfEmb : "token_embedding.weight");
@@ -292,44 +302,16 @@ int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     }
     Tok z = layer_norm(c, x, hf ? kHfFinal : "ln_final");
     bld.free(x);
-    *out_tok = z.p;
+    io->out = z.p;
     return bld.error;
 }
 
-Plan* get_plan(t2v_clip* m, int B, cudaStream_t stream) {
-    auto it = m->plans.find(B);
-    if (it != m->plans.end() && it->second->weights_version == m->params.version()) return it->second.get();
-    if (it != m->plans.end()) {
-        m->io.erase(it->second.get());
-        m->plans.erase(it);
-    }
-    std::string miss;
-    if (m->params.missing(&miss) > 0) {
-        set_error("CLIP text tower parameters missing (e.g. '%s')", miss.c_str());
-        return nullptr;
-    }
-    std::unique_ptr<Plan> plan(new Plan());
-    Arena arena;
-    int* tok = nullptr;
-    __half* out = nullptr;
-    {
-        Plan scratch;
-        arena.reset(nullptr, false);
-        if (build(m, &scratch, &arena, true, stream, B, &tok, &out) != 0) return nullptr;
-    }
-    const size_t bytes = arena.peak() + (1 << 20);
-    if (cudaMalloc(&plan->slab, bytes) != cudaSuccess) {
-        set_error("CLIP activation slab cudaMalloc(%zu MB) failed", bytes >> 20);
-        return nullptr;
-    }
-    plan->slab_bytes = bytes;
-    arena.reset(plan->slab, false);
-    if (build(m, plan.get(), &arena, false, stream, B, &tok, &out) != 0) return nullptr;
-    plan->weights_version = m->params.version();
-    Plan* raw = plan.get();
-    m->io[raw] = {tok, out};
-    m->plans[B] = std::move(plan);
-    return raw;
+PlanCache<ClipIO>::Entry* get_plan(t2v_clip* m, int B, cudaStream_t stream) {
+    const std::string key = std::to_string(B);
+    if (auto* e = m->plans.find(key, m->params.version())) return e;
+    if (!m->params.complete("CLIP text tower")) return nullptr;
+    return m->plans.build(key, m->params.version(), stream, std::unique_ptr<Plan>(new Plan()), false, "CLIP",
+                          [&](Plan* p, Arena* a, bool dry, ClipIO* io) { return build(m, p, a, dry, stream, B, io); });
 }
 
 __global__ void clip_out_kernel(const __half* __restrict__ z, void* __restrict__ out, int out_is_f32, long long n) {
@@ -368,34 +350,23 @@ int t2v_clip_set_param(t2v_clip* m, const char* name, const void* data, int dtyp
 }
 
 int t2v_clip_param_info(t2v_clip* m, int index, char* name_out, size_t name_cap, int64_t* shape_out, int* ndim_out) {
-    std::string name;
-    std::vector<long long> shape;
-    const int n = m->params.info(index, &name, &shape);
-    if (n < 0) return -1;
-    if (name_out && name_cap > 0) {
-        strncpy(name_out, name.c_str(), name_cap - 1);
-        name_out[name_cap - 1] = 0;
-    }
-    if (ndim_out) *ndim_out = static_cast<int>(shape.size());
-    if (shape_out)
-        for (size_t i = 0; i < shape.size() && i < 8; ++i) shape_out[i] = shape[i];
-    return n;
+    return param_info_out(m->params, index, name_out, name_cap, shape_out, ndim_out);
 }
 
 int t2v_clip_encode(t2v_clip* m, const int* tokens, void* out, int out_is_f32, int B, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    Plan* plan = get_plan(m, B, stream);
-    if (!plan) return -1;
-    const auto& io = m->io[plan];
+    auto* entry = get_plan(m, B, stream);
+    if (!entry) return -1;
+    const ClipIO& io = entry->io;
     const long long R = static_cast<long long>(B) * m->cfg.context;
-    cudaMemcpyAsync(io.first, tokens, static_cast<size_t>(R) * sizeof(int), cudaMemcpyDeviceToDevice, stream);
-    const int rc = run_plan(plan, stream, true);
+    cudaMemcpyAsync(io.tokens, tokens, static_cast<size_t>(R) * sizeof(int), cudaMemcpyDeviceToDevice, stream);
+    const int rc = run_plan(entry->plan.get(), stream, true);
     if (rc != 0) {
         set_error("CLIP launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
         return rc;
     }
     const long long n = R * m->cfg.width;
-    clip_out_kernel<<<static_cast<unsigned>((n + 255) / 256 > 4096 ? 4096 : (n + 255) / 256), 256, 0, stream>>>(io.second, out, out_is_f32, n);
+    clip_out_kernel<<<static_cast<unsigned>((n + 255) / 256 > 4096 ? 4096 : (n + 255) / 256), 256, 0, stream>>>(io.out, out, out_is_f32, n);
     return launch_status("clip launch");
 }
 

@@ -169,6 +169,39 @@ int ParamStore::missing(std::string* one) const {
     return n;
 }
 
+bool ParamStore::complete(const char* what) const {
+    std::string miss;
+    if (missing(&miss) == 0) return true;
+    set_error("%s parameters missing (e.g. '%s')", what, miss.c_str());
+    return false;
+}
+
+static void copy_name(const std::string& name, char* out, size_t cap) {
+    if (out && cap > 0) {
+        strncpy(out, name.c_str(), cap - 1);
+        out[cap - 1] = 0;
+    }
+}
+
+int param_info_out(const ParamStore& P, int index, char* name_out, size_t name_cap, int64_t* shape_out, int* ndim_out) {
+    std::string name;
+    std::vector<long long> shape;
+    const int n = P.info(index, &name, &shape);
+    if (n < 0) return -1;
+    copy_name(name, name_out, name_cap);
+    if (ndim_out) *ndim_out = static_cast<int>(shape.size());
+    if (shape_out)
+        for (size_t i = 0; i < shape.size() && i < 8; ++i) shape_out[i] = shape[i];
+    return n;
+}
+
+int missing_params_out(const ParamStore& P, char* name_out, size_t name_cap) {
+    std::string one;
+    const int n = P.missing(&one);
+    copy_name(one, name_out, name_cap);
+    return n;
+}
+
 int ParamStore::info(int index, std::string* name, std::vector<long long>* shape) const {
     int i = 0, n = 0;
     bool found = false;
@@ -437,6 +470,51 @@ int run_plan(Plan* plan, cudaStream_t stream, bool allow_graph) {
     }
     plan->eager_runs += 1;
     return 0;
+}
+
+long long dry_build(const std::shared_ptr<PlanShard>& shard, bool no_reuse, const BuildFn& build, double* flops) {
+    Plan scratch;
+    scratch.shard = shard;
+    Arena arena;
+    arena.reset(nullptr, no_reuse);
+    if (build(&scratch, &arena, true) != 0) return -1;
+    if (flops) *flops = scratch.flops;
+    return static_cast<long long>(arena.peak());
+}
+
+int build_plan(Plan* plan, unsigned long long weights_version, bool no_reuse, const char* label, const BuildFn& build) {
+    const long long peak = dry_build(plan->shard, no_reuse, build);
+    if (peak < 0) return -1;
+    const size_t bytes = static_cast<size_t>(peak) + (1 << 20);
+    if (cudaMalloc(&plan->slab, bytes) != cudaSuccess) {
+        plan->slab = nullptr;
+        set_error("%s activation slab cudaMalloc(%zu MB) failed", label, bytes >> 20);
+        return -1;
+    }
+    plan->slab_bytes = bytes;
+    Arena arena;
+    arena.reset(plan->slab, no_reuse);
+    if (build(plan, &arena, false) != 0) return -1;
+    plan->weights_version = weights_version;
+    return 0;
+}
+
+GnWorkspace::~GnWorkspace() {
+    if (ptr) cudaFree(ptr);
+}
+
+bool GnWorkspace::ensure(size_t need, cudaStream_t stream) {
+    if (need <= bytes) return false;
+    if (ptr) cudaFree(ptr);
+    bytes = 0;
+    if (cudaMalloc(&ptr, need) != cudaSuccess) {
+        ptr = nullptr;
+        set_error("groupnorm workspace cudaMalloc failed");
+        return true;
+    }
+    cudaMemsetAsync(ptr, 0, need, stream);
+    bytes = need;
+    return true;
 }
 
 void taps_3x3(GemmProblem& p) {

@@ -1,6 +1,7 @@
-// Host runtime shared by the denoiser and the VAE decoder: parameter store, packed-weight cache, a lifetime-aware
-// activation arena, and the "plan" -- a flat list of pre-encoded kernel launches (tensor maps encoded once per
-// shape) that one forward replays on a stream without any host-side shape logic.
+// Host runtime shared by every network of the library (UNet, VAE decoder and encoder, text towers, adapter): parameter
+// store, packed-weight cache, a lifetime-aware activation arena, the "plan" -- a flat list of pre-encoded kernel launches
+// (tensor maps encoded once per shape) that one forward replays on a stream without any host-side shape logic -- and the
+// per-handle cache of those plans.
 #pragma once
 #include "common.cuh"
 #include "gemm_tc.cuh"
@@ -10,7 +11,9 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <functional>
+#include <list>
 #include <map>
 #include <memory>
 #include <set>
@@ -43,6 +46,7 @@ public:
     void expect(const std::string& name, std::vector<long long> shape);
     int set(const std::string& name, const void* src, int dtype, int ndim, const int64_t* shape, cudaStream_t s);
     int missing(std::string* one) const;
+    bool complete(const char* what) const;      // false, with "<what> parameters missing (e.g. '<name>')" set, until all are set
     int info(int index, std::string* name, std::vector<long long>* shape) const;   // returns count, -1 if out of range
     const Param& get(const std::string& name) const;     // aborts via set_error + null data if absent
     bool has(const std::string& name) const { return params_.count(name) != 0; }
@@ -69,6 +73,12 @@ private:
     std::vector<PackRecipe> recipes_;
     unsigned long long version_ = 0;
 };
+
+// The C out-parameters of the handles' *_param_info / *_missing_params entry points.  param_info_out copies parameter
+// `index` of `P` (name, ndim, up to 8 dims) and returns P's count, -1 if out of range; missing_params_out copies the name
+// of one missing parameter and returns how many are missing.
+int param_info_out(const ParamStore& P, int index, char* name_out, size_t name_cap, int64_t* shape_out, int* ndim_out);
+int missing_params_out(const ParamStore& P, char* name_out, size_t name_cap);
 
 // ----------------------------------------------------------------------------------------- arena
 // Offsets are handed out by a first-fit free list while the plan is being built (the build order IS the execution
@@ -197,6 +207,81 @@ int profile_plan(Plan* plan, cudaStream_t stream, double* out13);
 // CUDA graph (through a private capture stream: the caller's may be the legacy default stream) and from then on a
 // forward is ONE cudaGraphLaunch -- the ~1k launches stop costing host time.  T2V_NO_GRAPH=1 disables it.
 int run_plan(Plan* plan, cudaStream_t stream, bool allow_graph);
+
+// ----------------------------------------------------------------------------------------- plan building and caching
+// A network's plan builder: records (or, when `dry`, only counts) its launches into the plan, allocating from the arena.
+using BuildFn = std::function<int(Plan* plan, Arena* arena, bool dry)>;
+
+// The dry pass alone, on a scratch plan sharing `shard`: returns the peak activation bytes (-1 if the build failed) and
+// stores the plan's algorithmic flop count in *flops.
+long long dry_build(const std::shared_ptr<PlanShard>& shard, bool no_reuse, const BuildFn& build, double* flops = nullptr);
+// Builds `plan` (a shell: the caller may have set its shard): the dry pass measures the peak, one slab of peak + 1 MB is
+// allocated, the real pass records the launches against it, and the plan is stamped with `weights_version`.  `label`
+// names the network in the error message of a failed slab allocation.  Returns 0, or < 0 with the error set.
+int build_plan(Plan* plan, unsigned long long weights_version, bool no_reuse, const char* label, const BuildFn& build);
+
+// One handle's plans, each with its I/O staging record (where the inputs and outputs sit inside the plan's slab), keyed by
+// shape and built for one weights version.  Every plan owns an activation slab (GBs at video shapes) and an instantiated
+// graph, so at most `bound` are kept, evicting the least recently used.
+template <class IO>
+class PlanCache {
+public:
+    struct Entry {
+        std::string key;
+        std::unique_ptr<Plan> plan;
+        IO io{};
+    };
+    explicit PlanCache(int bound) : bound_(static_cast<size_t>(std::max(bound, 1))) {}
+
+    // The plan of `key` built for weights `version`, made the most recently used; null if there is none.
+    Entry* find(const std::string& key, unsigned long long version) {
+        for (auto it = entries_.begin(); it != entries_.end(); ++it)
+            if (it->key == key && it->plan->weights_version == version) {
+                entries_.splice(entries_.end(), entries_, it);
+                return &entries_.back();
+            }
+        return nullptr;
+    }
+    // Builds the plan of `key` from `shell` with build_plan, `fn(plan, arena, dry, &io)` filling the entry's I/O record, and
+    // keeps it as the most recently used.  First drops every plan of an older weights version (versions only grow, so such
+    // a plan can never be replayed again) and then the least recently used ones down to the bound.  Null on failure.
+    template <class F>
+    Entry* build(const std::string& key, unsigned long long version, cudaStream_t stream, std::unique_ptr<Plan> shell,
+                 bool no_reuse, const char* label, F&& fn) {
+        auto stale = [&](const Entry& e) { return e.plan->weights_version != version || e.key == key; };
+        if (entries_.size() >= bound_ || std::any_of(entries_.begin(), entries_.end(), stale))
+            cudaStreamSynchronize(stream);          // a plan about to be destroyed may still be in flight on this stream
+        entries_.remove_if(stale);
+        while (entries_.size() >= bound_) entries_.pop_front();
+        Entry e{key, std::move(shell)};
+        const int rc = build_plan(e.plan.get(), version, no_reuse, label,
+                                  [&](Plan* p, Arena* a, bool dry) { return fn(p, a, dry, &e.io); });
+        if (rc != 0) return nullptr;
+        entries_.push_back(std::move(e));
+        return &entries_.back();
+    }
+    Entry* latest() { return entries_.empty() ? nullptr : &entries_.back(); }      // the most recently used; null if none
+    // Drops every plan (shard setup; a grown workspace that the plans captured by its old pointer).
+    void clear(cudaStream_t stream) {
+        if (entries_.empty()) return;
+        cudaStreamSynchronize(stream);
+        entries_.clear();
+    }
+
+private:
+    size_t bound_;
+    std::list<Entry> entries_;      // least recently used first
+};
+
+// The zero-initialised GroupNorm workspace (partials, statistics, counters) a handle's plans capture by pointer.
+struct GnWorkspace {
+    void* ptr = nullptr;
+    size_t bytes = 0;
+    ~GnWorkspace();
+    // Grows the workspace to at least `need` bytes, zeroed on `stream`.  Returns true if the old pointer is gone (the
+    // plans that captured it must be dropped); ptr is null if the allocation failed (error set).
+    bool ensure(size_t need, cudaStream_t stream);
+};
 
 // conv taps helpers over row dims (w, h, frames) and (pixels, frames, samples)
 void taps_3x3(GemmProblem& p);

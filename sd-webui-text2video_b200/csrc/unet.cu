@@ -26,6 +26,24 @@ struct Blk {
     int cin = 0, cout = 0, heads = 0, inner = 0;
 };
 
+constexpr int kMaxFeat = 8;
+
+struct IO {
+    __half* x_tok;      // [R, 8]
+    float* t;           // [B]
+    __half* ctx;        // [B*L, context_dim]
+    __half* out_tok;    // [R, 8]
+    // adapter features (plans built with feats_B > 0): staging [feats_B * F * h_i * w_i, C_i] per injection point
+    int n_feat = 0;
+    __half* feat[kMaxFeat] = {nullptr};
+    long long feat_elems[kMaxFeat] = {0};
+};
+
+int max_plans() {
+    static const int n = getenv("T2V_MAX_PLANS") ? std::max(1, atoi(getenv("T2V_MAX_PLANS"))) : 4;
+    return n;
+}
+
 }  // namespace
 
 }  // namespace t2v
@@ -37,22 +55,18 @@ struct t2v_unet {
     ParamStore params;
     std::vector<std::vector<Blk>> ins, outs;
     std::vector<Blk> mid;
-    std::map<std::string, std::unique_ptr<Plan>> plans;      // key: "B,F,h,w,L"
-    std::vector<std::string> plan_lru;                       // most recently used last; bounded (T2V_MAX_PLANS, default 4)
+    PlanCache<IO> plans{max_plans()};                        // key: plan_key()
     bool taps_enabled = false;
     int last_launches = 0;
     int last_exchanges = 0;
-    // fixed staging for graph replay
-    void* gn_ws = nullptr;
-    size_t gn_ws_bytes = 0;
+    GnWorkspace gn_ws;
     // frame-sharded clip (shard.cuh): one rank of `peers.nranks`, comm = this rank's IPC-shared flag / GroupNorm region
     bool shard_on = false;
     ShardPeers peers;
     ShardComm* comm = nullptr;
     t2v_unet() { memset(&peers, 0, sizeof(peers)); }
     ~t2v_unet() {
-        plans.clear();                      // closes the peers' slab mappings before the comm mappings go
-        if (gn_ws) cudaFree(gn_ws);
+        plans.clear(nullptr);               // closes the peers' slab mappings before the comm mappings go
         for (int r = 0; r < SHARD_MAX_RANKS; ++r)
             if (peers.comm[r] != nullptr && peers.comm[r] != comm) cudaIpcCloseMemHandle(peers.comm[r]);
         if (comm) cudaFree(comm);
@@ -771,19 +785,6 @@ Tok upsample(Ctx& c, const Tok& x, const Blk& blk, int hcur, int wcur) {
     return y;
 }
 
-constexpr int kMaxFeat = 8;
-
-struct IO {
-    __half* x_tok;      // [R, 8]
-    float* t;           // [B]
-    __half* ctx;        // [B*L, context_dim]
-    __half* out_tok;    // [R, 8]
-    // adapter features (plans built with feats_B > 0): staging [feats_B * F * h_i * w_i, C_i] per injection point
-    int n_feat = 0;
-    __half* feat[kMaxFeat] = {nullptr};
-    long long feat_elems[kMaxFeat] = {0};
-};
-
 // input blocks after which VideoCrafter's UNetModel adds an adapter feature (openaimodel3d.py:658): (id + 1) % 3 == 0
 bool feature_block(int id) { return (id + 1) % 3 == 0; }
 int n_feature_blocks(const t2v_unet* u) {
@@ -800,7 +801,7 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     c.params = &u->params;
     c.b = &bld;
     c.stream = stream;
-    c.gn_ws = u->gn_ws;
+    c.gn_ws = u->gn_ws.ptr;
     c.u = u;
     c.B = B; c.F = F; c.h = h; c.w = w; c.L = L;
     c.emb = nullptr; c.ctx = nullptr; c.plan = plan;
@@ -972,79 +973,37 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     return bld.error;
 }
 
-std::map<Plan*, IO> g_io;
-
-Plan* get_plan(t2v_unet* u, int B, int F, int h, int w, int L, cudaStream_t stream, int feats_B = 0) {
+// The plan-cache key of a forward shape.  The adapter-feature variant adds its feature batch (a forward without features
+// keeps its plan and key).
+std::string plan_key(const t2v_unet* u, int B, int F, int h, int w, int L, int feats_B) {
     char key[112];
     snprintf(key, sizeof(key), "%d,%d,%d,%d,%d,%d,%d/%d", B, F, h, w, L, u->taps_enabled ? 1 : 0, u->shard_on ? u->peers.rank : 0,
              u->shard_on ? u->peers.nranks : 1);
-    if (feats_B > 0) {                   // the adapter-feature variant (a forward without features keeps its plan and key)
+    if (feats_B > 0) {
         const size_t n = strlen(key);
         snprintf(key + n, sizeof(key) - n, ",a%d", feats_B);
     }
-    auto touch = [&](const std::string& k) {
-        auto& l = u->plan_lru;
-        l.erase(std::remove(l.begin(), l.end(), k), l.end());
-        l.push_back(k);
-    };
-    auto it = u->plans.find(key);
-    if (it != u->plans.end() && it->second->weights_version == u->params.version()) {
-        touch(key);
-        return it->second.get();
-    }
-    if (it != u->plans.end()) {
-        g_io.erase(it->second.get());
-        u->plans.erase(it);
-    }
-    {   // every plan owns an activation slab (GBs at video shapes) and an instantiated graph: keep only the most recently used
-        // few, and drop plans of an older weights version (they can never be replayed again)
-        static const int max_plans = getenv("T2V_MAX_PLANS") ? std::max(1, atoi(getenv("T2V_MAX_PLANS"))) : 4;
-        for (auto pit = u->plans.begin(); pit != u->plans.end();) {
-            if (pit->second->weights_version != u->params.version()) {
-                g_io.erase(pit->second.get());
-                u->plan_lru.erase(std::remove(u->plan_lru.begin(), u->plan_lru.end(), pit->first), u->plan_lru.end());
-                pit = u->plans.erase(pit);
-            } else {
-                ++pit;
-            }
-        }
-        while (static_cast<int>(u->plans.size()) >= max_plans && !u->plan_lru.empty()) {
-            const std::string victim = u->plan_lru.front();
-            u->plan_lru.erase(u->plan_lru.begin());
-            auto vit = u->plans.find(victim);
-            if (vit != u->plans.end()) {
-                cudaStreamSynchronize(stream);       // the victim's graph may still be in flight on this stream
-                g_io.erase(vit->second.get());
-                u->plans.erase(vit);
-            }
-        }
-    }
-    std::string miss;
-    if (u->params.missing(&miss) > 0) {
-        set_error("UNet parameters missing (e.g. '%s')", miss.c_str());
-        return nullptr;
-    }
+    return key;
+}
+
+// The frame partition of a sharded clip of F frames (null when the denoiser is not sharded).
+std::shared_ptr<PlanShard> new_plan_shard(const t2v_unet* u, int F) {
+    if (!u->shard_on) return nullptr;
+    std::shared_ptr<PlanShard> s(new PlanShard());
+    s->own_rank = u->peers.rank;
+    shard_partition(F, u->peers.nranks, s->fb);
+    return s;
+}
+
+PlanCache<IO>::Entry* get_plan(t2v_unet* u, int B, int F, int h, int w, int L, cudaStream_t stream, int feats_B = 0) {
+    const std::string key = plan_key(u, B, F, h, w, L, feats_B);
+    if (auto* e = u->plans.find(key, u->params.version())) return e;
+    if (!u->params.complete("UNet")) return nullptr;
     // groupnorm workspace: the largest (rows_per_inst, n_inst) pair is the per-sample 5-D norm at level 0
-    {
-        size_t need = std::max(gn_workspace_bytes(F * h * w, B, num_sms()), gn_workspace_bytes(h * w, B * F, num_sms()));
-        need = std::max(need, gn_workspace_bytes(1, B * F, num_sms()));
-        need += 1 << 20;
-        if (need > u->gn_ws_bytes) {
-            if (u->gn_ws) cudaFree(u->gn_ws);
-            if (cudaMalloc(&u->gn_ws, need) != cudaSuccess) {
-                set_error("groupnorm workspace cudaMalloc failed");
-                return nullptr;
-            }
-            cudaMemsetAsync(u->gn_ws, 0, need, stream);
-            u->gn_ws_bytes = need;
-            for (auto& kv : u->plans) g_io.erase(kv.second.get());     // only THIS denoiser's plans captured the old pointer
-            u->plans.clear();
-            u->plan_lru.clear();
-        }
-    }
-    std::unique_ptr<Plan> plan(new Plan());
-    Arena arena;
-    IO io;
+    size_t need = std::max(gn_workspace_bytes(F * h * w, B, num_sms()), gn_workspace_bytes(h * w, B * F, num_sms()));
+    need = std::max(need, gn_workspace_bytes(1, B * F, num_sms()));
+    if (u->gn_ws.ensure(need + (1 << 20), stream)) u->plans.clear(stream);
+    if (!u->gn_ws.ptr) return nullptr;
     if (u->shard_on) {
         if (u->cfg.arch != 0) {
             set_error("frame sharding is built for the ModelScope UNetSD (arch 0)");
@@ -1057,30 +1016,23 @@ Plan* get_plan(t2v_unet* u, int B, int F, int h, int w, int L, cudaStream_t stre
                       u->peers.nranks, u->peers.nranks, u->peers.nranks, deepest, SHARD_MAX_INST);
             return nullptr;
         }
-        plan->shard.reset(new PlanShard());
-        plan->shard->own_rank = u->peers.rank;
-        shard_partition(F, u->peers.nranks, plan->shard->fb);
     }
-    {   // dry pass: peak activation bytes
-        Plan scratch;
-        scratch.shard = plan->shard;
-        arena.reset(nullptr, u->taps_enabled || getenv("T2V_ARENA_NO_REUSE") != nullptr);
-        if (build(u, &scratch, &arena, true, stream, B, F, h, w, L, &io, feats_B) != 0) return nullptr;
+    std::unique_ptr<Plan> shell(new Plan());
+    shell->shard = new_plan_shard(u, F);
+    return u->plans.build(key, u->params.version(), stream, std::move(shell),
+                          u->taps_enabled || getenv("T2V_ARENA_NO_REUSE") != nullptr, "UNet",
+                          [&](Plan* p, Arena* a, bool dry, IO* io) { return build(u, p, a, dry, stream, B, F, h, w, L, io, feats_B); });
+}
+
+// A tap of the most recently used plan: (tokens, (h, w)); null, with the error set, if that plan has no such tap.
+const std::pair<Tok, std::pair<int, int>>* find_tap(t2v_unet* u, const char* name) {
+    auto* entry = u->plans.latest();
+    if (entry) {
+        auto it = entry->plan->taps.find(name);
+        if (it != entry->plan->taps.end()) return &it->second;
     }
-    const size_t bytes = arena.peak() + (1 << 20);
-    if (cudaMalloc(&plan->slab, bytes) != cudaSuccess) {
-        set_error("activation slab cudaMalloc(%zu MB) failed", bytes >> 20);
-        return nullptr;
-    }
-    plan->slab_bytes = bytes;
-    arena.reset(plan->slab, u->taps_enabled || getenv("T2V_ARENA_NO_REUSE") != nullptr);
-    if (build(u, plan.get(), &arena, false, stream, B, F, h, w, L, &io, feats_B) != 0) return nullptr;
-    plan->weights_version = u->params.version();
-    Plan* raw = plan.get();
-    g_io[raw] = io;
-    u->plans[key] = std::move(plan);
-    touch(key);
-    return raw;
+    set_error("tap '%s' not found (enable taps before the forward)", name);
+    return nullptr;
 }
 
 }  // namespace
@@ -1120,40 +1072,17 @@ int t2v_unet_create(const t2v_unet_config* cfg, t2v_unet** out) {
     return 0;
 }
 
-void t2v_unet_destroy(t2v_unet* u) {
-    if (!u) return;
-    for (auto& kv : u->plans) g_io.erase(kv.second.get());
-    delete u;
-}
+void t2v_unet_destroy(t2v_unet* u) { delete u; }
 
 int t2v_unet_set_param(t2v_unet* u, const char* name, const void* data, int dtype, int ndim, const int64_t* shape,
                        void* stream) {
     return u->params.set(name, data, dtype, ndim, shape, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int t2v_unet_missing_params(t2v_unet* u, char* name_out, size_t name_cap) {
-    std::string one;
-    const int n = u->params.missing(&one);
-    if (name_out && name_cap > 0) {
-        strncpy(name_out, one.c_str(), name_cap - 1);
-        name_out[name_cap - 1] = 0;
-    }
-    return n;
-}
+int t2v_unet_missing_params(t2v_unet* u, char* name_out, size_t name_cap) { return missing_params_out(u->params, name_out, name_cap); }
 
 int t2v_unet_param_info(t2v_unet* u, int index, char* name_out, size_t name_cap, int64_t* shape_out, int* ndim_out) {
-    std::string name;
-    std::vector<long long> shape;
-    const int n = u->params.info(index, &name, &shape);
-    if (n < 0) return -1;
-    if (name_out && name_cap > 0) {
-        strncpy(name_out, name.c_str(), name_cap - 1);
-        name_out[name_cap - 1] = 0;
-    }
-    if (ndim_out) *ndim_out = static_cast<int>(shape.size());
-    if (shape_out)
-        for (size_t i = 0; i < shape.size() && i < 8; ++i) shape_out[i] = shape[i];
-    return n;
+    return param_info_out(u->params, index, name_out, name_cap, shape_out, ndim_out);
 }
 
 }  // extern "C"
@@ -1167,14 +1096,10 @@ int unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const
         set_error("VideoCrafter temporal attention kernel: at most 32 frames per clip (got %d)", F);
         return -4;
     }
-    Plan* plan = get_plan(u, B, F, h, w, L, stream, feats_B);
-    if (!plan) return -1;
-    auto io_it = g_io.find(plan);
-    if (io_it == g_io.end()) {
-        set_error("internal: plan without I/O staging record");
-        return -6;
-    }
-    const IO& io = io_it->second;
+    auto* entry = get_plan(u, B, F, h, w, L, stream, feats_B);
+    if (!entry) return -1;
+    Plan* plan = entry->plan.get();
+    const IO& io = entry->io;
     const t2v_unet_config& cfg = u->cfg;
     const int cin_pad = (cfg.in_dim + 7) / 8 * 8;
     const int F_total = F;
@@ -1246,26 +1171,22 @@ int t2v_unet_forward_adapter(t2v_unet* u, const void* x, int x_is_f32, const flo
 }
 
 double t2v_unet_flops(t2v_unet* u, int B, int F, int h, int w, int L) {
-    Plan scratch;
-    Arena arena;
-    arena.reset(nullptr, false);
     IO io;
-    if (u->shard_on) {                   // this rank's share of the clip's work
-        scratch.shard.reset(new PlanShard());
-        scratch.shard->own_rank = u->peers.rank;
-        shard_partition(F, u->peers.nranks, scratch.shard->fb);
-    }
-    if (build(u, &scratch, &arena, true, nullptr, B, F, h, w, L, &io) != 0) return -1.0;
-    return scratch.flops;
+    double flops = 0.0;
+    // a sharded denoiser counts this rank's share of the clip's work
+    if (dry_build(new_plan_shard(u, F), false, [&](Plan* p, Arena* a, bool dry) { return build(u, p, a, dry, nullptr, B, F, h, w, L, &io); },
+                  &flops) < 0)
+        return -1.0;
+    return flops;
 }
 
 int t2v_unet_num_launches(t2v_unet* u) { return u->last_launches; }
 
 int t2v_unet_profile(t2v_unet* u, int B, int F, int h, int w, int L, void* stream_, double* out13) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    Plan* plan = get_plan(u, B, F, h, w, L, stream);
-    if (!plan) return -1;
-    return profile_plan(plan, stream, out13);
+    auto* entry = get_plan(u, B, F, h, w, L, stream);
+    if (!entry) return -1;
+    return profile_plan(entry->plan.get(), stream, out13);
 }
 
 // ------------------------------------------------------------------------------------------ frame sharding (shard.cuh)
@@ -1284,9 +1205,7 @@ int t2v_unet_shard_setup(t2v_unet* u, int rank, int nranks) {
             return -2;
         }
     }
-    for (auto& kv : u->plans) g_io.erase(kv.second.get());
-    u->plans.clear();
-    u->plan_lru.clear();
+    u->plans.clear(nullptr);
     u->peers.rank = rank;
     u->peers.nranks = nranks;
     u->peers.comm[rank] = u->comm;
@@ -1300,8 +1219,9 @@ int t2v_unet_shard_prepare(t2v_unet* u, int B, int F, int h, int w, int L, void*
         set_error("shard_prepare: call t2v_unet_shard_setup first");
         return -1;
     }
-    Plan* plan = get_plan(u, B, F, h, w, L, stream);
-    if (!plan) return -1;
+    auto* entry = get_plan(u, B, F, h, w, L, stream);
+    if (!entry) return -1;
+    Plan* plan = entry->plan.get();
     memset(out, 0, sizeof(*out));
     static_assert(sizeof(cudaIpcMemHandle_t) <= sizeof(out->comm_handle), "IPC handle size");
     cudaIpcMemHandle_t hc, hs;
@@ -1325,8 +1245,9 @@ int t2v_unet_shard_connect(t2v_unet* u, int B, int F, int h, int w, int L, const
         set_error("shard_connect: call t2v_unet_shard_setup / t2v_unet_shard_prepare first");
         return -1;
     }
-    Plan* plan = get_plan(u, B, F, h, w, L, stream);
-    if (!plan) return -1;
+    auto* entry = get_plan(u, B, F, h, w, L, stream);
+    if (!entry) return -1;
+    Plan* plan = entry->plan.get();
     PlanShard* ps = plan->shard.get();
     const int me = u->peers.rank, nr = u->peers.nranks;
     for (int r = 0; r < nr; ++r) {
@@ -1368,11 +1289,8 @@ int t2v_unet_shard_connect(t2v_unet* u, int B, int F, int h, int w, int L, const
 
 int t2v_unet_shard_connected(t2v_unet* u, int B, int F, int h, int w, int L) {
     if (!u->shard_on) return 0;
-    char key[96];
-    snprintf(key, sizeof(key), "%d,%d,%d,%d,%d,%d,%d/%d", B, F, h, w, L, 0, u->peers.rank, u->peers.nranks);
-    auto it = u->plans.find(key);
-    return (it != u->plans.end() && it->second->weights_version == u->params.version() && it->second->shard &&
-            it->second->shard->connected) ? 1 : 0;
+    auto* entry = u->plans.find(plan_key(u, B, F, h, w, L, 0), u->params.version());
+    return (entry && entry->plan->shard && entry->plan->shard->connected) ? 1 : 0;
 }
 
 int t2v_unet_shard_barrier(t2v_unet* u, void* stream_) {
@@ -1416,38 +1334,30 @@ int t2v_unet_enable_taps(t2v_unet* u, int on) {
 }
 
 int t2v_unet_tap_info(t2v_unet* u, const char* name, long long* rows, int* C, int* h, int* w) {
-    for (auto& kv : u->plans) {
-        auto it = kv.second->taps.find(name);
-        if (it == kv.second->taps.end()) continue;
-        if (rows) *rows = it->second.first.rows;
-        if (C) *C = it->second.first.C;
-        if (h) *h = it->second.second.first;
-        if (w) *w = it->second.second.second;
-        return 0;
-    }
-    set_error("tap '%s' not found (enable taps before the forward)", name);
-    return -1;
+    const auto* tap = find_tap(u, name);
+    if (!tap) return -1;
+    if (rows) *rows = tap->first.rows;
+    if (C) *C = tap->first.C;
+    if (h) *h = tap->second.first;
+    if (w) *w = tap->second.second;
+    return 0;
 }
 
 long long t2v_unet_read_tap(t2v_unet* u, const char* name, void* dst, long long cap_elems, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    for (auto& kv : u->plans) {
-        auto it = kv.second->taps.find(name);
-        if (it == kv.second->taps.end()) continue;
-        const Tok& t = it->second.first;
-        const int h = it->second.second.first, w = it->second.second.second;
-        const long long frames = t.rows / (static_cast<long long>(h) * w);
-        const long long n = t.rows * t.C;
-        if (n > cap_elems) {
-            set_error("tap '%s' needs %lld elements", name, n);
-            return -2;
-        }
-        // [(frames), h, w, C] tokens -> [(frames), C, h, w]: egress with B = frames, F = 1
-        if (egress_latent(t.p, t.ld, dst, 0, static_cast<int>(frames), t.C, 1, h, w, stream) != 0) return -3;
-        return n;
+    const auto* tap = find_tap(u, name);
+    if (!tap) return -1;
+    const Tok& t = tap->first;
+    const int h = tap->second.first, w = tap->second.second;
+    const long long frames = t.rows / (static_cast<long long>(h) * w);
+    const long long n = t.rows * t.C;
+    if (n > cap_elems) {
+        set_error("tap '%s' needs %lld elements", name, n);
+        return -2;
     }
-    set_error("tap '%s' not found (enable taps before the forward)", name);
-    return -1;
+    // [(frames), h, w, C] tokens -> [(frames), C, h, w]: egress with B = frames, F = 1
+    if (egress_latent(t.p, t.ld, dst, 0, static_cast<int>(frames), t.C, 1, h, w, stream) != 0) return -3;
+    return n;
 }
 
 }  // extern "C"

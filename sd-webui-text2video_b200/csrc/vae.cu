@@ -11,21 +11,6 @@
 #include <cstring>
 #include <memory>
 
-using namespace t2v;
-
-struct t2v_vae {
-    t2v_vae_config cfg;
-    ParamStore params;          // decoder + post_quant_conv (the hot path: missing_params counts these)
-    ParamStore enc_params;      // encoder + quant_conv (vid2vid / img2vid latent preparation; optional)
-    std::map<std::string, std::unique_ptr<Plan>> plans;
-    std::map<std::string, std::unique_ptr<Plan>> enc_plans;
-    void* gn_ws = nullptr;
-    size_t gn_ws_bytes = 0;
-    ~t2v_vae() {
-        if (gn_ws) cudaFree(gn_ws);
-    }
-};
-
 namespace t2v {
 namespace {
 
@@ -34,14 +19,38 @@ struct VIO {
     __half* out_tok;
     int out_ld;
 };
-std::map<Plan*, VIO> g_vio;
 struct EncIO {
     __half* x_tok;
     __half* out_tok;
     int out_ld;
     int ho, wo;
 };
-std::map<Plan*, EncIO> g_encio;
+
+}  // namespace
+}  // namespace t2v
+
+using namespace t2v;
+
+struct t2v_vae {
+    t2v_vae_config cfg;
+    ParamStore params;          // decoder + post_quant_conv (the hot path: missing_params counts these)
+    ParamStore enc_params;      // encoder + quant_conv (vid2vid / img2vid latent preparation; optional)
+    PlanCache<VIO> plans{3};    // key: "frames,h,w"
+    PlanCache<EncIO> enc_plans{3};
+    GnWorkspace gn_ws;          // shared by the decoder's and the encoder's plans
+};
+
+namespace t2v {
+namespace {
+
+// Grows the shared groupnorm workspace; a new pointer drops the plans of both directions, which captured the old one.
+bool ensure_gn_ws(t2v_vae* v, size_t need, cudaStream_t stream) {
+    if (v->gn_ws.ensure(need, stream)) {
+        v->plans.clear(stream);
+        v->enc_plans.clear(stream);
+    }
+    return v->gn_ws.ptr != nullptr;
+}
 
 void expect_params(t2v_vae* v) {
     ParamStore& P = v->params;
@@ -191,7 +200,7 @@ Tok attn_block(NetCtx& c, const Tok& x, const std::string& p, int frames, int hc
 
 int build(t2v_vae* v, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, int frames, int h, int w, VIO* io) {
     Builder bld(plan, arena, dry, num_sms());
-    NetCtx c{&v->params, &bld, stream, v->gn_ws};
+    NetCtx c{&v->params, &bld, stream, v->gn_ws.ptr};
     const t2v_vae_config& cfg = v->cfg;
     const long long R0 = static_cast<long long>(frames) * h * w;
     const int zpad = round_up(cfg.z_channels, 8);
@@ -249,64 +258,18 @@ int build(t2v_vae* v, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, i
     return bld.error;
 }
 
-Plan* get_plan(t2v_vae* v, int frames, int h, int w, cudaStream_t stream) {
-    char key[64];
-    snprintf(key, sizeof(key), "%d,%d,%d", frames, h, w);
-    auto it = v->plans.find(key);
-    if (it != v->plans.end() && it->second->weights_version == v->params.version()) return it->second.get();
-    if (it != v->plans.end()) {
-        g_vio.erase(it->second.get());
-        v->plans.erase(it);
-    }
-    if (v->plans.size() >= 3) {       // bounded cache: every plan owns a multi-GB activation slab (a webui session varies shapes)
-        cudaStreamSynchronize(stream);
-        for (auto& kv : v->plans) g_vio.erase(kv.second.get());
-        v->plans.clear();
-    }
-    std::string miss;
-    if (v->params.missing(&miss) > 0) {
-        set_error("VAE parameters missing (e.g. '%s')", miss.c_str());
-        return nullptr;
-    }
-    {
-        size_t need = gn_workspace_bytes(h * w, frames, num_sms());
-        need = std::max(need, gn_workspace_bytes(h * w * 64, frames, num_sms()));
-        need += 1 << 20;
-        if (need > v->gn_ws_bytes) {
-            if (v->gn_ws) cudaFree(v->gn_ws);
-            if (cudaMalloc(&v->gn_ws, need) != cudaSuccess) {
-                set_error("groupnorm workspace cudaMalloc failed");
-                return nullptr;
-            }
-            cudaMemsetAsync(v->gn_ws, 0, need, stream);
-            v->gn_ws_bytes = need;
-            for (auto& kv : v->plans) g_vio.erase(kv.second.get());          // only THIS handle's plans captured the old pointer
-            for (auto& kv : v->enc_plans) g_encio.erase(kv.second.get());
-            v->plans.clear();
-            v->enc_plans.clear();
-        }
-    }
-    std::unique_ptr<Plan> plan(new Plan());
-    Arena arena;
-    VIO io;
-    {
-        Plan scratch;
-        arena.reset(nullptr, false);
-        if (build(v, &scratch, &arena, true, stream, frames, h, w, &io) != 0) return nullptr;
-    }
-    const size_t bytes = arena.peak() + (1 << 20);
-    if (cudaMalloc(&plan->slab, bytes) != cudaSuccess) {
-        set_error("VAE activation slab cudaMalloc(%zu MB) failed", bytes >> 20);
-        return nullptr;
-    }
-    plan->slab_bytes = bytes;
-    arena.reset(plan->slab, false);
-    if (build(v, plan.get(), &arena, false, stream, frames, h, w, &io) != 0) return nullptr;
-    plan->weights_version = v->params.version();
-    Plan* raw = plan.get();
-    g_vio[raw] = io;
-    v->plans[key] = std::move(plan);
-    return raw;
+std::string shape_key(int frames, int h, int w) {
+    return std::to_string(frames) + "," + std::to_string(h) + "," + std::to_string(w);
+}
+
+PlanCache<VIO>::Entry* get_plan(t2v_vae* v, int frames, int h, int w, cudaStream_t stream) {
+    const std::string key = shape_key(frames, h, w);
+    if (auto* e = v->plans.find(key, v->params.version())) return e;
+    if (!v->params.complete("VAE")) return nullptr;
+    const size_t need = std::max(gn_workspace_bytes(h * w, frames, num_sms()), gn_workspace_bytes(h * w * 64, frames, num_sms()));
+    if (!ensure_gn_ws(v, need + (1 << 20), stream)) return nullptr;
+    return v->plans.build(key, v->params.version(), stream, std::unique_ptr<Plan>(new Plan()), false, "VAE",
+                          [&](Plan* p, Arena* a, bool dry, VIO* io) { return build(v, p, a, dry, stream, frames, h, w, io); });
 }
 
 
@@ -316,7 +279,7 @@ Plan* get_plan(t2v_vae* v, int frames, int h, int w, cudaStream_t stream) {
 
 int build_enc(t2v_vae* v, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, int frames, int H, int W, EncIO* io) {
     Builder bld(plan, arena, dry, num_sms());
-    NetCtx c{&v->enc_params, &bld, stream, v->gn_ws};
+    NetCtx c{&v->enc_params, &bld, stream, v->gn_ws.ptr};
     const t2v_vae_config& cfg = v->cfg;
     int hc = H, wc = W;
     Tok x0 = bld.alloc(static_cast<long long>(frames) * H * W, 8);          // RGB zero-padded to 8 channels
@@ -378,62 +341,13 @@ int build_enc(t2v_vae* v, Plan* plan, Arena* arena, bool dry, cudaStream_t strea
     return bld.error;
 }
 
-Plan* get_enc_plan(t2v_vae* v, int frames, int H, int W, cudaStream_t stream) {
-    char key[64];
-    snprintf(key, sizeof(key), "%d,%d,%d", frames, H, W);
-    auto it = v->enc_plans.find(key);
-    if (it != v->enc_plans.end() && it->second->weights_version == v->enc_params.version()) return it->second.get();
-    if (it != v->enc_plans.end()) {
-        g_encio.erase(it->second.get());
-        v->enc_plans.erase(it);
-    }
-    if (v->enc_plans.size() >= 3) {
-        cudaStreamSynchronize(stream);
-        for (auto& kv : v->enc_plans) g_encio.erase(kv.second.get());
-        v->enc_plans.clear();
-    }
-    std::string miss;
-    if (v->enc_params.missing(&miss) > 0) {
-        set_error("VAE encoder parameters missing (e.g. '%s')", miss.c_str());
-        return nullptr;
-    }
-    {
-        size_t need = gn_workspace_bytes(H * W, frames, num_sms()) + (1 << 20);
-        if (need > v->gn_ws_bytes) {
-            if (v->gn_ws) cudaFree(v->gn_ws);
-            if (cudaMalloc(&v->gn_ws, need) != cudaSuccess) {
-                set_error("groupnorm workspace cudaMalloc failed");
-                return nullptr;
-            }
-            cudaMemsetAsync(v->gn_ws, 0, need, stream);
-            v->gn_ws_bytes = need;
-            for (auto& kv : v->plans) g_vio.erase(kv.second.get());
-            for (auto& kv : v->enc_plans) g_encio.erase(kv.second.get());
-            v->plans.clear();
-            v->enc_plans.clear();
-        }
-    }
-    std::unique_ptr<Plan> plan(new Plan());
-    Arena arena;
-    EncIO io;
-    {
-        Plan scratch;
-        arena.reset(nullptr, false);
-        if (build_enc(v, &scratch, &arena, true, stream, frames, H, W, &io) != 0) return nullptr;
-    }
-    const size_t bytes = arena.peak() + (1 << 20);
-    if (cudaMalloc(&plan->slab, bytes) != cudaSuccess) {
-        set_error("VAE encoder activation slab cudaMalloc(%zu MB) failed", bytes >> 20);
-        return nullptr;
-    }
-    plan->slab_bytes = bytes;
-    arena.reset(plan->slab, false);
-    if (build_enc(v, plan.get(), &arena, false, stream, frames, H, W, &io) != 0) return nullptr;
-    plan->weights_version = v->enc_params.version();
-    Plan* raw = plan.get();
-    g_encio[raw] = io;
-    v->enc_plans[key] = std::move(plan);
-    return raw;
+PlanCache<EncIO>::Entry* get_enc_plan(t2v_vae* v, int frames, int H, int W, cudaStream_t stream) {
+    const std::string key = shape_key(frames, H, W);
+    if (auto* e = v->enc_plans.find(key, v->enc_params.version())) return e;
+    if (!v->enc_params.complete("VAE encoder")) return nullptr;
+    if (!ensure_gn_ws(v, gn_workspace_bytes(H * W, frames, num_sms()) + (1 << 20), stream)) return nullptr;
+    return v->enc_plans.build(key, v->enc_params.version(), stream, std::unique_ptr<Plan>(new Plan()), false, "VAE encoder",
+                              [&](Plan* p, Arena* a, bool dry, EncIO* io) { return build_enc(v, p, a, dry, stream, frames, H, W, io); });
 }
 
 }  // namespace
@@ -455,12 +369,7 @@ int t2v_vae_create(const t2v_vae_config* cfg, t2v_vae** out) {
     return 0;
 }
 
-void t2v_vae_destroy(t2v_vae* v) {
-    if (!v) return;
-    for (auto& kv : v->plans) g_vio.erase(kv.second.get());
-    for (auto& kv : v->enc_plans) g_encio.erase(kv.second.get());
-    delete v;
-}
+void t2v_vae_destroy(t2v_vae* v) { delete v; }
 
 int t2v_vae_set_param(t2v_vae* v, const char* name, const void* data, int dtype, int ndim, const int64_t* shape,
                       void* stream) {
@@ -468,51 +377,29 @@ int t2v_vae_set_param(t2v_vae* v, const char* name, const void* data, int dtype,
     return (enc ? v->enc_params : v->params).set(name, data, dtype, ndim, shape, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int t2v_vae_missing_params(t2v_vae* v, char* name_out, size_t name_cap) {
-    std::string one;
-    const int n = v->params.missing(&one);
-    if (name_out && name_cap > 0) {
-        strncpy(name_out, one.c_str(), name_cap - 1);
-        name_out[name_cap - 1] = 0;
-    }
-    return n;
-}
+int t2v_vae_missing_params(t2v_vae* v, char* name_out, size_t name_cap) { return missing_params_out(v->params, name_out, name_cap); }
 
 int t2v_vae_param_info(t2v_vae* v, int index, char* name_out, size_t name_cap, int64_t* shape_out, int* ndim_out) {
-    std::string name;
-    std::vector<long long> shape;
     // decoder-side parameters first, then the encoder's (same state_dict, t2v_model.py:1585-1617)
     const int n_dec = v->params.info(0, nullptr, nullptr);
     const int n_enc = v->enc_params.info(0, nullptr, nullptr);
     if (index < 0 || index >= n_dec + n_enc) return -1;
-    if (index < n_dec) v->params.info(index, &name, &shape);
-    else v->enc_params.info(index - n_dec, &name, &shape);
-    const int n = n_dec + n_enc;
-    if (name_out && name_cap > 0) {
-        strncpy(name_out, name.c_str(), name_cap - 1);
-        name_out[name_cap - 1] = 0;
-    }
-    if (ndim_out) *ndim_out = static_cast<int>(shape.size());
-    if (shape_out)
-        for (size_t i = 0; i < shape.size() && i < 8; ++i) shape_out[i] = shape[i];
-    return n;
+    if (index < n_dec) param_info_out(v->params, index, name_out, name_cap, shape_out, ndim_out);
+    else param_info_out(v->enc_params, index - n_dec, name_out, name_cap, shape_out, ndim_out);
+    return n_dec + n_enc;
 }
 
 int t2v_vae_decode(t2v_vae* v, const void* z, int z_is_f32, float z_scale, void* out, int out_mode, int B, int F, int h,
                    int w, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const int frames = B * F;
-    Plan* plan = get_plan(v, frames, h, w, stream);
-    if (!plan) return -1;
-    if (g_vio.find(plan) == g_vio.end()) {
-        set_error("internal: VAE plan without I/O staging record");
-        return -6;
-    }
-    const VIO& io = g_vio[plan];
+    auto* entry = get_plan(v, frames, h, w, stream);
+    if (!entry) return -1;
+    const VIO& io = entry->io;
     const int zpad = (v->cfg.z_channels + 7) / 8 * 8;
     int rc = ingest_latent(z, z_is_f32, io.z_tok, zpad, zpad, B, v->cfg.z_channels, F, h, w, z_scale, stream);
     if (rc != 0) return rc;
-    rc = run_plan(plan, stream, true);
+    rc = run_plan(entry->plan.get(), stream, true);
     if (rc != 0) {
         set_error("VAE launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
         return rc;
@@ -537,16 +424,12 @@ int t2v_vae_encode(t2v_vae* v, const void* x, int x_is_f32, void* moments_out, i
         set_error("t2v_vae_encode: H and W must be multiples of %d (got %d x %d)", down, H, W);
         return -3;
     }
-    Plan* plan = get_enc_plan(v, N, H, W, stream);
-    if (!plan) return -1;
-    if (g_encio.find(plan) == g_encio.end()) {
-        set_error("internal: VAE encoder plan without I/O staging record");
-        return -6;
-    }
-    const EncIO& io = g_encio[plan];
+    auto* entry = get_enc_plan(v, N, H, W, stream);
+    if (!entry) return -1;
+    const EncIO& io = entry->io;
     int rc = ingest_latent(x, x_is_f32, io.x_tok, 8, 8, N, 3, 1, H, W, 1.0f, stream);
     if (rc != 0) return rc;
-    rc = run_plan(plan, stream, true);
+    rc = run_plan(entry->plan.get(), stream, true);
     if (rc != 0) {
         set_error("VAE encoder launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
         return rc;
@@ -555,12 +438,11 @@ int t2v_vae_encode(t2v_vae* v, const void* x, int x_is_f32, void* moments_out, i
 }
 
 double t2v_vae_flops(t2v_vae* v, int nframes, int h, int w) {
-    Plan scratch;
-    Arena arena;
-    arena.reset(nullptr, false);
     VIO io;
-    if (build(v, &scratch, &arena, true, nullptr, nframes, h, w, &io) != 0) return -1.0;
-    return scratch.flops;
+    double flops = 0.0;
+    if (dry_build(nullptr, false, [&](Plan* p, Arena* a, bool dry) { return build(v, p, a, dry, nullptr, nframes, h, w, &io); }, &flops) < 0)
+        return -1.0;
+    return flops;
 }
 
 }  // extern "C"
