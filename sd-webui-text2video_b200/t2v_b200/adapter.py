@@ -12,12 +12,10 @@ import ctypes as C
 import torch
 
 from . import _lib
-from .modules import _NativeModule, _param_table, _build_tree
+from .modules import _NativeModule, _build_tree
 
 
 class Adapter(_NativeModule):
-    _set_fn = 't2v_adapter_set_param'
-
     def __init__(self, channels=(320, 640, 1280, 1280), nums_rb=3, cin=64, ksize=3, sk=False, use_conv=True):
         super().__init__()
         channels = [int(c) for c in channels]
@@ -30,28 +28,12 @@ class Adapter(_NativeModule):
         for i, c in enumerate(channels):
             cfg.channels[i] = c
         cfg.sk, cfg.use_conv = int(self.sk), int(self.use_conv)
-        l = _lib.load_library()
-        h = C.c_void_p()
-        rc = l.t2v_adapter_create(C.byref(cfg), C.byref(h))
-        if rc != 0:
+        try:
+            table = self._open('adapter', cfg)
+        except RuntimeError:
             raise ValueError(f'Adapter({channels}, nums_rb={nums_rb}, cin={cin}, ksize={ksize}, sk={sk}, use_conv={use_conv}): '
-                             f'{l.t2v_last_error().decode()}')
-        object.__setattr__(self, '_handle', h)
-        _build_tree(self, _param_table('t2v_adapter_param_info', h))
-        self._init_native()
-
-    def __del__(self):
-        h = self.__dict__.get('_handle')
-        if h:
-            try:
-                _lib.load_library().t2v_adapter_destroy(h)
-            except Exception:
-                pass
-
-    def _load_from_state_dict(self, *a, **kw):
-        # also reached when a parent module (e.g. T2VAdapterDepth) loads a state dict: its in-place copies must reship
-        self._dirty = True
-        super()._load_from_state_dict(*a, **kw)
+                             f'{_lib.load_library().t2v_last_error().decode()}') from None
+        _build_tree(self, table)
 
     def feature_sizes(self, H, W):
         """[(h_l, w_l)] of a H x W input: PixelUnshuffle(8), then halved per level (stride-2 conv: rounding up, average

@@ -15,7 +15,6 @@ syntax parser (`modules.prompt_parser`, used when importable; otherwise every to
 `FrozenCLIPEmbedder` is VideoCrafter's text conditioning (videocrafter/lvdm/models/modules/condition_modules.py:15-40): the
 OpenAI CLIP ViT-L/14 text model with transformers' parameter names, on the same library tower (arch 1).
 """
-import ctypes as C
 import math
 import os
 
@@ -23,7 +22,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .modules import _NativeModule, _param_table, _Holder
+from .modules import _NativeModule, _Holder
 
 
 class _InProj(nn.Module):
@@ -37,37 +36,12 @@ class _InProj(nn.Module):
 
 
 class _NativeTextTower(_NativeModule):
-    """A CLIP text transformer whose arithmetic runs in libt2v_b200.so (csrc/clip.cu); subclasses build the parameter tree."""
-    _set_fn = 't2v_clip_set_param'
+    """A CLIP text transformer whose arithmetic runs in libt2v_b200.so (csrc/clip.cu); subclasses build the parameter tree,
+    which may hold checkpoint tensors the library does not use (they are not shipped)."""
 
     def _create(self, width, heads, layers, layers_run, context, vocab, arch):
-        cfg = _lib.ClipConfigC(width, heads, layers_run, context, vocab, arch)
         self.width, self.heads, self.layers, self.layers_run, self.context, self.vocab = width, heads, layers, layers_run, context, vocab
-        h = C.c_void_p()
-        _lib.check(_lib.load_library().t2v_clip_create(C.byref(cfg), C.byref(h)), 'clip_create')
-        object.__setattr__(self, '_handle', h)
-        self._native_names = set(_param_table('t2v_clip_param_info', h))
-
-    def __del__(self):
-        h = self.__dict__.get('_handle')
-        if h:
-            try:
-                _lib.load_library().t2v_clip_destroy(h)
-            except Exception:
-                pass
-
-    def named_parameters(self, *a, **kw):
-        for name, p in super().named_parameters(*a, **kw):
-            if name in self._native_names:
-                yield name, p
-
-    def state_dict(self, *a, **kw):
-        return nn.Module.state_dict(self, *a, **kw)
-
-    def _load_from_state_dict(self, *a, **kw):
-        # also reached when a parent module (e.g. LatentDiffusion) loads a state dict: its in-place copies must reship
-        self._dirty = True
-        super()._load_from_state_dict(*a, **kw)
+        self._open('clip', _lib.ClipConfigC(width, heads, layers_run, context, vocab, arch))
 
     @torch.no_grad()
     def encode_tokens(self, tokens, out_dtype=torch.float32):
@@ -106,7 +80,6 @@ class _TextTower(_NativeTextTower):
         self.ln_final = nn.LayerNorm(width)
         self.text_projection = nn.Parameter(torch.zeros(width, width))      # in the checkpoint, unused on this path
         self.logit_scale = nn.Parameter(torch.zeros(()))
-        self._init_native()
 
 
 class _HFEmbeddings(_Holder):
@@ -149,7 +122,6 @@ class _CLIPTextModel(_NativeTextTower):
         tm.encoder.layers = nn.ModuleList(blocks)
         tm.final_layer_norm = nn.LayerNorm(width)
         self.text_model = tm
-        self._init_native()
 
     def forward(self, input_ids):
         """input_ids [B, context] -> last_hidden_state [B, context, width] fp32 (no attention mask: causal only)."""

@@ -73,50 +73,60 @@ def _build_tree(root, table):
         node.add_module(parts[-1], _leaf_for(path, shapes))
 
 
-def _param_table(info_fn, handle):
-    l = _lib.load_library()
-    name = C.create_string_buffer(256)
-    shape = (C.c_int64 * 8)()
-    ndim = C.c_int(0)
-    out = {}
-    n = getattr(l, info_fn)(handle, 0, name, 256, shape, C.byref(ndim))
-    for i in range(max(n, 0)):
-        getattr(l, info_fn)(handle, i, name, 256, shape, C.byref(ndim))
-        out[name.value.decode()] = tuple(int(shape[k]) for k in range(ndim.value))
-    return out
-
-
 class _NativeModule(nn.Module):
-    """Common weight-shipping logic."""
-    _set_fn = None
+    """An nn.Module mirror backed by one library handle of a kind ('unet', 'vae', 'clip', 'adapter'): it owns the handle,
+    ships the parameters the library's table names, and reships after anything that may have changed them -- `.to()` /
+    `.half()`, and a state dict loaded through this module or any parent of it."""
 
-    def _init_native(self):
+    def _open(self, kind, cfg):
+        """t2v_{kind}_create(cfg); returns the library's parameter table {name: shape}, the names this module ships."""
+        l = _lib.load_library()
+        h = C.c_void_p()
+        _lib.check(getattr(l, f't2v_{kind}_create')(C.byref(cfg), C.byref(h)), f'{kind}_create')
+        object.__setattr__(self, '_handle', h)
+        self._kind = kind
+        info = getattr(l, f't2v_{kind}_param_info')
+        name, shape, ndim = C.create_string_buffer(256), (C.c_int64 * 8)(), C.c_int(0)
+        table = {}
+        for i in range(max(info(h, 0, name, 256, shape, C.byref(ndim)), 0)):
+            info(h, i, name, 256, shape, C.byref(ndim))
+            table[name.value.decode()] = tuple(int(shape[k]) for k in range(ndim.value))
+        self._native_names = set(table)
         self._shipped = {}
         self._dirty = True
+        return table
+
+    def __del__(self):
+        h = self.__dict__.get('_handle')
+        if h:
+            try:
+                getattr(_lib.load_library(), f't2v_{self._kind}_destroy')(h)
+            except Exception:
+                pass
 
     def _apply(self, fn, *a, **kw):
         self._dirty = True
         return super()._apply(fn, *a, **kw)
 
-    def load_state_dict(self, *a, **kw):
+    def _load_from_state_dict(self, *a, **kw):
+        # also reached when a parent module (e.g. LatentDiffusion) loads a state dict: its in-place copies must reship
         self._dirty = True
-        return super().load_state_dict(*a, **kw)
+        super()._load_from_state_dict(*a, **kw)
 
     def mark_dirty(self):
         """Call after editing weights in place through objects this module cannot observe."""
         self._dirty = True
 
     def sync_weights(self, force=False):
-        """Ships every parameter whose (storage, version, dtype) changed since the last call.  The full scan costs
+        """Ships every library parameter whose (storage, version, dtype) changed since the last call.  The full scan costs
         ~1 ms of Python for 1480 tensors, so forward() only rescans when flagged dirty or asked to (the samplers
         ask once per run, which also catches LoRA's re-assigned `.weight` Parameters)."""
         if not (self._dirty or force):
             return
-        l = _lib.lib()
-        fn = getattr(l, self._set_fn)
+        fn = getattr(_lib.lib(), f't2v_{self._kind}_set_param')
         stream = _lib.stream_ptr()
         for name, p in self.named_parameters():
-            if self._already_shipped(name, p):
+            if name not in self._native_names or self._already_shipped(name, p):
                 continue
             if not p.is_cuda:
                 raise RuntimeError(f"parameter '{name}' is on {p.device}; move the model to the GPU "
@@ -127,7 +137,7 @@ class _NativeModule(nn.Module):
             t = t.contiguous()
             shape = (C.c_int64 * t.dim())(*t.shape)
             rc = fn(self._handle, name.encode(), _lib.ptr(t), int(t.dtype == torch.float32), t.dim(), shape, stream)
-            _lib.check(rc, f'{self._set_fn}({name})')
+            _lib.check(rc, f'{self._kind}_set_param({name})')
             self._mark_shipped(name, p)
         self._dirty = False
 
@@ -143,9 +153,14 @@ class _NativeModule(nn.Module):
         self._shipped[name] = ((p.data_ptr(), p._version, p.dtype), weakref.ref(p))
 
 
+def _unet_config(dim_mult, attn_scales, **fields):
+    """UNetConfigC from its scalar fields and the two lists."""
+    return _lib.UNetConfigC(dim_mult=(C.c_int * 8)(*map(int, dim_mult)), n_mult=len(dim_mult),
+                            attn_scales=(C.c_float * 8)(*map(float, attn_scales)), n_attn_scales=len(attn_scales), **fields)
+
+
 class UNetSD(_NativeModule):
     """Drop-in for modelscope/t2v_model.py::UNetSD (constructor keywords as consumed at t2v_pipeline.py:76-94)."""
-    _set_fn = 't2v_unet_set_param'
 
     def __init__(self, in_dim=4, dim=320, y_dim=768, context_dim=1024, out_dim=4, dim_mult=(1, 2, 4, 4),
                  num_heads=8, head_dim=64, num_res_blocks=2, attn_scales=(1.0, 0.5, 0.25), dropout=0.1,
@@ -158,29 +173,9 @@ class UNetSD(_NativeModule):
         self.num_res_blocks, self.attn_scales = num_res_blocks, list(attn_scales)
         self.parameterization = parameterization
         self.v_posterior = 0
-        cfg = _lib.UNetConfigC()
-        cfg.in_dim, cfg.dim, cfg.context_dim, cfg.out_dim = in_dim, dim, context_dim, out_dim
-        for i, m in enumerate(self.dim_mult):
-            cfg.dim_mult[i] = int(m)
-        cfg.n_mult = len(self.dim_mult)
-        cfg.num_heads, cfg.head_dim, cfg.num_res_blocks = num_heads, head_dim, num_res_blocks
-        for i, s in enumerate(self.attn_scales):
-            cfg.attn_scales[i] = float(s)
-        cfg.n_attn_scales = len(self.attn_scales)
-        l = _lib.load_library()
-        h = C.c_void_p()
-        _lib.check(l.t2v_unet_create(C.byref(cfg), C.byref(h)), 'unet_create')
-        object.__setattr__(self, '_handle', h)
-        _build_tree(self, _param_table('t2v_unet_param_info', h))
-        self._init_native()
-
-    def __del__(self):
-        h = self.__dict__.get('_handle')
-        if h:
-            try:
-                _lib.load_library().t2v_unet_destroy(h)
-            except Exception:
-                pass
+        cfg = _unet_config(self.dim_mult, self.attn_scales, in_dim=in_dim, dim=dim, context_dim=context_dim, out_dim=out_dim,
+                           num_heads=num_heads, head_dim=head_dim, num_res_blocks=num_res_blocks)
+        _build_tree(self, self._open('unet', cfg))
 
     # -- DDPM schedule buffers (t2v_model.py:329-384): same names, dtypes and fp64->fp32 conversion points
     def register_schedule(self, given_betas=None, beta_schedule='linear', timesteps=1000, linear_start=1e-4,
@@ -298,6 +293,19 @@ class UNetSD(_NativeModule):
                 raise ValueError(f'this rank holds frames [{b0}, {b1}) of {F_total}; got {F} frames')
         if Cc != self.in_dim:
             raise ValueError(f'expected {self.in_dim} latent channels, got {Cc}')
+        x, t, y, out = self._stage(x, t, y)
+        if getattr(self, '_shard', None) is not None:
+            self._shard_connect(B, F_total, h, w, y.shape[1])
+            F = F_total
+        rc = l.t2v_unet_forward(self._handle, _lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(t), _lib.ptr(y),
+                                _lib.ptr(out), 0, B, F, h, w, y.shape[1], _lib.stream_ptr())
+        _lib.check(rc, 'unet_forward')
+        return out
+
+    def _stage(self, x, t, y):
+        """The library's forward inputs: x fp16 / fp32 contiguous, t fp32 [B], y fp16 [B, L, context_dim] (t and y of batch
+        1 broadcast to B), and the fp16 eps output [B, out_dim, F, h, w] to write."""
+        B, _, F, h, w = x.shape
         if x.dtype not in (torch.float32, torch.float16):
             x = x.float()
         x = x.contiguous()
@@ -311,14 +319,7 @@ class UNetSD(_NativeModule):
         y = y.contiguous()
         if y.shape[2] != self.context_dim:
             raise ValueError(f'context dim {y.shape[2]} != {self.context_dim}')
-        out = torch.empty((B, self.out_dim, F, h, w), device=x.device, dtype=torch.float16)
-        if getattr(self, '_shard', None) is not None:
-            self._shard_connect(B, F_total, h, w, y.shape[1])
-            F = F_total
-        rc = l.t2v_unet_forward(self._handle, _lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(t), _lib.ptr(y),
-                                _lib.ptr(out), 0, B, F, h, w, y.shape[1], _lib.stream_ptr())
-        _lib.check(rc, 'unet_forward')
-        return out
+        return x, t, y, torch.empty((B, self.out_dim, F, h, w), device=x.device, dtype=torch.float16)
 
     # -- introspection used by bench / tests
     def flops(self, B, F, h, w, L=77):
@@ -380,22 +381,10 @@ class UNetModel(UNetSD):
         self.parameterization = parameterization
         self.v_posterior = 0
         self.dtype = torch.float16
-        cfg = _lib.UNetConfigC()
-        cfg.in_dim, cfg.dim, cfg.context_dim, cfg.out_dim = in_channels, model_channels, context_dim, out_channels
-        for i, m in enumerate(self.dim_mult):
-            cfg.dim_mult[i] = int(m)
-        cfg.n_mult = len(self.dim_mult)
-        cfg.num_heads, cfg.head_dim, cfg.num_res_blocks = num_heads, 0, num_res_blocks
-        for i, ds in enumerate(self.attention_resolutions):
-            cfg.attn_scales[i] = 1.0 / float(ds)
-        cfg.n_attn_scales = len(self.attention_resolutions)
-        cfg.arch, cfg.temporal_length = 1, temporal_length
-        l = _lib.load_library()
-        h = C.c_void_p()
-        _lib.check(l.t2v_unet_create(C.byref(cfg), C.byref(h)), 'unet_create (VideoCrafter)')
-        object.__setattr__(self, '_handle', h)
-        _build_tree(self, _param_table('t2v_unet_param_info', h))
-        self._init_native()
+        cfg = _unet_config(self.dim_mult, [1.0 / float(ds) for ds in self.attention_resolutions], in_dim=in_channels,
+                           dim=model_channels, context_dim=context_dim, out_dim=out_channels, num_heads=num_heads, head_dim=0,
+                           num_res_blocks=num_res_blocks, arch=1, temporal_length=temporal_length)
+        _build_tree(self, self._open('unet', cfg))
 
     @torch.no_grad()
     def forward(self, x, timesteps=None, time_emb_replace=None, context=None, features_adapter=None, y=None,
@@ -465,66 +454,12 @@ class UNetModel(UNetSD):
         staged = [self._channels_last(f.to(x.device) if f.device != x.device else f) for f in feats]
         self.sync_weights()
         l = _lib.lib()
-        if x.dtype not in (torch.float32, torch.float16):
-            x = x.float()
-        x = x.contiguous()
-        t = torch.as_tensor(t, device=x.device).reshape(-1).to(torch.float32)
-        if t.numel() == 1 and B > 1:
-            t = t.expand(B)
-        t = t.contiguous()
-        y = context.to(device=x.device, dtype=torch.float16)
-        if y.shape[0] == 1 and B > 1:
-            y = y.expand(B, -1, -1)
-        y = y.contiguous()
-        if y.shape[2] != self.context_dim:
-            raise ValueError(f'context dim {y.shape[2]} != {self.context_dim}')
-        out = torch.empty((B, self.out_dim, T, h, w), device=x.device, dtype=torch.float16)
+        x, t, y, out = self._stage(x, t, context)
         ptrs = (C.c_void_p * len(staged))(*[s.data_ptr() for s in staged])
         rc = l.t2v_unet_forward_adapter(self._handle, _lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(t), _lib.ptr(y), ptrs,
                                         len(staged), fb, _lib.ptr(out), 0, B, T, h, w, y.shape[1], _lib.stream_ptr())
         _lib.check(rc, 'unet_forward_adapter')
         return out
-
-
-def _encoder_table(ch, ch_mult, num_res_blocks, in_channels, z_channels):
-    """Parameter table of the ldm Encoder + quant_conv (checkpoint compatibility only; see AutoencoderKL.encode)."""
-    t = {}
-
-    def conv(p, o, i, k):
-        t[p + '.weight'] = (o, i, k, k)
-        t[p + '.bias'] = (o,)
-
-    def norm(p, c):
-        t[p + '.weight'] = (c,)
-        t[p + '.bias'] = (c,)
-
-    def resnet(p, ci, co):
-        norm(p + '.norm1', ci)
-        conv(p + '.conv1', co, ci, 3)
-        norm(p + '.norm2', co)
-        conv(p + '.conv2', co, co, 3)
-        if ci != co:
-            conv(p + '.nin_shortcut', co, ci, 1)
-
-    conv('encoder.conv_in', ch, in_channels, 3)
-    in_mult = (1,) + tuple(ch_mult)
-    block_in = ch
-    for lvl in range(len(ch_mult)):
-        block_in = ch * in_mult[lvl]
-        block_out = ch * ch_mult[lvl]
-        for j in range(num_res_blocks):
-            resnet(f'encoder.down.{lvl}.block.{j}', block_in, block_out)
-            block_in = block_out
-        if lvl != len(ch_mult) - 1:
-            conv(f'encoder.down.{lvl}.downsample.conv', block_in, block_in, 3)
-    resnet('encoder.mid.block_1', block_in, block_in)
-    norm('encoder.mid.attn_1.norm', block_in)
-    for n in ('q', 'k', 'v', 'proj_out'):
-        conv(f'encoder.mid.attn_1.{n}', block_in, block_in, 1)
-    resnet('encoder.mid.block_2', block_in, block_in)
-    norm('encoder.norm_out', block_in)
-    conv('encoder.conv_out', 2 * z_channels, block_in, 3)
-    return t
 
 
 class DiagonalGaussianDistribution(object):
@@ -554,7 +489,6 @@ class AutoencoderKL(_NativeModule):
     """Drop-in for modelscope/t2v_model.py::AutoencoderKL (ctor :1587-1617): decode() (the hot path) and encode()
     (vid2vid / img2vid latent preparation, SURVEY.md section 8f row 2) both run on the library; state_dict keys of
     VQGAN_autoencoder.pth (`encoder.*`, `decoder.*`, `quant_conv.*`, `post_quant_conv.*`)."""
-    _set_fn = 't2v_vae_set_param'
 
     def __init__(self, ddconfig, embed_dim, ckpt_path=None, **unused):
         super().__init__()
@@ -567,52 +501,9 @@ class AutoencoderKL(_NativeModule):
         cfg.num_res_blocks = ddconfig['num_res_blocks']
         cfg.z_channels, cfg.out_ch, cfg.embed_dim = ddconfig['z_channels'], ddconfig['out_ch'], embed_dim
         self.upscale = 2 ** (cfg.n_mult - 1)
-        l = _lib.load_library()
-        h = C.c_void_p()
-        _lib.check(l.t2v_vae_create(C.byref(cfg), C.byref(h)), 'vae_create')
-        object.__setattr__(self, '_handle', h)
-        table = _param_table('t2v_vae_param_info', h)
-        self._native_names = set(table)
-        enc = _encoder_table(ddconfig['ch'], ddconfig['ch_mult'], ddconfig['num_res_blocks'], ddconfig['in_channels'],
-                             ddconfig['z_channels'])
-        enc['quant_conv.weight'] = (2 * embed_dim, 2 * ddconfig['z_channels'], 1, 1)
-        enc['quant_conv.bias'] = (2 * embed_dim,)
-        table.update(enc)
-        _build_tree(self, table)
-        self._init_native()
+        _build_tree(self, self._open('vae', cfg))             # decoder + post_quant_conv, then encoder + quant_conv
         if ckpt_path is not None:
             self.init_from_ckpt(ckpt_path)
-
-    def __del__(self):
-        h = self.__dict__.get('_handle')
-        if h:
-            try:
-                _lib.load_library().t2v_vae_destroy(h)
-            except Exception:
-                pass
-
-    def named_parameters(self, *a, **kw):      # only decoder-side tensors are shipped to the library
-        return super().named_parameters(*a, **kw)
-
-    def sync_weights(self, force=False):
-        if not (self._dirty or force):
-            return
-        l = _lib.lib()
-        stream = _lib.stream_ptr()
-        for name, p in self.named_parameters():
-            if name not in self._native_names:
-                continue
-            if self._already_shipped(name, p):
-                continue
-            if not p.is_cuda:
-                raise RuntimeError(f"parameter '{name}' is on {p.device}; move the VAE to the GPU")
-            t = p.detach()
-            t = (t if t.dtype in (torch.float16, torch.float32) else t.float()).contiguous()
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            _lib.check(l.t2v_vae_set_param(self._handle, name.encode(), _lib.ptr(t), int(t.dtype == torch.float32),
-                                           t.dim(), shape, stream), f'vae_set_param({name})')
-            self._mark_shipped(name, p)
-        self._dirty = False
 
     def init_from_ckpt(self, path):
         """Keys carry a `first_stage_model.` prefix in VQGAN_autoencoder.pth (t2v_model.py:1619-1631)."""
