@@ -102,8 +102,9 @@ int t2v_op_gemm(const void* a, long long lda, int K, int nd, const int* dims, in
     p.n_alloc = n_alloc;
     p.N = N;
     p.b_batch_dim = b_batch_dim;
-    p.flags = flags & ~(GEMM_DBG_FORCE_BS | GEMM_DBG_NO_BS);
+    p.flags = flags & ~(GEMM_DBG_FORCE_BS | GEMM_DBG_NO_BS | GEMM_DBG_SLAB_OUT);
     p.force_bs = (flags & GEMM_DBG_FORCE_BS) ? 1 : ((flags & GEMM_DBG_NO_BS) ? -1 : 0);
+    p.slab_out = (flags & GEMM_DBG_SLAB_OUT) ? 1 : 0;
     p.out = out;
     p.ldo = ldo;
     p.bias = reinterpret_cast<const __half*>(bias);

@@ -7,11 +7,15 @@
 //                                  colsum / bias32) into shared memory
 //   warpgroups 1, 2 consumers    : each owns 64 rows of the 128-row tile; per ring stage 4 k-steps of wgmma m64 x BN x 16
 //                                  (both operands from shared memory) into fp32 registers, then the epilogue (alpha, bias,
-//                                  LayerNorm fold, residual, GEGLU) through a per-warp shared-memory staging slab, so that
-//                                  global loads and stores are 16 B per thread over whole 128 B row segments.
+//                                  LayerNorm fold, residual, GEGLU) into a shared fp16 output tile that one thread hands
+//                                  to TMA bulk stores (epilogue_tile), so the tile's writes drain to HBM while the next
+//                                  tile's MMAs run.
 // The producer runs ahead into the next tile while the consumers are in the epilogue.  What the epilogue needs besides the
 // accumulators is fetched before they are ready: the row table and LayerNorm row statistics at tile start, the column
-// operands by warp 1, the first residual units while the tile's last MMAs run.
+// operands by warp 1, the residual by a TMA load into the output tile issued as the tile's main loop starts.
+// Outputs TMA cannot address (rows that are not 16-byte aligned), fp32 split-K partials (a 128 x 256 x 4 B tile does not fit
+// beside the ring) and the B-stationary variant, whose resident weights leave no room for an output tile, store through
+// per-warp staging slabs instead (epilogue_warp).
 // CG = 2: a cluster of two CTAs owns two consecutive M-tiles of the same N-tile; each CTA fetches half of the B box and
 // TMA-multicasts it into both CTAs, so B crosses L2 -> SM once per pair.
 // Roofline: tensor-bound (2*M*N*K*taps flop per launch) whenever K*taps is large; see DESIGN.md.
@@ -32,27 +36,40 @@ constexpr int kThreads = 384;
 constexpr int kRegsProducer = 40;                            // setmaxnreg budgets: 128 x 40 + 256 x 232 <= 64 K registers
 constexpr int kRegsConsumer = 232;
 constexpr int kABytes = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;     // 16 KB
-constexpr int kSmemBudget = 216 * 1024;                      // ring (barriers + alignment slack on top; 227 KB per block)
+constexpr int kSmemPerBlock = 227 * 1024;
+constexpr int kSmemBudget = 216 * 1024;                      // B-stationary: resident weights + A ring
 constexpr int kMaxStages = 8;
-// Epilogue staging, per consumer warp: 8 rows x 128 B (half of the warp's 16 rows at a time) + the global row index of each of
-// its 16 rows (32-bit: gemm_plan rejects problems of 2^31 rows or more).  Behind the 8 slabs, the tile's per-column epilogue
-// operands, BN x 8 B.  All of it sits outside the ring budget, in what the 227 KB per block leaves over, so no ring loses a
-// stage (BN = 160: 768 B spare before the column buffer, which the 32-bit row table makes room for).
+// Slab-path staging, per consumer warp: 8 rows x 128 B (half of the warp's 16 rows at a time).  The slabs share the space of
+// the TMA path's output tile (a launch uses one of the two).
 constexpr int kEpiRowBytes = 128;
-constexpr int kEpiWarpBytes = 8 * kEpiRowBytes + 16 * 4;
-constexpr int kEpiBytes = 8 * kEpiWarpBytes;
+constexpr int kSlabBytes = 8 * 8 * kEpiRowBytes;
+// Global row index of each consumer warp's 16 rows (32-bit: gemm_plan rejects problems of 2^31 rows or more).
+constexpr int kRowTabBytes = 8 * 16 * 4;
 
-template <int BN>
+// The output tile of the TMA path: 128 rows x OUTW fp16, as column chunks of [128 rows x OCW columns], each the smem image of
+// one TMA box.  OCW = 32 columns (64 B rows, SWIZZLE_64B) divides every tile width of 32 or more, so no box reaches into the
+// next tile's columns; BN = 16 tiles use 16-column boxes (32 B rows, SWIZZLE_32B).
+__host__ __device__ constexpr int out_chunk_cols(int outw) { return outw >= 32 ? 32 : 16; }
+__host__ __device__ constexpr int out_chunks(int outw) { return (outw + out_chunk_cols(outw) - 1) / out_chunk_cols(outw); }
+
+// SLAB: the layout without an output tile (slab stores only), whose ring keeps the stage the tile would take at BN 224 / 256.
+template <int BN, bool SLAB = false>
 struct Cfg {
     static constexpr int kBBytes = BN * GEMM_BLOCK_K * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kStages = (kSmemBudget / kStageBytes) > kMaxStages ? kMaxStages : (kSmemBudget / kStageBytes);
     static constexpr int kColBytes = BN * 8;      // (colsum, bias32) fp32 pairs, or the fp16 bias
-    static constexpr int kTailBytes = 1024 /*align slack*/ + 256 /*barriers*/ + kEpiBytes + kColBytes;
-    static constexpr int kSmemBytes = kStages * kStageBytes + kTailBytes;
-    static constexpr int kBsSmemBytes = kSmemBudget + kTailBytes;      // B-stationary: resident weights + A ring fill the budget
-    static_assert(kSmemBytes <= 227 * 1024, "shared memory per block");
+    static constexpr int kTailBytes = 1024 /*align slack*/ + 256 /*barriers*/ + kRowTabBytes + kColBytes;
+    // output tile (sized for the plain variant, whose tile is the wider one) or the slabs, whichever is larger
+    static constexpr int kOutBytes = SLAB ? kSlabBytes : std::max(kSlabBytes, out_chunks(BN) * GEMM_BLOCK_M * out_chunk_cols(BN) * 2);
+    static constexpr int kStages = std::min(kMaxStages, (kSmemPerBlock - kTailBytes - kOutBytes) / kStageBytes);
+    static constexpr int kSmemBytes = kStages * kStageBytes + kOutBytes + kTailBytes;
+    static constexpr int kBsSmemBytes = kSmemBudget + kSlabBytes + kTailBytes;
+    static_assert(kSmemBytes <= kSmemPerBlock, "shared memory per block");
 };
+static_assert(Cfg<256>::kStages == 3 && Cfg<224>::kStages == 3 && Cfg<192>::kStages == 4 && Cfg<160>::kStages == 5 &&
+                  Cfg<128>::kStages == 6 && Cfg<64>::kStages == 8 && Cfg<16>::kStages == 8,
+              "ring depths next to the output tile");
+static_assert(Cfg<256, true>::kStages == 4 && Cfg<224, true>::kStages == 4, "ring depths without the output tile");
 
 // erf-form GELU x * Phi(x) (F.gelu default, t2v_model.py:821).  Phi(x) = 1/2 erfc(-x / sqrt 2); for z = |x| / sqrt 2
 // erfc(z) = t (a1 + t (a2 + t (a3 + t (a4 + t a5)))) exp(-z^2), t = 1 / (1 + p z) (Abramowitz-Stegun 7.1.26, |error| <=
@@ -86,22 +103,22 @@ template <int BN, bool GEGLU>
 __device__ __forceinline__ void epilogue_affine(const GemmDesc& g, float (&acc)[BN / 2], const uint8_t* cols, const int* rowg,
                                                 const float2 (&rs)[2], int tn, int lane) {
     const int quad = lane & 3, fr = lane >> 2;           // fragment: rows fr, fr + 8; columns 8j + 2 quad + {0, 1}
-    if (g.bias != nullptr && g.bias_rows > 0 && (g.flags & GEMM_LN) == 0) {
-        const int nvalid = GEGLU ? g.N / 2 : g.N;
+    if (!GEGLU && g.bias != nullptr && g.bias_rows > 0 && (g.flags & GEMM_LN) == 0) {      // (gemm_plan: not with GEGLU)
+        const int col0 = tn * BN + 2 * quad;                 // column of acc[0]
+        const int nrem = g.N - col0;                         // acc[4j + e] is inside the problem while 8j + e < nrem
         const __half* brow[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int fg = rowg[fr + 8 * h];
-            brow[h] = g.bias + (fg >= 0 ? (fg / g.bias_rows) * g.bias_stride : 0);
+            brow[h] = g.bias + (fg >= 0 ? (fg / g.bias_rows) * g.bias_stride : 0) + col0;
         }
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                const int col = tn * BN + 8 * j + 2 * quad + e;              // packed accumulator column
-                if (!GEGLU && col >= nvalid) continue;
-                acc[4 * j + e] = fmaf(acc[4 * j + e], g.alpha, __half2float(__ldg(brow[0] + col)));
-                acc[4 * j + 2 + e] = fmaf(acc[4 * j + 2 + e], g.alpha, __half2float(__ldg(brow[1] + col)));
+                if (8 * j + e >= nrem) continue;
+                acc[4 * j + e] = fmaf(acc[4 * j + e], g.alpha, __half2float(__ldg(brow[0] + 8 * j + e)));
+                acc[4 * j + 2 + e] = fmaf(acc[4 * j + 2 + e], g.alpha, __half2float(__ldg(brow[1] + 8 * j + e)));
             }
         }
         return;
@@ -126,7 +143,7 @@ __device__ __forceinline__ void epilogue_affine(const GemmDesc& g, float (&acc)[
     }
 }
 
-// Residual of the fp16 epilogue, unit by unit (a unit = 128 B of output per row for 8 rows: chunk u / 2, rows 8 (u % 2) ..
+// Slab path: the residual of the fp16 epilogue, unit by unit (a unit = 128 B of output per row for 8 rows: chunk u / 2, rows 8 (u % 2) ..
 // 8 (u % 2) + 7), in the row-side layout of the staging slab: 16 B per thread.  kResUnits units of a tile are in flight at
 // a time; the first ones are issued while the tile's last MMAs run.  BN <= 192: the warp's whole slice (<= 12 x 16 B per
 // thread); wider tiles keep four units in flight, which fits their register budget without spills.
@@ -164,8 +181,9 @@ struct ResQ {
     }
 };
 
-// Step 2 of a warp's epilogue: its 16 rows x BN accumulator columns -> global memory, per unit (chunk of 128 B of output per
-// row, half h = rows 8h .. 8h + 7).  The residual slice (queued in rq, ResQ) goes into the staging slab; each thread adds it
+// Step 2 of a warp's epilogue on the slab path: its 16 rows x BN accumulator columns -> global memory, per unit (chunk of
+// 128 B of output per row, half h = rows 8h .. 8h + 7).  The residual slice (queued in rq, ResQ) goes into the staging slab;
+// each thread adds it
 // to its fragment values, rounds, and writes the result back to the same place; then the rows leave with 16 B stores.
 // Per element the arithmetic is that of a direct store: fp32 affine, + residual in fp32, one rounding (GEGLU: fp16 value,
 // fp16 gate, fp16 gelu, fp16 product).  fp32 output (split-K partials) stages 32 columns per unit and has no residual
@@ -253,27 +271,126 @@ __device__ __forceinline__ void epilogue_warp(const GemmDesc& g, float (&acc)[BN
     }
 }
 
+// Row-grid origin of M-tile tmi (the coordinates of its row 0 along d0 .. d_{nd-1}).
+__device__ __forceinline__ void tile_origin(const GemmDesc& g, int tmi, int (&org)[GEMM_MAX_RDIMS]) {
+#pragma unroll
+    for (int d = 0; d < GEMM_MAX_RDIMS; ++d) org[d] = 0;
+    if (g.nd == 1) {
+        org[0] = tmi * g.box[0];
+        return;
+    }
+    int tm = tmi;
+#pragma unroll
+    for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
+        if (d < g.nd) {
+            const int td = g.tdim[d];
+            const int qd = tm / td;
+            org[d] = (tm - qd * td) * g.box[d];
+            tm = qd;
+        }
+    }
+}
+
+// One output-tile box (map_o / map_r: rank 1 + nd) at column c0 and row-grid origin org.
+__device__ __forceinline__ void tma_store_box(const CUtensorMap* map, const void* src, int nd, int c0, const int (&org)[GEMM_MAX_RDIMS]) {
+    if (nd == 1) tma_store_2d(map, src, c0, org[0]);
+    else if (nd == 2) tma_store_3d(map, src, c0, org[0], org[1]);
+    else if (nd == 3) tma_store_4d(map, src, c0, org[0], org[1], org[2]);
+    else tma_store_5d(map, src, c0, org[0], org[1], org[2], org[3]);
+}
+__device__ __forceinline__ void tma_load_box(void* dst, const CUtensorMap* map, uint64_t* bar, int nd, int c0,
+                                             const int (&org)[GEMM_MAX_RDIMS]) {
+    if (nd == 1) tma_load_2d(dst, map, bar, c0, org[0]);
+    else if (nd == 2) tma_load_3d(dst, map, bar, c0, org[0], org[1]);
+    else if (nd == 3) tma_load_4d(dst, map, bar, c0, org[0], org[1], org[2]);
+    else tma_load_5d(dst, map, bar, c0, org[0], org[1], org[2], org[3]);
+}
+
+// The output tile's chunks hold rows of OCW * 2 bytes whose 16 B units are XOR-swizzled as the TMA SWIZZLE_{64,32}B modes
+// lay out a box: byte offset bits [4, 4 + log2(OCW / 8)) ^= bits [7, ...), which for a 1024 B aligned chunk are bits of the
+// row index alone.  A warp's fragment writes (8 rows x 4 quads, one 16 B unit column) hit 32 distinct banks.
+template <int OCW>
+__device__ __forceinline__ int out_unit_swizzle(int r) { return ((r * OCW * 2) >> 7) & (OCW / 8 - 1); }
+
+// Output chunks of tile column tn that hold columns < N (TMA path: the boxes stored, and loaded for the residual).
+template <int BN, bool GEGLU>
+__device__ __forceinline__ int live_out_chunks(const GemmDesc& g, int tn) {
+    constexpr int OUTW = GEGLU ? BN / 2 : BN;
+    constexpr int OCW = out_chunk_cols(OUTW);
+    return min(out_chunks(OUTW), ((GEGLU ? g.N / 2 : g.N) - tn * OUTW + OCW - 1) / OCW);
+}
+
+// Step 2 of a warp's epilogue on the TMA path: the warp's 16 rows (r0 = its first tile row) go into the output tile, each
+// value rounded once to fp16 after adding the residual that a TMA load put in the same place.  Per element the arithmetic is
+// that of epilogue_warp.  The tile is free once tilefree completes (the store warp saw the previous tile's stores read it,
+// and the residual landed); the warp then signals tilefull, and the store warp hands the tile to TMA stores.
+template <int BN, bool GEGLU>
+__device__ __forceinline__ void epilogue_tile(const GemmDesc& g, const float (&acc)[BN / 2], uint8_t* tile, uint64_t* tilefree,
+                                              uint32_t tphase, uint64_t* tilefull, int r0, int lane) {
+    constexpr int OUTW = GEGLU ? BN / 2 : BN;
+    constexpr int OCW = out_chunk_cols(OUTW);
+    const int quad = lane & 3, fr = lane >> 2;
+    const bool has_res = !GEGLU && g.residual != nullptr;
+    // rows r0 + fr and r0 + fr + 8 share the swizzle (it depends on row bits >= 1 below 8 only)
+    const uint32_t row = smem_u32(tile) + static_cast<uint32_t>((r0 + fr) * (OCW * 2) + 4 * quad);      // shared address
+    const int sw = out_unit_swizzle<OCW>(r0 + fr);
+    mbar_wait(tilefree, tphase);
+#pragma unroll
+    for (int j = 0; j < OUTW / 8; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            // column 8j + 2 quad: chunk j / (OCW / 8), 16 B unit j % (OCW / 8) of the row
+            const uint32_t p = row + (j / (OCW / 8)) * (GEMM_BLOCK_M * OCW * 2) + 8 * h * (OCW * 2) + (((j % (OCW / 8)) ^ sw) << 4);
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            __half2 v;
+            if constexpr (GEGLU) {
+                // out = fp16(value) * fp16(gelu(fp16(gate))): the reference's rounding points under autocast (t2v_model.py:819-821)
+                const __half2 xh = __floats2half2_rn(v0, v1);
+                const float2 gf = __half22float2(__floats2half2_rn(acc[BN / 4 + 4 * j + 2 * h], acc[BN / 4 + 4 * j + 2 * h + 1]));
+                v = __hmul2(xh, __floats2half2_rn(gelu_erf(gf.x), gelu_erf(gf.y)));
+            } else {
+                if (has_res) {
+                    const uint32_t rw = ld_shared_u32(p);
+                    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&rw));
+                    v0 += f.x;
+                    v1 += f.y;
+                }
+                v = __floats2half2_rn(v0, v1);
+            }
+            st_shared_u32(p, *reinterpret_cast<const uint32_t*>(&v));
+        }
+    }
+    fence_proxy_async_smem();          // the writes are ordered before the TMA stores that read them
+    __syncwarp();
+    if (lane == 0) mbar_arrive(tilefull);
+}
+
 // BS = "B-stationary": the CTA keeps the WHOLE weight slice of its N-tile (all taps x K chunks) resident in shared memory and
 // walks M-tiles of that N-tile only, so per tile just the A box moves through the ring.
-template <int BN, bool GEGLU, int CG, bool BS = false>
+template <int BN, bool GEGLU, int CG, bool BS = false, bool SLAB = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmDesc g) {
-    using Cf = Cfg<BN>;
+    using Cf = Cfg<BN, SLAB>;
     static_assert(!BS || CG == 1, "B-stationary tiles are single-CTA");
-    static_assert(!BS || Cf::kBsSmemBytes <= 227 * 1024, "shared memory per block");
+    static_assert(!BS || Cf::kBsSmemBytes <= kSmemPerBlock, "shared memory per block");
     constexpr int kBarStages = BS ? kMaxStages : Cf::kStages;      // barrier slots (BS: ring depth is a run-time value <= 8)
     const uint32_t rank = CG == 2 ? cluster_ctarank() : 0u;       // position in the cluster
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);   // SWIZZLE_128B atoms need 1024 B alignment
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (BS ? kSmemBudget : Cf::kStages * Cf::kStageBytes));
+    // smem map: [ring][output tile | slabs][barriers][row table][column operands]
+    // BS:       [resident B: k_total chunks of BN x 64][A ring: bs_stages x 16 KB] up to the fixed budget, then [slabs] ...
+    uint8_t* const epi = smem + (BS ? kSmemBudget : Cf::kStages * Cf::kStageBytes);     // output tile (1024 B aligned) or slabs
+    uint64_t* bars = reinterpret_cast<uint64_t*>(epi + (BS ? kSlabBytes : Cf::kOutBytes));
     uint64_t* full = bars;                       // [kStages] TMA -> consumers
     uint64_t* empty = bars + kBarStages;         // [kStages] consumers (of both CTAs of a cluster) -> TMA
     uint64_t* bfull = empty + kBarStages;        // BS: the resident weight slice has landed
     uint64_t* colfull = bfull + 1;               // column operands of the next tile are in `cols` (warp 1 -> consumers)
     uint64_t* colempty = bfull + 2;              // every consumer warp has read them (consumers -> warp 1)
-    uint8_t* const epi = reinterpret_cast<uint8_t*>(bars) + 256;       // epilogue staging, kEpiBytes
-    uint8_t* const cols = epi + kEpiBytes;                             // per-column epilogue operands, Cf::kColBytes
-    // BS smem map: [resident B: k_total chunks of BN x 64][A ring: bs_stages x 16 KB] ... barriers at the fixed ring budget
+    uint64_t* tilefree = bfull + 3;              // TMA path: the output tile may be written, residual in place (warp 2 -> consumers)
+    uint64_t* tilefull = bfull + 4;              // every consumer warp has written its rows of the tile (consumers -> warp 2)
+    int* const rowtab = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(bars) + 256);
+    uint8_t* const cols = reinterpret_cast<uint8_t*>(rowtab) + kRowTabBytes;      // per-column epilogue operands, Cf::kColBytes
+    const bool tma_out = !BS && !SLAB && g.tma_out != 0;         // else per-warp slabs (epilogue_warp)
     const int nst = BS ? g.bs_stages : Cf::kStages;
     uint8_t* const sB_res = smem;
     uint8_t* const sA_ring = smem + (BS ? g.ntaps * g.k_chunks * Cf::kBBytes : 0);
@@ -283,6 +400,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&g.map_a);
         tma_prefetch_desc(&g.map_b);
+        if (tma_out) {
+            tma_prefetch_desc(&g.map_o);
+            if (g.residual != nullptr) tma_prefetch_desc(&g.map_r);
+        }
         for (int i = 0; i < kBarStages; ++i) {
             mbar_init(&full[i], 1);
             mbar_init(&empty[i], 2 * CG);         // one arrival per consumer warpgroup of every CTA that writes this stage
@@ -290,6 +411,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         if constexpr (BS) mbar_init(bfull, 1);
         mbar_init(colfull, 1);
         mbar_init(colempty, 8);                   // one arrival per consumer warp
+        mbar_init(tilefree, 1);
+        mbar_init(tilefull, 8);                   // one arrival per consumer warp
         fence_barrier_init();
     }
     if constexpr (CG == 2) cluster_sync_all();    // peer barriers are initialised before any multicast / remote arrive
@@ -346,21 +469,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                     tn = pt - pm * tiles_n_;
                     tmi = pm * CG + static_cast<int>(rank);
                 }
-                int org[GEMM_MAX_RDIMS] = {0, 0, 0, 0};
-                if (nd == 1) {
-                    org[0] = tmi * g.box[0];
-                } else {
-                    int tm = tmi;
-#pragma unroll
-                    for (int d = 0; d < GEMM_MAX_RDIMS; ++d) {
-                        if (d < nd) {
-                            const int td = g.tdim[d];
-                            const int qd = tm / td;
-                            org[d] = (tm - qd * td) * g.box[d];
-                            tm = qd;
-                        }
-                    }
-                }
+                int org[GEMM_MAX_RDIMS];
+                tile_origin(g, tmi, org);
                 if (tmi >= tiles_m_) org[0] = g.dim[0];       // odd tail of a cluster: this CTA's tile is all out of bounds (zeros)
                 const int bbatch = bdim < 0 ? 0 : (bdim == 0 ? org[0] : (bdim == 1 ? org[1] : (bdim == 2 ? org[2] : org[3])));
                 int tap = 0, kc = it0;
@@ -430,6 +540,40 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 if (lane == 0) mbar_arrive(colfull);
                 cphase ^= 1u;
             }
+        } else if (threadIdx.x >= 64 && threadIdx.x < 96 && tma_out) {
+            // Warp 2, TMA path: one thread moves each output tile.  It readies the tile for the consumers (residual boxes
+            // loaded into it, or a plain arrival), waits until they have written it, hands it to TMA stores and waits only
+            // until those have read the tile -- the writes drain to HBM while the consumers run the next tile's MMAs.  The
+            // consumer warpgroups never wait on the stores themselves, which would hold back their warpgroup-wide wgmmas.
+            if (elect_one()) {
+                constexpr int OUTW = GEGLU ? BN / 2 : BN;
+                constexpr int OCW = out_chunk_cols(OUTW);
+                constexpr int kChunkBytes = GEMM_BLOCK_M * OCW * 2;
+                const bool has_res = !GEGLU && g.residual != nullptr;
+                const uint32_t box_bytes = static_cast<uint32_t>(g.a_tx_bytes / GEMM_BLOCK_K * OCW);    // box rows x OCW x 2 B
+                uint32_t fphase = 0;
+                for (int wi = first_pair; wi < total_items; wi += pair_stride) {
+                    const int pt = wi / nsplit;
+                    const int tn = pt % g.tiles_n;
+                    const int tmi = (pt / g.tiles_n) * CG + static_cast<int>(rank);
+                    const int nch = tmi < g.tiles_m ? live_out_chunks<BN, GEGLU>(g, tn) : 0;    // odd cluster tail: nothing
+                    int org[GEMM_MAX_RDIMS];
+                    tile_origin(g, tmi, org);
+                    if (has_res && nch > 0) {
+                        mbar_expect_tx(tilefree, nch * box_bytes);
+                        for (int c = 0; c < nch; ++c)
+                            tma_load_box(epi + c * kChunkBytes, &g.map_r, tilefree, g.nd, tn * OUTW + c * OCW, org);
+                    } else {
+                        mbar_arrive(tilefree);
+                    }
+                    mbar_wait(tilefull, fphase);
+                    fphase ^= 1u;
+                    for (int c = 0; c < nch; ++c) tma_store_box(&g.map_o, epi + c * kChunkBytes, g.nd, tn * OUTW + c * OCW, org);
+                    bulk_commit_group();
+                    bulk_wait_group_read_0();
+                }
+                bulk_wait_group_0();              // the shared memory outlives the stores
+            }
         }
         __syncwarp();
     } else {
@@ -445,18 +589,18 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
         const bool out_f32 = (g.flags & GEMM_OUT_F32) != 0;
         const bool ln = (g.flags & GEMM_LN) != 0;
-        uint8_t* const stg = epi + (cw * 4 + wr) * kEpiWarpBytes;          // this warp's staging slab and row table
-        int* const rowg = reinterpret_cast<int*>(stg + 8 * kEpiRowBytes);
-        uint32_t cphase = 0;
+        uint8_t* const stg = epi + (cw * 4 + wr) * (8 * kEpiRowBytes);    // slab path: this warp's staging slab
+        int* const rowg = rowtab + (cw * 4 + wr) * 16;                     // global row of each of the warp's 16 rows
+        uint32_t cphase = 0, tphase = 0;
         float acc[BN / 2];
-        uint4 rq[ResQ<BN>::kDepth][2];
+        uint4 rq[ResQ<BN>::kDepth][2];                                     // slab path: residual units in flight
         for (int wi = first_pair; wi < total_items; wi += pair_stride) {
             const int sp = BS ? 0 : wi % nsplit;
             const int pt = wi / nsplit;
             const int tn = BS ? bs_tn : pt % g.tiles_n;
             const int tmi = BS ? wi : (pt / g.tiles_n) * CG + static_cast<int>(rank);
             const int it0s = BS ? 0 : sp * k_per;
-            const int k_iters = min(k_total, it0s + k_per) - it0s;
+            const int k_iters = min(g.ntaps * g.k_chunks, it0s + k_per) - it0s;
 
             // ---- global row of each of this warp's 16 rows (-1: outside the problem) and the LayerNorm (mean, rstd) of the
             // thread's two fragment rows.  Both depend on the tile index only, so they are fetched before the main loop (the
@@ -521,9 +665,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                     phase ^= 1u;
                 }
             }
-            // the first residual units are in flight while the last MMAs run
+            // slab path: the first residual units are in flight while the last MMAs run
             if constexpr (!GEGLU) {
-                if (g.residual != nullptr) {
+                if (!tma_out && g.residual != nullptr) {
 #pragma unroll
                     for (int u = 0; u < ResQ<BN>::kDepth; ++u) ResQ<BN>::load(g, rowg, tn, u, lane, rq[u]);
                 }
@@ -536,7 +680,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 if constexpr (CG == 2) mbar_arrive_cluster(&empty[prev], rank ^ 1u);
             }
 
-            // ---- epilogue: affine (column operands from `cols`, then the buffer goes back to warp 1), staged stores
+            // ---- epilogue: affine (column operands from `cols`, then the buffer goes back to warp 1), then the stores.  The
+            // ring position crosses it packed into one opaque register (GEGLU, BN = 256 has none to spare).
+            uint32_t ring = static_cast<uint32_t>(stage) | (phase << 16);
+            asm volatile("" : "+r"(ring));
             if (col_operands) mbar_wait(colfull, cphase);
             epilogue_affine<BN, GEGLU>(g, acc, cols, rowg, rs, tn, lane);
             if (col_operands) {
@@ -544,9 +691,19 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 if (lane == 0) mbar_arrive(colempty);
                 cphase ^= 1u;
             }
-            if constexpr (GEGLU) epilogue_warp<BN, true, false>(g, acc, rq, stg, rowg, tn, sp, lane);
-            else if (out_f32) epilogue_warp<BN, false, true>(g, acc, rq, stg, rowg, tn, sp, lane);
-            else epilogue_warp<BN, false, false>(g, acc, rq, stg, rowg, tn, sp, lane);
+            if (tma_out) {
+                epilogue_tile<BN, GEGLU>(g, acc, epi, tilefree, tphase, tilefull, cw * 64 + wr * 16, lane);
+                tphase ^= 1u;
+            } else if constexpr (GEGLU) {
+                epilogue_warp<BN, true, false>(g, acc, rq, stg, rowg, tn, sp, lane);
+            } else if (out_f32) {
+                epilogue_warp<BN, false, true>(g, acc, rq, stg, rowg, tn, sp, lane);
+            } else {
+                epilogue_warp<BN, false, false>(g, acc, rq, stg, rowg, tn, sp, lane);
+            }
+            asm volatile("" : "+r"(ring));
+            stage = static_cast<int>(ring & 0xffffu);
+            phase = ring >> 16;
         }
     }
     if constexpr (CG == 2) cluster_sync_all();    // no CTA may exit while its peer can still multicast into it or signal it
@@ -560,10 +717,10 @@ EncodeTiledFn g_encode = nullptr;
 bool g_inited = false;
 
 int encode_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-               const cuuint32_t* box) {
+               const cuuint32_t* box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, static_cast<cuuint32_t>(rank), const_cast<void*>(base),
-                          dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                          dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
         fprintf(stderr, "[t2v] cuTensorMapEncodeTiled failed: %d (rank %d, dims %llu %llu %llu %llu %llu)\n",
@@ -579,15 +736,19 @@ int encode_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dim
 struct Variant {
     int bn, geglu, cg, smem;
     const void* fn;
-    int bs;
+    int bs, slab;
 };
 template <int BN, bool G, int CG>
 Variant variant() {
-    return Variant{BN, G ? 1 : 0, CG, Cfg<BN>::kSmemBytes, reinterpret_cast<const void*>(&gemm_tc_kernel<BN, G, CG>), 0};
+    return Variant{BN, G ? 1 : 0, CG, Cfg<BN>::kSmemBytes, reinterpret_cast<const void*>(&gemm_tc_kernel<BN, G, CG>), 0, 0};
 }
 template <int BN, bool G>
 Variant variant_bs() {
-    return Variant{BN, G ? 1 : 0, 1, Cfg<BN>::kBsSmemBytes, reinterpret_cast<const void*>(&gemm_tc_kernel<BN, G, 1, true>), 1};
+    return Variant{BN, G ? 1 : 0, 1, Cfg<BN>::kBsSmemBytes, reinterpret_cast<const void*>(&gemm_tc_kernel<BN, G, 1, true>), 1, 0};
+}
+template <int BN>
+Variant variant_slab() {
+    return Variant{BN, 0, 1, Cfg<BN, true>::kSmemBytes, reinterpret_cast<const void*>(&gemm_tc_kernel<BN, false, 1, false, true>), 0, 1};
 }
 const Variant* variants(int* n) {
     static const Variant v[] = {
@@ -597,15 +758,16 @@ const Variant* variants(int* n) {
         variant<64, false, 2>(),  variant<128, false, 2>(), variant<160, false, 2>(), variant<256, false, 2>(),
         variant<64, true, 2>(),   variant<128, true, 2>(),  variant<256, true, 2>(),
         variant_bs<160, false>(), variant_bs<128, false>(), variant_bs<128, true>(), variant_bs<64, false>(),
+        variant_slab<224>(),      variant_slab<256>(),
     };
     *n = static_cast<int>(sizeof(v) / sizeof(v[0]));
     return v;
 }
-const Variant* find_variant(int bn, bool geglu, int cg, int bs = 0) {
+const Variant* find_variant(int bn, bool geglu, int cg, int bs, int slab) {
     int n;
     const Variant* v = variants(&n);
     for (int i = 0; i < n; ++i)
-        if (v[i].bn == bn && v[i].geglu == (geglu ? 1 : 0) && v[i].cg == cg && v[i].bs == bs) return &v[i];
+        if (v[i].bn == bn && v[i].geglu == (geglu ? 1 : 0) && v[i].cg == cg && v[i].bs == bs && v[i].slab == slab) return &v[i];
     return nullptr;
 }
 
@@ -853,11 +1015,47 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
         cuuint32_t box[3] = {GEMM_BLOCK_K, static_cast<cuuint32_t>(bn / plan->cg), 1};   // a CTA of a cluster fetches half of B
         if (encode_map(&g.map_b, p.b, 3, dims, strides, box) != 0) return -6;
     }
-    const Variant* var = find_variant(bn, (p.flags & GEMM_GEGLU) != 0, plan->cg, plan->bs);
-    if (var == nullptr) return -7;
+    // ---- output path: TMA stores from a shared output tile wherever TMA can address the fp16 output (and residual) rows;
+    // per-warp slabs for fp32 output, rows that are not 16-byte aligned, and the B-stationary variant (no room for the tile)
+    const auto tma_rows = [](const void* ptr, long long ld) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && (ld & 7) == 0; };
+    g.tma_out = !(p.flags & GEMM_OUT_F32) && !plan->bs && !p.slab_out && tma_rows(p.out, p.ldo) &&
+                (p.residual == nullptr || tma_rows(p.residual, p.ldr));
+    // The stores of a tile drain behind the CTA's next tile; with no next tile (one wave: every CTA has at most one) or no
+    // TMA stores at all (fp32 split-K partials, unaligned rows) the output tile only costs the 224 / 256-wide rings a stage,
+    // so those launches take the variant without it (4 stages instead of 3; the K-heavy one-wave level-2 layers).
     const int kt = g.ntaps * g.k_chunks;
     g.k_per_split = (kt + g.splits - 1) / g.splits;
     g.splits = (kt + g.k_per_split - 1) / g.k_per_split;      // no empty splits
+    const long long tiles_all = static_cast<long long>(g.tiles_m) * g.tiles_n * g.splits;
+    plan->slab = !plan->bs && plan->cg == 1 && !(p.flags & GEMM_GEGLU) && (bn == 224 || bn == 256) &&
+                 (!g.tma_out || tiles_all <= num_sms) ? 1 : 0;
+    if (plan->slab) g.tma_out = 0;
+    if (g.tma_out) {
+        // rank 1 + nd over the same row grid as map_a: (output columns, d0, .., d_{nd-1}); box = one output-tile chunk
+        const int outw = (p.flags & GEMM_GEGLU) ? bn / 2 : bn;
+        const int ocw = out_chunk_cols(outw);
+        cuuint64_t dims[5];
+        cuuint64_t strides[4];
+        cuuint32_t box[5];
+        dims[0] = static_cast<cuuint64_t>((p.flags & GEMM_GEGLU) ? p.N / 2 : p.N);
+        box[0] = static_cast<cuuint32_t>(ocw);
+        for (int d = 0; d < p.nd; ++d) {
+            dims[d + 1] = static_cast<cuuint64_t>(g.dim[d]);
+            box[d + 1] = static_cast<cuuint32_t>(g.box[d]);
+        }
+        const CUtensorMapSwizzle sw = ocw == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+        for (int which = 0; which < (p.residual != nullptr ? 2 : 1); ++which) {
+            long long pitch = (which == 0 ? p.ldo : p.ldr) * 2;
+            for (int d = 0; d < p.nd; ++d) {
+                strides[d] = static_cast<cuuint64_t>(pitch);
+                pitch *= g.dim[d];
+            }
+            if (encode_map(which == 0 ? &g.map_o : &g.map_r, which == 0 ? p.out : p.residual, p.nd + 1, dims, strides, box, sw) != 0)
+                return -8;
+        }
+    }
+    const Variant* var = find_variant(bn, (p.flags & GEMM_GEGLU) != 0, plan->cg, plan->bs, plan->slab);
+    if (var == nullptr) return -7;
     const long long pairs = static_cast<long long>((g.tiles_m + plan->cg - 1) / plan->cg) * g.tiles_n * g.splits;
     plan->grid = plan->cg * static_cast<int>(std::min<long long>(pairs, num_sms / plan->cg));
     if (plan->bs) plan->grid = (num_sms / g.tiles_n) * g.tiles_n;             // equal groups of CTAs per N-tile
@@ -867,7 +1065,7 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
 }
 
 int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
-    const Variant* var = find_variant(plan.bn, (plan.desc.flags & GEMM_GEGLU) != 0, plan.cg, plan.bs);
+    const Variant* var = find_variant(plan.bn, (plan.desc.flags & GEMM_GEGLU) != 0, plan.cg, plan.bs, plan.slab);
     if (var == nullptr) return -1;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));

@@ -28,11 +28,15 @@ enum GemmFlags : int {
     // switches of t2v_op_gemm (never set by the model code)
     GEMM_DBG_FORCE_BS = 2048,  // t2v_op_gemm only: take the B-stationary variant whenever it is eligible (any K chunk count)
     GEMM_DBG_NO_BS = 4096,     // t2v_op_gemm only: never take it
+    GEMM_DBG_SLAB_OUT = 8192,  // t2v_op_gemm only: store through the per-warp slabs even where TMA stores could
 };
 
 struct GemmDesc {
     CUtensorMap map_a;               // rank 1 + nd : (K, d0, d1, ...)
     CUtensorMap map_b;               // rank 3      : (K, N, taps | batch)
+    CUtensorMap map_o;               // tma_out: rank 1 + nd : (output columns, d0, d1, ...) over `out`
+    CUtensorMap map_r;               // tma_out with a residual: the same over `residual`
+    int tma_out;                     // 1: fp16 tiles leave through TMA stores from a shared output tile (else per-warp slabs)
     int nd;                          // number of row dims (1..4)
     int dim[GEMM_MAX_RDIMS];         // extent of each row dim (d0 fastest)
     int box[GEMM_MAX_RDIMS];         // rows-box extent per dim; prod(box) <= 128
@@ -91,6 +95,7 @@ struct GemmProblem {
     int splits;                      // 0/1 = no split-K; >1: out must be fp32 [splits][rows][ldo], no bias/residual/GEGLU
     long long split_stride;          // elements between split partials
     int force_bs;                    // 0 = auto, 1 = B-stationary if eligible, -1 = never (tests / A-B runs)
+    int slab_out;                    // 1 = per-warp slab stores even where TMA stores could (tests)
 };
 
 struct GemmPlan {
@@ -98,6 +103,7 @@ struct GemmPlan {
     int bn;
     int cg;                          // 1 = one CTA per tile, 2 = cluster of two CTAs (two M-tiles) that multicast halves of B
     int bs;                          // 1 = B-stationary variant (CTA = one N-tile, walks M-tiles; weights resident in smem)
+    int slab;                        // 1 = variant without the output tile (slab stores, one more ring stage; BN 224 / 256)
     int grid;
     int smem;
     double flops;

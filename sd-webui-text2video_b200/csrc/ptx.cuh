@@ -22,6 +22,15 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+
 // ----------------------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -121,6 +130,35 @@ __device__ __forceinline__ void tma_load_3d_mc(void* dst, const void* map, uint6
 __device__ __forceinline__ void tma_prefetch_desc(const void* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
+
+// ----------------------------------------------------------------------------- TMA stores (shared -> global)
+// The box is read from smem in the tensor map's swizzle layout; out-of-bounds elements are not written.  Completion is
+// tracked per thread in bulk groups: commit, then wait until the source smem may be reused (.read) or the writes are done.
+__device__ __forceinline__ void tma_store_2d(const void* map, const void* src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void tma_store_3d(const void* map, const void* src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+                 ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const void* map, const void* src, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                 : "memory");
+}
+__device__ __forceinline__ void tma_store_5d(const void* map, const void* src, int c0, int c1, int c2, int c3, int c4) {
+    asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+                 ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_group_read_0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_group_0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// Orders this thread's generic-proxy shared-memory accesses before later async-proxy (TMA) accesses.
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------- warpgroup MMA (wgmma)
 // Shared-memory matrix descriptor for an operand tile written by TMA with SWIZZLE_128B: rows of 128 B (64 fp16), 8-row

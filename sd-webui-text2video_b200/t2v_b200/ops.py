@@ -12,6 +12,7 @@ from . import _lib
 GEMM_GEGLU = 1
 GEMM_FORCE_BS, GEMM_NO_BS = 2048, 4096      # bring-up switches of t2v_op_gemm: B-stationary variant on / off
 GEMM_OUT_F32 = 2
+GEMM_SLAB_OUT = 8192      # test switch of t2v_op_gemm: per-warp slab stores even where the TMA-store epilogue applies
 
 
 def _ia(vals):
