@@ -115,6 +115,23 @@ int t2v_unet_lora_merge(t2v_unet* u, const char* weight_name, const void* lora_A
 int t2v_unet_lora_clear(t2v_unet* u, void* stream);
 int t2v_unet_lora_merged(t2v_unet* u);          /* number of weights currently carrying a merge */
 
+/* ------------------------------------------------------------------------------------------ VideoCrafter LoRA
+ * replaces net_load_lora / change_lora / net_load_lora_v2 / change_lora_v2 (videocrafter/lvdm/models/modules/lora.py:620-755):
+ * `weight.data += alpha * torch.mm(up, down)` on ONE weight of a handle (UNet, VAE, CLIP text tower, depth adapter), in the
+ * library's own copy,
+ *     W <- fp16(float(W) + alpha * sum_r float(up[o, r]) * float(down[r, j]))     (fp32 product and sum, ONE rounding)
+ * followed by the same in-place re-pack as t2v_unet_lora_merge: plans and captured graphs stay valid.  up [out, rank] and
+ * down [rank, cols] are device pointers, both fp16 (dtype 0) or both fp32 (dtype 1; LoRA checkpoints are usually fp32 and
+ * are not rounded first); cols = the weight's elements per output row (a 1x1 conv's input channels; the caller squeezes 4-D
+ * factors).  The reference's `remove=True` (`-=`) is alpha negated: a subtraction in fp16 storage leaves up to one fp16 ulp
+ * of residue per element.  The first merge into a weight keeps a base copy; *_lora_restore copies it back into that one
+ * weight and frees it (net_load_lora_v2's origin_weight restore: bit-identical to never merging; a weight without a merge
+ * is left as it is), *_lora_clear does so for every weight, *_lora_merged counts the weights carrying a merge.  The UNet's
+ * t2v_unet_lora_clear / t2v_unet_lora_merged above serve both merge kinds.                                            */
+int t2v_unet_lora_apply(t2v_unet* u, const char* weight_name, const void* up, const void* down, int dtype, int rank, float alpha,
+                        void* stream);
+int t2v_unet_lora_restore(t2v_unet* u, const char* weight_name, void* stream);
+
 /* ------------------------------------------------------------------------------------------ frame-sharded clip
  * ONE clip split over the GPUs of a node, one process per GPU (e.g. BASELINE config 4's 125 frames over 8 GPUs).  Frames are
  * independent inside the spatial modules and coupled in TemporalConvBlock_v2 (t2v_model.py:1201-1212), TemporalTransformer
@@ -179,6 +196,12 @@ int t2v_vae_decode(t2v_vae* v, const void* z, int z_is_f32, float z_scale, void*
  * mean * 0.18215.  Needs the `encoder.*` / `quant_conv.*` parameters (optional for decode-only use). */
 int t2v_vae_encode(t2v_vae* v, const void* x, int x_is_f32, void* moments_out, int N, int H, int W, void* stream);
 double t2v_vae_flops(t2v_vae* v, int nframes, int h, int w);
+/* VideoCrafter LoRA on the decoder's and the encoder's weights (see "VideoCrafter LoRA" above) */
+int t2v_vae_lora_apply(t2v_vae* v, const char* weight_name, const void* up, const void* down, int dtype, int rank, float alpha,
+                       void* stream);
+int t2v_vae_lora_restore(t2v_vae* v, const char* weight_name, void* stream);
+int t2v_vae_lora_clear(t2v_vae* v, void* stream);
+int t2v_vae_lora_merged(t2v_vae* v);
 
 /* ------------------------------------------------------------------------------------------ text conditioning
  * replaces FrozenOpenCLIPEmbedder.encode_with_transformer (modelscope/clip_hardcode.py:112-119, :269-274): the OpenCLIP
@@ -211,6 +234,12 @@ int t2v_clip_param_info(t2v_clip* m, int index, char* name_out, size_t name_cap,
 /* tokens [B, context] int32 (device) -> out [B, context, width] fp16 (out_is_f32 = 0) or fp32: ln_final(transformer(...))
  * (arch 1: final_layer_norm(encoder(...)) = last_hidden_state) */
 int t2v_clip_encode(t2v_clip* m, const int* tokens, void* out, int out_is_f32, int B, void* stream);
+/* VideoCrafter LoRA on the tower's weights (see "VideoCrafter LoRA" above) */
+int t2v_clip_lora_apply(t2v_clip* m, const char* weight_name, const void* up, const void* down, int dtype, int rank, float alpha,
+                        void* stream);
+int t2v_clip_lora_restore(t2v_clip* m, const char* weight_name, void* stream);
+int t2v_clip_lora_clear(t2v_clip* m, void* stream);
+int t2v_clip_lora_merged(t2v_clip* m);
 
 /* ------------------------------------------------------------------------------------------ depth adapter
  * replaces VideoCrafter's T2I-Adapter (videocrafter/lvdm/models/modules/adapter.py: Adapter(channels, nums_rb, cin, ksize, sk,
@@ -243,6 +272,12 @@ int t2v_adapter_param_info(t2v_adapter* a, int index, char* name_out, size_t nam
  * second and later ones replay it as one CUDA graph.                                                                */
 int t2v_adapter_encode(t2v_adapter* a, const void* cond, int cond_is_f32, void* const* feats_out, int N, int H, int W,
                        void* stream);
+/* VideoCrafter LoRA on the adapter's weights (see "VideoCrafter LoRA" above) */
+int t2v_adapter_lora_apply(t2v_adapter* a, const char* weight_name, const void* up, const void* down, int dtype, int rank,
+                           float alpha, void* stream);
+int t2v_adapter_lora_restore(t2v_adapter* a, const char* weight_name, void* stream);
+int t2v_adapter_lora_clear(t2v_adapter* a, void* stream);
+int t2v_adapter_lora_merged(t2v_adapter* a);
 
 /* ------------------------------------------------------------------------------------------ sampler steps
  * replace the per-step tensor arithmetic of scripts/samplers (ddim/gaussian_sampler.py:125-136,:269-283;

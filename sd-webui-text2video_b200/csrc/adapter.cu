@@ -226,6 +226,21 @@ int t2v_adapter_param_info(t2v_adapter* a, int index, char* name_out, size_t nam
     return param_info_out(a->params, index, name_out, name_cap, shape_out, ndim_out);
 }
 
+int t2v_adapter_lora_apply(t2v_adapter* a, const char* weight_name, const void* up, const void* down, int dtype, int rank, float alpha,
+                           void* stream) {
+    clear_pending_error("t2v_adapter_lora_apply");
+    return a->params.lora_apply(weight_name, up, down, dtype, rank, alpha, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int t2v_adapter_lora_restore(t2v_adapter* a, const char* weight_name, void* stream) {
+    clear_pending_error("t2v_adapter_lora_restore");
+    return a->params.lora_restore(weight_name, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int t2v_adapter_lora_clear(t2v_adapter* a, void* stream) { return a->params.lora_clear(reinterpret_cast<cudaStream_t>(stream)); }
+
+int t2v_adapter_lora_merged(t2v_adapter* a) { return a->params.merged_count(); }
+
 int t2v_adapter_encode(t2v_adapter* a, const void* cond, int cond_is_f32, void* const* feats_out, int N, int H, int W,
                        void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);

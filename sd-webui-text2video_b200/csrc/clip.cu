@@ -353,6 +353,21 @@ int t2v_clip_param_info(t2v_clip* m, int index, char* name_out, size_t name_cap,
     return param_info_out(m->params, index, name_out, name_cap, shape_out, ndim_out);
 }
 
+int t2v_clip_lora_apply(t2v_clip* m, const char* weight_name, const void* up, const void* down, int dtype, int rank, float alpha,
+                        void* stream) {
+    clear_pending_error("t2v_clip_lora_apply");
+    return m->params.lora_apply(weight_name, up, down, dtype, rank, alpha, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int t2v_clip_lora_restore(t2v_clip* m, const char* weight_name, void* stream) {
+    clear_pending_error("t2v_clip_lora_restore");
+    return m->params.lora_restore(weight_name, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int t2v_clip_lora_clear(t2v_clip* m, void* stream) { return m->params.lora_clear(reinterpret_cast<cudaStream_t>(stream)); }
+
+int t2v_clip_lora_merged(t2v_clip* m) { return m->params.merged_count(); }
+
 int t2v_clip_encode(t2v_clip* m, const int* tokens, void* out, int out_is_f32, int B, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     auto* entry = get_plan(m, B, stream);

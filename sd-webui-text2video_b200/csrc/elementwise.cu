@@ -562,6 +562,28 @@ __global__ void lora_merge_kernel(__half* __restrict__ w, const __half* __restri
     }
 }
 
+// VideoCrafter LoRA merge (videocrafter/lvdm/models/modules/lora.py:650-666, `weight.data += alpha * torch.mm(up, down)` on an
+// fp16 weight): the product is accumulated in fp32 from fp32 (or exactly widened fp16) factors, scaled in fp32, added to the
+// widened weight in fp32, and rounded to fp16 once.
+__device__ __forceinline__ float widen(float v) { return v; }
+__device__ __forceinline__ float widen(__half v) { return __half2float(v); }
+
+template <class T>
+__global__ void lora_apply_kernel(__half* __restrict__ w, const T* __restrict__ up, const T* __restrict__ down, int out, int cols,
+                                  int rank, float alpha) {
+    griddep_wait();
+    griddep_launch_small();
+    const long long n = static_cast<long long>(out) * cols;
+    GRID_STRIDE(i, n) {
+        const int o = static_cast<int>(i / cols);
+        const int j = static_cast<int>(i - static_cast<long long>(o) * cols);
+        float acc = 0.f;
+        for (int r = 0; r < rank; ++r)
+            acc = fmaf(widen(up[static_cast<long long>(o) * rank + r]), widen(down[static_cast<long long>(r) * cols + j]), acc);
+        w[i] = __float2half_rn(__fadd_rn(__half2float(w[i]), __fmul_rn(alpha, acc)));
+    }
+}
+
 inline int ok() { return launch_status("elementwise launch"); }
 
 }  // namespace
@@ -700,6 +722,17 @@ int lora_merge_weight(__half* w, const __half* A, const __half* B, int out, int 
                       cudaStream_t stream) {
     const long long n = static_cast<long long>(out) * cols;
     launch_pdl(lora_merge_kernel, grid_for(n, 256), 256, 0, stream, w, A, B, out, cols, rank, alpha, temporal_mean);
+    return ok();
+}
+int lora_apply_weight(__half* w, const void* up, const void* down, int dtype, int out, int cols, int rank, float alpha,
+                      cudaStream_t stream) {
+    const long long n = static_cast<long long>(out) * cols;
+    if (dtype == 1)
+        launch_pdl(lora_apply_kernel<float>, grid_for(n, 256), 256, 0, stream, w, static_cast<const float*>(up),
+                   static_cast<const float*>(down), out, cols, rank, alpha);
+    else
+        launch_pdl(lora_apply_kernel<__half>, grid_for(n, 256), 256, 0, stream, w, static_cast<const __half*>(up),
+                   static_cast<const __half*>(down), out, cols, rank, alpha);
     return ok();
 }
 

@@ -121,6 +121,10 @@ int convert_to_f16(const void* src, int src_is_f32, __half* dst, long long n, cu
 //   w[o, i, kt] += alpha * mean_j fp16(sum_r B[o, r] A[r, (i * 3 + kt) * 3 + j]), j = 0..2, same roundings   (temporal_mean = 1, cols = in * 3)
 int lora_merge_weight(__half* w, const __half* A, const __half* B, int out, int cols, int rank, float alpha, int temporal_mean,
                       cudaStream_t stream);
+// VideoCrafter LoRA merge into a weight in its PyTorch layout [out, cols]: up [out, rank], down [rank, cols], both fp16
+// (dtype 0) or fp32 (dtype 1):  w[o, j] = fp16(float(w[o, j]) + alpha * sum_r up[o, r] down[r, j]), fp32 throughout, one rounding
+int lora_apply_weight(__half* w, const void* up, const void* down, int dtype, int out, int cols, int rank, float alpha,
+                      cudaStream_t stream);
 // LayerNorm folded into a Linear: wout[n,k] = fp16(w[n,k] * gamma[k]); colsum[n] = sum_k wout[n,k];
 // bias32[n] = sum_k w[n,k] * beta[k] (+ bias[n])
 int fold_ln_into_linear(const __half* w, const __half* bias, const __half* gamma, const __half* beta, __half* wout,

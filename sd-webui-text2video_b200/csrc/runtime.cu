@@ -47,34 +47,78 @@ int ParamStore::repack(const std::vector<std::string>& dirty_in, cudaStream_t s)
     return 0;
 }
 
-int ParamStore::lora_merge(const std::string& name, const __half* A, const __half* B, int rank, float alpha, int temporal_mean,
-                           cudaStream_t s) {
+Param* ParamStore::mergeable(const char* what, const std::string& name, int rank, cudaStream_t s) {
     auto it = params_.find(name);
     if (it == params_.end() || !it->second.set) {
-        set_error("lora_merge: parameter '%s' is not loaded", name.c_str());
-        return -1;
+        set_error("%s: parameter '%s' is not loaded", what, name.c_str());
+        return nullptr;
     }
     Param& p = it->second;
     if (p.shape.size() < 2 || rank < 1) {
-        set_error("lora_merge: '%s' is not a matrix / conv weight", name.c_str());
-        return -2;
-    }
-    const int out = static_cast<int>(p.shape[0]);
-    const int cols = static_cast<int>(p.elems / out);
-    if (temporal_mean && !(p.shape.size() == 5 && p.shape[2] == 3 && p.shape[3] == 1 && p.shape[4] == 1)) {
-        set_error("lora_merge: temporal_mean needs a Conv3d (3,1,1) weight, '%s' is not", name.c_str());
-        return -2;
+        set_error("%s: '%s' is not a matrix / conv weight", what, name.c_str());
+        return nullptr;
     }
     if (p.base == nullptr) {
         const size_t bytes = ((p.elems + 7) / 8 * 8) * sizeof(__half);
         if (cudaMalloc(&p.base, bytes) != cudaSuccess) {
-            set_error("lora_merge: cudaMalloc of the base copy of '%s' failed", name.c_str());
-            return -3;
+            set_error("%s: cudaMalloc of the base copy of '%s' failed", what, name.c_str());
+            return nullptr;
         }
-        if (cudaMemcpyAsync(p.base, p.data, bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess) return launch_status("lora_merge base copy");
+        if (cudaMemcpyAsync(p.base, p.data, bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
+            launch_status("LoRA base copy");
+            return nullptr;
+        }
     }
-    int rc = lora_merge_weight(p.data, A, B, out, cols, rank, alpha, temporal_mean, s);
+    return &p;
+}
+
+int ParamStore::lora_merge(const std::string& name, const __half* A, const __half* B, int rank, float alpha, int temporal_mean,
+                           cudaStream_t s) {
+    auto it = params_.find(name);
+    if (temporal_mean && it != params_.end()) {
+        const std::vector<long long>& sh = it->second.shape;
+        if (!(sh.size() == 5 && sh[2] == 3 && sh[3] == 1 && sh[4] == 1)) {
+            set_error("lora_merge: temporal_mean needs a Conv3d (3,1,1) weight, '%s' is not", name.c_str());
+            return -2;
+        }
+    }
+    Param* p = mergeable("lora_merge", name, rank, s);
+    if (p == nullptr) return -1;
+    const int out = static_cast<int>(p->shape[0]);
+    const int cols = static_cast<int>(p->elems / out);
+    int rc = lora_merge_weight(p->data, A, B, out, cols, rank, alpha, temporal_mean, s);
     if (rc != 0) return rc;
+    return repack({name}, s);
+}
+
+int ParamStore::lora_apply(const std::string& name, const void* up, const void* down, int dtype, int rank, float alpha,
+                           cudaStream_t s) {
+    if (dtype != 0 && dtype != 1) {
+        set_error("lora_apply('%s'): dtype must be 0 (fp16) or 1 (fp32)", name.c_str());
+        return -3;
+    }
+    Param* p = mergeable("lora_apply", name, rank, s);
+    if (p == nullptr) return -1;
+    const int out = static_cast<int>(p->shape[0]);
+    const int cols = static_cast<int>(p->elems / out);
+    int rc = lora_apply_weight(p->data, up, down, dtype, out, cols, rank, alpha, s);
+    if (rc != 0) return rc;
+    return repack({name}, s);
+}
+
+int ParamStore::lora_restore(const std::string& name, cudaStream_t s) {
+    auto it = params_.find(name);
+    if (it == params_.end() || !it->second.expected) {
+        set_error("lora_restore: no parameter '%s'", name.c_str());
+        return -1;
+    }
+    Param& p = it->second;
+    if (p.base == nullptr) return 0;
+    if (cudaMemcpyAsync(p.data, p.base, ((p.elems + 7) / 8 * 8) * sizeof(__half), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+        return launch_status("lora_restore copy");
+    cudaStreamSynchronize(s);
+    cudaFree(p.base);
+    p.base = nullptr;
     return repack({name}, s);
 }
 

@@ -63,11 +63,19 @@ public:
     // viewed [out, in, 3, 3, 1] and averaged over the second kernel axis (:86-94).
     int lora_merge(const std::string& name, const __half* lora_A, const __half* lora_B, int rank, float alpha, int temporal_mean,
                    cudaStream_t s);
+    // VideoCrafter LoRA (videocrafter/lvdm/models/modules/lora.py:620-672): data = fp16(data + alpha * up @ down) with fp32
+    // factors / accumulation and one rounding (up [out, rank], down [rank, cols], dtype 0 fp16 / 1 fp32), then the same in-place
+    // re-pack as lora_merge.  A removal (`-=`) is alpha negated.
+    int lora_apply(const std::string& name, const void* up, const void* down, int dtype, int rank, float alpha, cudaStream_t s);
+    // ONE merged weight back to its base copy (net_load_lora_v2's origin_weight restore, :727-736), base copy freed; a weight
+    // carrying no merge is left as it is
+    int lora_restore(const std::string& name, cudaStream_t s);
     int lora_clear(cudaStream_t s);          // every merged weight back to its base copy (bit-identical to never merging)
     int merged_count() const;
 
 private:
     int repack(const std::vector<std::string>& dirty, cudaStream_t s);
+    Param* mergeable(const char* what, const std::string& name, int rank, cudaStream_t s);   // loaded matrix / conv weight, base kept
     std::map<std::string, Param> params_;
     std::map<std::string, __half*> packed_;
     std::vector<PackRecipe> recipes_;

@@ -1324,6 +1324,17 @@ int t2v_unet_lora_merge(t2v_unet* u, const char* weight_name, const void* lora_A
                                 alpha, temporal_mean, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int t2v_unet_lora_apply(t2v_unet* u, const char* weight_name, const void* up, const void* down, int dtype, int rank, float alpha,
+                        void* stream) {
+    clear_pending_error("t2v_unet_lora_apply");
+    return u->params.lora_apply(weight_name, up, down, dtype, rank, alpha, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int t2v_unet_lora_restore(t2v_unet* u, const char* weight_name, void* stream) {
+    clear_pending_error("t2v_unet_lora_restore");
+    return u->params.lora_restore(weight_name, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int t2v_unet_lora_clear(t2v_unet* u, void* stream) { return u->params.lora_clear(reinterpret_cast<cudaStream_t>(stream)); }
 
 int t2v_unet_lora_merged(t2v_unet* u) { return u->params.merged_count(); }

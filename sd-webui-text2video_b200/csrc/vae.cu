@@ -379,6 +379,27 @@ int t2v_vae_set_param(t2v_vae* v, const char* name, const void* data, int dtype,
 
 int t2v_vae_missing_params(t2v_vae* v, char* name_out, size_t name_cap) { return missing_params_out(v->params, name_out, name_cap); }
 
+// LoRA: a weight lives in the decoder's store or in the encoder's, as t2v_vae_set_param routes it
+int t2v_vae_lora_apply(t2v_vae* v, const char* weight_name, const void* up, const void* down, int dtype, int rank, float alpha,
+                       void* stream) {
+    clear_pending_error("t2v_vae_lora_apply");
+    ParamStore& P = v->params.has(weight_name) ? v->params : v->enc_params;
+    return P.lora_apply(weight_name, up, down, dtype, rank, alpha, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int t2v_vae_lora_restore(t2v_vae* v, const char* weight_name, void* stream) {
+    clear_pending_error("t2v_vae_lora_restore");
+    ParamStore& P = v->params.has(weight_name) ? v->params : v->enc_params;
+    return P.lora_restore(weight_name, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int t2v_vae_lora_clear(t2v_vae* v, void* stream) {
+    const int rc = v->params.lora_clear(reinterpret_cast<cudaStream_t>(stream));
+    return rc != 0 ? rc : v->enc_params.lora_clear(reinterpret_cast<cudaStream_t>(stream));
+}
+
+int t2v_vae_lora_merged(t2v_vae* v) { return v->params.merged_count() + v->enc_params.merged_count(); }
+
 int t2v_vae_param_info(t2v_vae* v, int index, char* name_out, size_t name_cap, int64_t* shape_out, int* ndim_out) {
     // decoder-side parameters first, then the encoder's (same state_dict, t2v_model.py:1585-1617)
     const int n_dec = v->params.info(0, nullptr, nullptr);

@@ -34,6 +34,20 @@ SIGNATURES = {
     't2v_unet_lora_merge': (c_int, [P, c_char_p, P, P, c_int, c_float, c_int, P]),
     't2v_unet_lora_clear': (c_int, [P, P]),
     't2v_unet_lora_merged': (c_int, [P]),
+    't2v_unet_lora_apply': (c_int, [P, c_char_p, P, P, c_int, c_int, c_float, P]),
+    't2v_unet_lora_restore': (c_int, [P, c_char_p, P]),
+    't2v_vae_lora_apply': (c_int, [P, c_char_p, P, P, c_int, c_int, c_float, P]),
+    't2v_vae_lora_restore': (c_int, [P, c_char_p, P]),
+    't2v_vae_lora_clear': (c_int, [P, P]),
+    't2v_vae_lora_merged': (c_int, [P]),
+    't2v_clip_lora_apply': (c_int, [P, c_char_p, P, P, c_int, c_int, c_float, P]),
+    't2v_clip_lora_restore': (c_int, [P, c_char_p, P]),
+    't2v_clip_lora_clear': (c_int, [P, P]),
+    't2v_clip_lora_merged': (c_int, [P]),
+    't2v_adapter_lora_apply': (c_int, [P, c_char_p, P, P, c_int, c_int, c_float, P]),
+    't2v_adapter_lora_restore': (c_int, [P, c_char_p, P]),
+    't2v_adapter_lora_clear': (c_int, [P, P]),
+    't2v_adapter_lora_merged': (c_int, [P]),
     't2v_unet_shard_setup': (c_int, [P, c_int, c_int]),
     't2v_unet_shard_prepare': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P]),
     't2v_unet_shard_connect': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P]),

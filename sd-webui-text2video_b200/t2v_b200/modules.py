@@ -152,6 +152,43 @@ class _NativeModule(nn.Module):
     def _mark_shipped(self, name, p):
         self._shipped[name] = ((p.data_ptr(), p._version, p.dtype), weakref.ref(p))
 
+    # -- VideoCrafter LoRA on the library's weights (include/t2v_b200.h "VideoCrafter LoRA"; t2v_b200/videocrafter.py's
+    # net_load_lora / change_lora / net_load_lora_v2 / change_lora_v2 drive it)
+    def lora_apply(self, weight_name, up, down, alpha):
+        """W <- fp16(W + alpha * up @ down) for ONE weight of this module's state dict, on the device (lora.py:650-666):
+        up [out, rank] and down [rank, cols] stay fp32 when either is (fp16 pairs are widened exactly), the product is summed
+        in fp32 and rounded once.  A negative alpha removes.  The nn.Parameter held by this mirror keeps the base value;
+        lora_restore / lora_clear return the library to it exactly, and the plans are not rebuilt."""
+        if weight_name not in self._native_names:
+            raise KeyError(f'{weight_name!r} is not a parameter this {self._kind} handle runs')
+        p = self.get_parameter(weight_name)
+        if up.dim() != 2 or down.dim() != 2:
+            raise ValueError(f'LoRA factors for {weight_name} must be matrices (1x1 conv factors squeezed): '
+                             f'up {tuple(up.shape)}, down {tuple(down.shape)}')
+        out, cols = p.shape[0], p.numel() // p.shape[0]
+        if up.shape[0] != out or down.shape[1] != cols or up.shape[1] != down.shape[0]:
+            raise ValueError(f'LoRA shapes do not fit {weight_name} {tuple(p.shape)}: up {tuple(up.shape)} down {tuple(down.shape)}')
+        self.sync_weights()
+        dt = torch.float16 if up.dtype == down.dtype == torch.float16 else torch.float32
+        up = up.detach().to(p.device, dt).contiguous()
+        down = down.detach().to(p.device, dt).contiguous()
+        fn = getattr(_lib.lib(), f't2v_{self._kind}_lora_apply')
+        _lib.check(fn(self._handle, weight_name.encode(), _lib.ptr(up), _lib.ptr(down), int(dt == torch.float32), up.shape[1],
+                      float(alpha), _lib.stream_ptr()), f'{self._kind}_lora_apply({weight_name})')
+
+    def lora_restore(self, weight_name):
+        """ONE weight back to its value before its first merge, bit for bit (net_load_lora_v2's origin_weight restore)."""
+        fn = getattr(_lib.lib(), f't2v_{self._kind}_lora_restore')
+        _lib.check(fn(self._handle, weight_name.encode(), _lib.stream_ptr()), f'{self._kind}_lora_restore({weight_name})')
+
+    def lora_clear(self):
+        """Every merged weight back to its base value, bit for bit."""
+        _lib.check(getattr(_lib.lib(), f't2v_{self._kind}_lora_clear')(self._handle, _lib.stream_ptr()), f'{self._kind}_lora_clear')
+
+    def lora_merged(self):
+        """Number of weights currently carrying a merge."""
+        return getattr(_lib.load_library(), f't2v_{self._kind}_lora_merged')(self._handle)
+
 
 def _unet_config(dim_mult, attn_scales, **fields):
     """UNetConfigC from its scalar fields and the two lists."""
@@ -220,12 +257,6 @@ class UNetSD(_NativeModule):
             raise ValueError(f'LoRA shapes do not fit {weight_name} {tuple(p.shape)}: A {tuple(A.shape)} B {tuple(B.shape)}')
         _lib.check(_lib.lib().t2v_unet_lora_merge(self._handle, weight_name.encode(), _lib.ptr(A), _lib.ptr(B), A.shape[0], float(alpha),
                                                   int(temporal_mean), _lib.stream_ptr()), f'lora_merge({weight_name})')
-
-    def lora_clear(self):
-        _lib.check(_lib.lib().t2v_unet_lora_clear(self._handle, _lib.stream_ptr()), 'lora_clear')
-
-    def lora_merged(self):
-        return _lib.load_library().t2v_unet_lora_merged(self._handle)
 
     # -- frame-sharded clip (include/t2v_b200.h "frame-sharded clip"; t2v_b200/distributed.py drives it)
     def shard_setup(self, group=None):

@@ -8,7 +8,10 @@ Mirrors, with the reference's names / signatures for the calls on the path:
                            `model.diffusion_model.*` (UNetModel) and `first_stage_model.*` (AutoencoderKL),
                            and, with `cond_stage_config` (model_config.yaml:71-72), `cond_stage_model.transformer.text_model.*`
                            (the library's FrozenCLIPEmbedder); without it the text encoder is a pluggable callable.
-  * `load_model`           sample_utils.py:10-40 (no LoRA).
+  * `load_model`           sample_utils.py:10-40, LoRA included (`inject_lora`, `lora_scale`, `lora_path`).
+  * `net_load_lora`, `change_lora`, `net_load_lora_v2`, `change_lora_v2`
+                           videocrafter/lvdm/models/modules/lora.py:620-755: the reference's walk over a LoRA file, each pair
+                           merged on the device into the library handle that owns the weight (_NativeModule.lora_apply).
   * `DDIMSampler`          videocrafter/lvdm/samplers/ddim.py:13-279 (`make_schedule`, `sample`, `ddim_sampling`,
                            `p_sample_ddim`; per-step noise from the sampler's CPU `noise_gen`, util.py:321-325).
   * `sample_text2video`    videocrafter/sample_text2video.py:75-131, `make_model_input_shape` sample_utils.py:77-84.
@@ -138,10 +141,12 @@ def _plain(config):
     return OmegaConf.to_container(config, resolve=True)
 
 
-def load_model(config, ckpt_path, gpu_id=None):
-    """sample_utils.py:10-40 without LoRA: builds `LatentDiffusion` from `config.model.params` (a dict, or the OmegaConf of
+def load_model(config, ckpt_path, gpu_id=None, inject_lora=False, lora_scale=1.0, lora_path=''):
+    """sample_utils.py:10-40: builds `LatentDiffusion` from `config.model.params` (a dict, or the OmegaConf of
     base_t2v/model_config.yaml), loads the checkpoint's `state_dict` (or a bare state dict) with strict=True, then
-    `.half()`, moves it to the GPU and sets eval mode.  Returns (model, global_step, epoch) as the reference does."""
+    `.half()`, moves it to the GPU and sets eval mode.  With `inject_lora`, `net_load_lora(model, lora_path, alpha=lora_scale)`
+    then merges the LoRA on the GPU (the reference merges before the move; the weights are the library's there).  Returns
+    (model, global_step, epoch) as the reference does."""
     params = dict(_plain(config)['model'].get('params', None) or {})
     for k in ('unet_config', 'first_stage_config'):          # yaml form {target, params} -> the constructor's keywords
         if isinstance(params.get(k), dict) and 'target' in params[k]:
@@ -153,7 +158,115 @@ def load_model(config, ckpt_path, gpu_id=None):
     model.load_state_dict(sd, strict=True)
     model = model.half()
     model = model.to(f'cuda:{gpu_id}') if gpu_id is not None else model.cuda()
+    if inject_lora:
+        net_load_lora(model, lora_path, alpha=lora_scale)
     return model.eval(), global_step, epoch
+
+
+# ------------------------------------------------------------------------------------------------- LoRA
+# lora.py:620-755.  A LoRA file is keyed from the LatentDiffusion root, `<module path>.lora_up.weight` / `.lora_down.weight`, so
+# one file may touch weights of several library handles (UNet, VAE, text tower, adapter).  The walk is the reference's; each
+# up / down pair goes to the nearest library-backed ancestor of its module (a _NativeModule), under the parameter name
+# relative to it, and is merged there on the device (_NativeModule.lora_apply) -- no plan is rebuilt.
+
+class _Origin(object):
+    """An `origin_weight` entry of net_load_lora_v2: where the base weight lives (the library keeps the copy itself)."""
+
+    def __init__(self, module, weight_name):
+        self.module, self.weight_name = module, weight_name
+
+    def __repr__(self):
+        return f'_Origin({type(self.module).__name__}, {self.weight_name!r})'
+
+
+def _lora_state_dict(checkpoint_path):
+    """A path (torch.load, as the reference) or an already-loaded {key: tensor} dict."""
+    if isinstance(checkpoint_path, dict):
+        return checkpoint_path
+    return torch.load(checkpoint_path, map_location='cpu')
+
+
+def _lora_walk(net, checkpoint_path, visit):
+    """The reference's walk (lora.py:623-671): `.alpha` keys are skipped, each up / down pair is visited once, the module is
+    resolved with `__getattr__` from `net` (an unknown path raises AttributeError), and only modules whose class is exactly
+    nn.Linear or nn.Conv2d merge ("missing param at" otherwise).  visit(key, native, weight_name, up, down) gets the pair
+    (4-D conv factors squeezed to matrices, dtypes as stored) and the nearest library-backed ancestor with the weight's name
+    relative to it.  Returns the visited keys and the skipped ones."""
+    from .modules import _NativeModule
+    state_dict = _lora_state_dict(checkpoint_path)
+    visited, skipped = [], []
+    for key in state_dict:
+        if '.alpha' in key or key in visited:
+            continue
+        layer_infos = key.split('.')[:-2]                # remove lora_up / lora_down and weight
+        curr, native, rel = net, None, []
+        for name in layer_infos:
+            curr = curr.__getattr__(name)
+            rel.append(name)
+            if isinstance(curr, _NativeModule):
+                native, rel = curr, []
+        if curr.__class__ not in [nn.Linear, nn.Conv2d]:
+            print('missing param at:', key)
+            skipped.append(key)
+            continue
+        if 'lora_down' in key:
+            pair_keys = [key.replace('lora_down', 'lora_up'), key]
+        else:
+            pair_keys = [key, key.replace('lora_up', 'lora_down')]
+        up, down = state_dict[pair_keys[0]], state_dict[pair_keys[1]]
+        if len(up.shape) == 4:                           # for conv
+            up, down = up.squeeze(3).squeeze(2), down.squeeze(3).squeeze(2)
+        if native is None:
+            raise NotImplementedError(f'LoRA key {key}: the module is not part of a library-backed network '
+                                      f'(UNet, VAE, text tower or adapter)')
+        visit(key, native, '.'.join(rel + ['weight']), up, down)
+        visited.extend(pair_keys)
+    print('load_weight_num:', len(visited))
+    return visited, skipped
+
+
+def net_load_lora(net, checkpoint_path, alpha=1.0, remove=False):
+    """lora.py:620-672: W += alpha * up @ down for every pair of the LoRA (`remove=True`: W -= ..., i.e. alpha negated; in fp16
+    storage add-then-remove leaves up to one fp16 ulp of residue per element -- net_load_lora_v2 restores exactly).
+    `checkpoint_path`: a path or an already-loaded dict."""
+    a = -float(alpha) if remove else float(alpha)
+    _lora_walk(net, checkpoint_path, lambda key, native, name, up, down: native.lora_apply(name, up, down, a))
+
+
+def change_lora(model, inject_lora=False, lora_scale=1.0, lora_path='', last_time_lora='', last_time_lora_scale=1.0):
+    """lora.py:674-681: subtract the last LoRA, add the new one."""
+    if last_time_lora != '':
+        net_load_lora(model, last_time_lora, alpha=last_time_lora_scale, remove=True)
+    if inject_lora:
+        net_load_lora(model, lora_path, alpha=lora_scale)
+
+
+def net_load_lora_v2(net, checkpoint_path, alpha=1.0, remove=False, origin_weight=None):
+    """lora.py:683-746: as net_load_lora, but `remove=True` restores each weight the LoRA touches to its value before its first
+    merge, bit for bit, instead of subtracting.  Returns `origin_weight` keyed as the reference's (the pair's key with
+    lora_up / lora_down -> lora); its values name the library weight, whose base copy the library keeps."""
+    origin_weight = {} if origin_weight is None else origin_weight
+
+    def visit(key, native, name, up, down):
+        storage_key = key.replace('lora_down', 'lora').replace('lora_up', 'lora')
+        if storage_key not in origin_weight:
+            origin_weight[storage_key] = _Origin(native, name)
+        if remove:
+            native.lora_restore(name)
+        else:
+            native.lora_apply(name, up, down, float(alpha))
+    _lora_walk(net, checkpoint_path, visit)
+    return origin_weight
+
+
+def change_lora_v2(model, inject_lora=False, lora_scale=1.0, lora_path='', last_time_lora='', last_time_lora_scale=1.0,
+                   origin_weight=None):
+    """lora.py:748-755: restore the weights of the last LoRA exactly, then add the new one."""
+    if last_time_lora != '':
+        origin_weight = net_load_lora_v2(model, last_time_lora, alpha=last_time_lora_scale, remove=True, origin_weight=origin_weight)
+    if inject_lora:
+        origin_weight = net_load_lora_v2(model, lora_path, alpha=lora_scale, origin_weight=origin_weight)
+    return origin_weight
 
 
 class DDIMSampler(object):
@@ -302,16 +415,24 @@ def process_videocrafter(args_dict, model=None):
     n_prompt, 1, 1, sample_type='ddim', sampler=ddim_sampler, ddim_steps=steps, eta=eta, cfg_scale=cfg_scale,
     decode_frame_bs=1, num_frames=frames)`.  Checkpoint / yaml discovery under the webui models directory, mp4 writing and
     the data-URL are webui plumbing outside the path: pass `model` (a `LatentDiffusion`) or install one in `model_cache`;
-    `prompt_embeds` / `n_prompt_embeds` keys may carry pre-encoded conditioning."""
+    `prompt_embeds` / `n_prompt_embeds` keys may carry pre-encoded conditioning.
+
+    LoRA (sample_text2video.py:42-46, :202-206, :231-233): `inject_lora`, `lora_path` (a path or a loaded dict), `lora_scale`
+    and `lora_trigger_word`, which is appended to a string prompt.  The model keeps the LoRA merged between calls; a call with
+    another LoRA or scale, or without inject_lora, switches with change_lora_v2 (exact restore, then the new merge)."""
     global model_cache
     a = SimpleNamespace(**{**_DEFAULTS, **args_dict})
     model = model if model is not None else model_cache
     if model is None:
         raise RuntimeError('process_videocrafter: no LatentDiffusion model attached (see docstring)')
     model_cache = model
+    inject = bool(getattr(a, 'inject_lora', False))
+    _switch_lora(model, inject, getattr(a, 'lora_path', ''), float(getattr(a, 'lora_scale', 1.0)))
     sampler = DDIMSampler(model)
     prompt = getattr(a, 'prompt_embeds', None)
     n_prompt = getattr(a, 'n_prompt_embeds', None)
+    if prompt is None and inject:
+        prompt = a.prompt + getattr(a, 'lora_trigger_word', '')
     prompt = a.prompt if prompt is None else prompt
     n_prompt = a.n_prompt if n_prompt is None else n_prompt
     outputs = []
@@ -322,6 +443,22 @@ def process_videocrafter(args_dict, model=None):
                                     show_denoising_progress=False, num_frames=a.frames, x_T=getattr(a, 'x_T', None))
         outputs.append(video_encoder(samples[0:1], a) if video_encoder is not None else samples[0:1])
     return outputs
+
+
+def _switch_lora(model, inject, lora_path, lora_scale):
+    """Brings the model's merged LoRA to (lora_path, lora_scale), or to none when not `inject`, with change_lora_v2.  What is
+    merged is remembered on the model as (path, scale, origin_weight); a loaded dict is compared by identity."""
+    last = getattr(model, '_lora_loaded', None)
+    if last is None and not inject:
+        return
+    if last is not None and inject and last[1] == lora_scale and (
+            last[0] is lora_path or (isinstance(lora_path, str) and isinstance(last[0], str) and last[0] == lora_path)):
+        return
+    origin = change_lora_v2(model, inject_lora=inject, lora_scale=lora_scale, lora_path=lora_path,
+                            last_time_lora=last[0] if last is not None else '',
+                            last_time_lora_scale=last[1] if last is not None else 1.0,
+                            origin_weight=last[2] if last is not None else None)
+    model._lora_loaded = (lora_path, lora_scale, origin) if inject else None
 
 
 # ------------------------------------------------------------------------------------------------- depth-guided synthesis
