@@ -297,6 +297,19 @@ int t2v_lincomb(float* out, const float* const* src, const float* coef, int n_sr
 int t2v_latent_blend(const float* image_latents, int image_frames, const double* noise, const double* weights, double* out,
                      double* mask_out, int BC, int F, long long hw, void* stream);
 
+/* VideoCrafter q_sample (videocrafter/lvdm/models/ddpm3d.py:283-286) and the masked-DDIM blend (lvdm/samplers/ddim.py:188-195)
+ * over a fp32 latent of shape[5] = [B, C, T, h, w], with torch's fp32 rounding op by op (bit-identical to torch's ops):
+ *   known = a[b] * x0 + s[b] * noise
+ *   out   = known                                  (mask = img = NULL: q_sample)
+ *   out   = known * mask + (1 - mask) * img        (blend)
+ * a / s [B]: sqrt_alphas_cumprod[t_b] / sqrt_one_minus_alphas_cumprod[t_b].  x0, noise and mask are addressed through five
+ * element strides each, 0 on a broadcast dimension (a frame mask [1,1,T,1,1], a region mask [1,1,1,h,w], a batch-1 x0);
+ * img and out are contiguous and out may equal img.  All pointers are device pointers.  Errors: a dimension < 1, a negative
+ * stride, a missing pointer, or exactly one of mask / img given.                                                     */
+int t2v_q_sample_blend(const float* x0, const long long* x0_strides, const float* noise, const long long* noise_strides,
+                       const float* a, const float* s, const float* mask, const long long* mask_strides, const float* img,
+                       float* out, const int* shape, void* stream);
+
 /* ------------------------------------------------------------------------------------------ kernel-level entry
  * points (used by the parity tests; the model-level calls above are built from exactly these launchers).   */
 int t2v_op_gemm(const void* a, long long lda, int K, int nd, const int* dims, int ntaps, const int* tap_off,

@@ -135,6 +135,43 @@ int t2v_latent_blend(const float* image_latents, int image_frames, const double*
     return latent_blend(image_latents, image_frames, noise, weights, out, mask_out, BC, F, hw, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int t2v_q_sample_blend(const float* x0, const long long* x0_strides, const float* noise, const long long* noise_strides,
+                       const float* a, const float* s, const float* mask, const long long* mask_strides, const float* img,
+                       float* out, const int* shape, void* stream) {
+    if (!x0 || !x0_strides || !noise || !noise_strides || !a || !s || !out || !shape) {
+        set_error("q_sample_blend: x0, noise, a, s, out, their strides and the shape are required");
+        return -1;
+    }
+    if ((mask == nullptr) != (img == nullptr) || (mask && !mask_strides)) {
+        set_error("q_sample_blend: mask and img go together (both null for q_sample), and a mask needs strides");
+        return -1;
+    }
+    QSampleBlendParams p;
+    memset(&p, 0, sizeof(p));
+    p.x0 = x0;
+    p.noise = noise;
+    p.a = a;
+    p.s = s;
+    p.mask = mask;
+    p.img = img;
+    p.out = out;
+    for (int d = 0; d < 5; ++d) {
+        if (shape[d] < 1) {
+            set_error("q_sample_blend: shape[%d] = %d, every dimension must be >= 1", d, shape[d]);
+            return -1;
+        }
+        if (x0_strides[d] < 0 || noise_strides[d] < 0 || (mask && mask_strides[d] < 0)) {
+            set_error("q_sample_blend: negative stride in dimension %d", d);
+            return -1;
+        }
+        p.shape[d] = shape[d];
+        p.x0_stride[d] = x0_strides[d];
+        p.noise_stride[d] = noise_strides[d];
+        p.mask_stride[d] = mask ? mask_strides[d] : 0;
+    }
+    return q_sample_blend(p, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int t2v_op_pack_conv_weight(const void* src, int src_is_f32, void* dst, int Cout, int Cin, int taps, int n_alloc,
                             int k_alloc, void* stream) {
     return pack_conv_weight(src, src_is_f32, reinterpret_cast<__half*>(dst), Cout, Cin, taps, n_alloc, k_alloc,

@@ -530,6 +530,41 @@ __global__ void latent_blend_kernel(const float* __restrict__ img, int img_frame
     }
 }
 
+// VideoCrafter q_sample / masked DDIM blend (videocrafter/lvdm/models/ddpm3d.py:283-286, lvdm/samplers/ddim.py:188-195) in
+// torch's fp32 op order, no contraction: known = a[b]*x0 + s[b]*noise; out = known*mask + (1 - mask)*img when blending.
+// x0 / noise / mask are read through element strides (0 on a broadcast dimension); img and out are contiguous.
+__global__ void q_sample_blend_kernel(QSampleBlendParams p) {
+    griddep_wait();
+    griddep_launch_small();
+    const long long hw = static_cast<long long>(p.shape[3]) * p.shape[4];
+    const long long n = static_cast<long long>(p.shape[0]) * p.shape[1] * p.shape[2] * hw;
+    GRID_STRIDE(i, n) {
+        const int x = static_cast<int>(i % p.shape[4]);
+        long long r = i / p.shape[4];
+        const int y = static_cast<int>(r % p.shape[3]);
+        r /= p.shape[3];
+        const int t = static_cast<int>(r % p.shape[2]);
+        r /= p.shape[2];
+        const int c = static_cast<int>(r % p.shape[1]);
+        const int b = static_cast<int>(r / p.shape[1]);
+        const int idx[5] = {b, c, t, y, x};
+        long long ox = 0, on = 0, om = 0;
+#pragma unroll
+        for (int d = 0; d < 5; ++d) {
+            ox += idx[d] * p.x0_stride[d];
+            on += idx[d] * p.noise_stride[d];
+            om += idx[d] * p.mask_stride[d];
+        }
+        const float known = __fadd_rn(__fmul_rn(p.a[b], p.x0[ox]), __fmul_rn(p.s[b], p.noise[on]));
+        if (p.mask == nullptr) {
+            p.out[i] = known;
+        } else {
+            const float m = p.mask[om];
+            p.out[i] = __fadd_rn(__fmul_rn(known, m), __fmul_rn(__fsub_rn(1.0f, m), p.img[i]));
+        }
+    }
+}
+
 // LoRA hot-merge (stable_lora/stable_utils/lora_processor.py:50-96 under autocast): the low-rank product is formed with fp32
 // accumulation and rounded to fp16 (torch's autocast matmul), scaled by alpha in fp16, added in fp16.
 __global__ void lora_merge_kernel(__half* __restrict__ w, const __half* __restrict__ A, const __half* __restrict__ B, int out, int cols,
@@ -740,6 +775,12 @@ int latent_blend(const float* img, int img_frames, const double* noise, const do
                  long long hw, cudaStream_t stream) {
     const long long n = static_cast<long long>(BC) * F * hw;
     launch_pdl(latent_blend_kernel, grid_for(n, 256), 256, 0, stream, img, img_frames, noise, w, out, mask, n, F, hw);
+    return ok();
+}
+
+int q_sample_blend(const QSampleBlendParams& p, cudaStream_t stream) {
+    const long long n = static_cast<long long>(p.shape[0]) * p.shape[1] * p.shape[2] * p.shape[3] * p.shape[4];
+    launch_pdl(q_sample_blend_kernel, grid_for(n, 256), 256, 0, stream, p);
     return ok();
 }
 

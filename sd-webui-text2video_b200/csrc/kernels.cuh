@@ -140,6 +140,23 @@ int splitk_reduce(const float* part, int splits, long long split_stride, long lo
 int latent_blend(const float* img, int img_frames, const double* noise, const double* w, double* out, double* mask, int BC, int F,
                  long long hw, cudaStream_t stream);
 
+// VideoCrafter q_sample and masked-DDIM blend over a fp32 latent of `shape` [B, C, T, h, w], rounded op by op as torch's fp32
+// ops (ddpm3d.py:283-286, ddim.py:194-195): known = a[b]*x0 + s[b]*noise; out = known (mask == null) or
+// known*mask + (1 - mask)*img.  x0 / noise / mask take element strides per dimension (0 = broadcast); img / out are contiguous
+// (out may be img); a / s hold one coefficient per sample.
+struct QSampleBlendParams {
+    const float* x0;
+    const float* noise;
+    const float* a;           // sqrt_alphas_cumprod[t_b], [B]
+    const float* s;           // sqrt_one_minus_alphas_cumprod[t_b], [B]
+    const float* mask;        // null: q_sample
+    const float* img;         // null iff mask is null
+    float* out;
+    int shape[5];
+    long long x0_stride[5], noise_stride[5], mask_stride[5];
+};
+int q_sample_blend(const QSampleBlendParams& p, cudaStream_t stream);
+
 // sampler updates (fp32 latents [B,C,F,h,w]; eps from the UNet in fp16, cond / uncond)
 struct DdimStepParams {
     const float* x;           // x_t

@@ -78,6 +78,7 @@ SIGNATURES = {
     't2v_cfg_x0': (c_int, [P, P, P, c_int, P, c_ll, c_float, c_float, c_float, c_int, P]),
     't2v_lincomb': (c_int, [P, C.POINTER(P), C.POINTER(c_float), c_int, c_ll, P]),
     't2v_latent_blend': (c_int, [P, c_int, P, P, P, P, c_int, c_int, c_ll, P]),
+    't2v_q_sample_blend': (c_int, [P, C.POINTER(c_ll), P, C.POINTER(c_ll), P, P, P, C.POINTER(c_ll), P, P, C.POINTER(c_int), P]),
     't2v_op_gemm': (c_int, [P, c_ll, c_int, c_int, C.POINTER(c_int), c_int, C.POINTER(c_int), P, c_int, c_int, c_int,
                             c_int, P, c_ll, P, c_int, c_ll, P, c_ll, c_float, c_int, c_int, P]),
     't2v_op_pack_conv_weight': (c_int, [P, c_int, P, c_int, c_int, c_int, c_int, c_int, P]),

@@ -1,5 +1,6 @@
 """Thin Python wrappers over the kernel-level C entry points (t2v_op_*).  Used by the parity tests and by
-small host-side utilities; the model-level path (t2v_unet_forward / t2v_vae_decode) does not go through here.
+small host-side utilities (q_sample_blend also by the VideoCrafter sampler's masked mode); the model-level path
+(t2v_unet_forward / t2v_vae_decode) does not go through here.
 
 All tensors are CUDA fp16, channels-last token matrices [rows, C] unless stated otherwise.
 """
@@ -119,6 +120,39 @@ def attention_hd(q, k, v, o, q_bs, q_ss, k_bs, k_ss, v_bs, v_ss, o_bs, o_ss, bat
                                o_ss, batch, heads, head_dim, sq, skv, kv_batch_div, scale, _lib.stream_ptr())
     _lib.check(rc, 'op_attention_hd')
     return o
+
+
+def q_sample_blend(x0, noise, a, s, mask=None, img=None, out=None):
+    """t2v_q_sample_blend on fp32 CUDA tensors: a[b] * x0 + s[b] * noise (q_sample), or, with `mask` and `img`,
+    that * mask + (1 - mask) * img (the masked-DDIM blend), rounded as torch's fp32 ops.  The output has img's shape
+    ([B, C, T, h, w]; x0's without img); x0, noise and mask broadcast to it as torch broadcasts.  a, s: [B] fp32.
+    `out` may be `img` (in place)."""
+    l = _lib.lib()
+    shape = tuple((img if img is not None else x0).shape)
+    if len(shape) != 5:
+        raise ValueError(f'q_sample_blend: the latent must be 5-D [B, C, T, h, w], got {list(shape)}')
+    if img is not None:
+        img = img.contiguous()
+    out = torch.empty(shape, device=x0.device, dtype=torch.float32) if out is None else out
+    if not out.is_contiguous() or tuple(out.shape) != shape:
+        raise ValueError('q_sample_blend: out must be contiguous with the output shape')
+    if a.numel() != shape[0] or s.numel() != shape[0]:
+        raise ValueError(f'q_sample_blend: a and s need one coefficient per sample ({shape[0]})')
+    ts = [t for t in (x0, noise, a, s, mask, img, out) if t is not None]
+    if any(t.dtype != torch.float32 or not t.is_cuda for t in ts):
+        raise TypeError('q_sample_blend: every tensor must be fp32 on the GPU')
+
+    def view(t):                                        # (tensor, strides): expand gives stride 0 on broadcast dimensions
+        e = t.expand(shape)
+        return e, (C.c_longlong * 5)(*e.stride())
+    x0e, xs = view(x0)
+    ne, ns = view(noise)
+    me, ms = view(mask) if mask is not None else (None, None)
+    a, s = a.contiguous(), s.contiguous()
+    rc = l.t2v_q_sample_blend(_lib.ptr(x0e), xs, _lib.ptr(ne), ns, _lib.ptr(a), _lib.ptr(s), _lib.ptr(me), ms, _lib.ptr(img),
+                              _lib.ptr(out), _ia(shape), _lib.stream_ptr())
+    _lib.check(rc, 'q_sample_blend')
+    return out
 
 
 def attention_relpos(q, k, v, o, table_k, table_v, n_seq, seq_inner, bs_outer, bs_inner, ss, o_bs_outer, o_bs_inner, o_ss,
