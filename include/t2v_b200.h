@@ -316,6 +316,24 @@ int t2v_op_gemm(const void* a, long long lda, int K, int nd, const int* dims, in
                 const void* w_packed, int n_alloc, int N, int b_batch_dim, int flags, void* out, long long ldo,
                 const void* bias, int bias_rows, long long bias_stride, const void* residual, long long ldr,
                 float alpha, int force_bn, int force_cg, void* stream);
+/* t2v_op_gemm's problem through split-K, the path the model takes for contractions too small to fill the GPU: `splits`
+ * splits are requested, *splits_used returns how many run (no split is left empty), each writes an fp32 partial into
+ * scratch [splits_used][rows][N] (scratch_elems = its capacity), and a fix-up pass adds them in split order plus bias
+ * (per sample with bias_rows) and residual.  Errors, before any launch: GEGLU, fp32 output, batched B, alpha != 1,
+ * N % 8 != 0, output / residual / bias rows not 16-byte aligned, scratch too small. */
+int t2v_op_gemm_splitk(const void* a, long long lda, int K, int nd, const int* dims, int ntaps, const int* tap_off,
+                       const void* w_packed, int n_alloc, int N, int b_batch_dim, int flags, void* out, long long ldo,
+                       const void* bias, int bias_rows, long long bias_stride, const void* residual, long long ldr,
+                       float alpha, int splits, float* scratch, long long scratch_elems, int* splits_used, int force_bn,
+                       int force_cg, void* stream);
+/* Linear(LayerNorm(x)) with the LayerNorm folded into the GEMM, as the transformer blocks and text towers run it (eps 1e-5):
+ * w_folded [N, K] = fp16(w * gamma), colsum [N] = sum_k w_folded, bias32 [N] = w @ beta + bias (fp32), rowstat [rows][2] =
+ * (mean, rstd) of each x row; then out = rstd * (x @ w_folded^T - mean * colsum) + bias32 (+ residual).  The caller owns the
+ * four intermediates.  w / bias are already GEGLU-packed when flags = GEMM_GEGLU (out then has N / 2 columns); flags is 0
+ * or GEMM_GEGLU.  x rows: K % 8 == 0, K <= 2048. */
+int t2v_op_ln_linear(const void* x, long long ldx, long long rows, int K, const void* w, const void* bias, const void* gamma,
+                     const void* beta, int N, int flags, void* w_folded, float* colsum, float* bias32, float* rowstat,
+                     const void* residual, long long ldr, void* out, long long ldo, int force_bn, int force_cg, void* stream);
 int t2v_op_pack_conv_weight(const void* src, int src_is_f32, void* dst, int Cout, int Cin, int taps, int n_alloc,
                             int k_alloc, void* stream);
 int t2v_op_pack_geglu_weight(const void* w, const void* b, int src_is_f32, void* wdst, void* bdst, int H, int K, int bn,

@@ -84,10 +84,13 @@ const char* t2v_last_error(void) { return g_err; }
 int t2v_num_sms(void) { return g_num_sms; }
 const char* t2v_version(void) { return "t2v_b200 0.2 (sm_90a; wgmma+TMA implicit GEMM)"; }
 
-int t2v_op_gemm(const void* a, long long lda, int K, int nd, const int* dims, int ntaps, const int* tap_off,
-                const void* w_packed, int n_alloc, int N, int b_batch_dim, int flags, void* out, long long ldo,
-                const void* bias, int bias_rows, long long bias_stride, const void* residual, long long ldr,
-                float alpha, int force_bn, int force_cg, void* stream) {
+}  // extern "C"
+
+// the problem of t2v_op_gemm's arguments (also t2v_op_gemm_splitk's)
+static GemmProblem op_problem(const void* a, long long lda, int K, int nd, const int* dims, int ntaps, const int* tap_off,
+                              const void* w_packed, int n_alloc, int N, int b_batch_dim, int flags, void* out, long long ldo,
+                              const void* bias, int bias_rows, long long bias_stride, const void* residual, long long ldr,
+                              float alpha, int force_bn, int force_cg) {
     GemmProblem p;
     memset(&p, 0, sizeof(p));
     p.a = reinterpret_cast<const __half*>(a);
@@ -115,15 +118,119 @@ int t2v_op_gemm(const void* a, long long lda, int K, int nd, const int* dims, in
     p.alpha = alpha;
     p.force_bn = force_bn;
     p.force_cg = force_cg;
+    return p;
+}
+
+static int plan_op(const GemmProblem& p, GemmPlan* plan, const char* what) {
+    const int rc = gemm_plan(p, plan, g_num_sms);
+    if (rc != 0) set_error("%s: gemm_plan failed (%d)", what, rc);
+    return rc;
+}
+
+static int launch_op(const GemmPlan& plan, const char* what, cudaStream_t stream) {
+    const int rc = gemm_launch(plan, stream);
+    if (rc != 0) set_error("%s: gemm_launch failed: %s", what, cudaGetErrorString(cudaGetLastError()));
+    return rc;
+}
+
+extern "C" {
+
+int t2v_op_gemm(const void* a, long long lda, int K, int nd, const int* dims, int ntaps, const int* tap_off,
+                const void* w_packed, int n_alloc, int N, int b_batch_dim, int flags, void* out, long long ldo,
+                const void* bias, int bias_rows, long long bias_stride, const void* residual, long long ldr,
+                float alpha, int force_bn, int force_cg, void* stream) {
+    const GemmProblem p = op_problem(a, lda, K, nd, dims, ntaps, tap_off, w_packed, n_alloc, N, b_batch_dim, flags, out, ldo, bias,
+                                     bias_rows, bias_stride, residual, ldr, alpha, force_bn, force_cg);
     GemmPlan plan;
-    int rc = gemm_plan(p, &plan, g_num_sms);
+    const int rc = plan_op(p, &plan, "op_gemm");
+    return rc != 0 ? rc : launch_op(plan, "op_gemm", reinterpret_cast<cudaStream_t>(stream));
+}
+
+int t2v_op_gemm_splitk(const void* a, long long lda, int K, int nd, const int* dims, int ntaps, const int* tap_off,
+                       const void* w_packed, int n_alloc, int N, int b_batch_dim, int flags, void* out, long long ldo,
+                       const void* bias, int bias_rows, long long bias_stride, const void* residual, long long ldr,
+                       float alpha, int splits, float* scratch, long long scratch_elems, int* splits_used, int force_bn,
+                       int force_cg, void* stream) {
+    const GemmProblem p = op_problem(a, lda, K, nd, dims, ntaps, tap_off, w_packed, n_alloc, N, b_batch_dim, flags, out, ldo, bias,
+                                     bias_rows, bias_stride, residual, ldr, alpha, force_bn, force_cg);
+    if (const char* why = gemm_splitk_unsupported(p)) {
+        set_error("op_gemm_splitk: split-K does not take this problem: %s", why);
+        return -1;
+    }
+    if (splits < 1 || scratch == nullptr || splits_used == nullptr) {
+        set_error("op_gemm_splitk: needs splits >= 1, a scratch buffer and a place for the split count");
+        return -1;
+    }
+    const int S = gemm_split_count(p, splits);
+    const long long need = gemm_splitk_scratch_elems(p, S);
+    if (scratch_elems < need) {
+        set_error("op_gemm_splitk: %d splits need %lld fp32 scratch elements, the buffer holds %lld", S, need, scratch_elems);
+        return -1;
+    }
+    GemmPlan plan;
+    int rc = plan_op(gemm_splitk_partials(p, S, scratch), &plan, "op_gemm_splitk");
+    if (rc != 0) return rc;
+    *splits_used = S;
+    const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    rc = launch_op(plan, "op_gemm_splitk", s);
+    if (rc != 0) return rc;
+    rc = gemm_splitk_reduce(p, S, scratch, s);
+    if (rc != 0) set_error("op_gemm_splitk: splitk_reduce failed (%d)", rc);
+    return rc;
+}
+
+int t2v_op_ln_linear(const void* x, long long ldx, long long rows, int K, const void* w, const void* bias, const void* gamma,
+                     const void* beta, int N, int flags, void* w_folded, float* colsum, float* bias32, float* rowstat,
+                     const void* residual, long long ldr, void* out, long long ldo, int force_bn, int force_cg, void* stream) {
+    if (!x || !w || !gamma || !beta || !w_folded || !colsum || !bias32 || !rowstat || !out) {
+        set_error("op_ln_linear: x, w, gamma, beta, out and the four intermediate buffers are required");
+        return -1;
+    }
+    if ((flags & ~GEMM_GEGLU) != 0) {
+        set_error("op_ln_linear: flags must be 0 or GEMM_GEGLU (%d)", flags);
+        return -1;
+    }
+    if (K % 8 != 0 || K > 2048 || rows < 1 || rows >= (1LL << 31) || N < 1) {
+        set_error("op_ln_linear: LayerNorm rows need K %% 8 == 0 and K <= 2048, 1 <= rows < 2^31 (K %d rows %lld N %d)", K, rows, N);
+        return -1;
+    }
+    // the GEMM of ln_linear (runtime.cu): weights pre-scaled by gamma, out = rstd_r * (acc - mean_r * colsum_n) + bias32_n
+    GemmProblem p;
+    memset(&p, 0, sizeof(p));
+    p.a = reinterpret_cast<const __half*>(x);
+    p.lda = ldx;
+    p.K = K;
+    p.nd = 1;
+    p.dim[0] = static_cast<int>(rows);
+    p.ntaps = 1;
+    p.b = reinterpret_cast<const __half*>(w_folded);
+    p.n_alloc = N;
+    p.N = N;
+    p.b_batch_dim = -1;
+    p.flags = flags | GEMM_LN;
+    p.out = out;
+    p.ldo = ldo;
+    p.residual = reinterpret_cast<const __half*>(residual);
+    p.ldr = ldr;
+    p.alpha = 1.0f;
+    p.force_bn = force_bn;
+    p.force_cg = force_cg;
+    p.rowstat = reinterpret_cast<const float2*>(rowstat);
+    p.colsum = colsum;
+    p.bias32 = bias32;
+    GemmPlan plan;
+    int rc = plan_op(p, &plan, "op_ln_linear");
+    if (rc != 0) return rc;
+    const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    rc = fold_ln_into_linear(reinterpret_cast<const __half*>(w), reinterpret_cast<const __half*>(bias),
+                             reinterpret_cast<const __half*>(gamma), reinterpret_cast<const __half*>(beta),
+                             reinterpret_cast<__half*>(w_folded), colsum, bias32, N, K, s);
+    if (rc == 0) rc = layernorm_rowstats(p.a, ldx, rows, K, 1e-5f, reinterpret_cast<float2*>(rowstat), s);
     if (rc != 0) {
-        set_error("gemm_plan failed (%d)", rc);
+        set_error("op_ln_linear: fold / row statistics launch failed (%d)", rc);
         return rc;
     }
-    rc = gemm_launch(plan, reinterpret_cast<cudaStream_t>(stream));
-    if (rc != 0) set_error("gemm_launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-    return rc;
+    return launch_op(plan, "op_ln_linear", s);
 }
 
 int t2v_latent_blend(const float* image_latents, int image_frames, const double* noise, const double* weights, double* out,

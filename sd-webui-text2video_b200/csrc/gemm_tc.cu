@@ -21,6 +21,7 @@
 // Roofline: tensor-bound (2*M*N*K*taps flop per launch) whenever K*taps is large; see DESIGN.md.
 #include "common.cuh"
 #include "gemm_tc.cuh"
+#include "kernels.cuh"
 #include "ptx.cuh"
 
 #include <algorithm>
@@ -900,7 +901,8 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
     g.rowstat = p.rowstat;
     g.colsum = p.colsum;
     g.bias32 = p.bias32;
-    g.splits = p.splits > 1 ? p.splits : 1;
+    g.splits = gemm_split_count(p, p.splits);
+    g.k_per_split = (g.ntaps * g.k_chunks + g.splits - 1) / g.splits;
     g.split_stride = p.split_stride;
 
     // ---- N tiling: the tile width with the shortest modelled kernel time.  A persistent CTA walks ceil(tiles / CTAs) tiles
@@ -1023,9 +1025,6 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
     // The stores of a tile drain behind the CTA's next tile; with no next tile (one wave: every CTA has at most one) or no
     // TMA stores at all (fp32 split-K partials, unaligned rows) the output tile only costs the 224 / 256-wide rings a stage,
     // so those launches take the variant without it (4 stages instead of 3; the K-heavy one-wave level-2 layers).
-    const int kt = g.ntaps * g.k_chunks;
-    g.k_per_split = (kt + g.splits - 1) / g.splits;
-    g.splits = (kt + g.k_per_split - 1) / g.k_per_split;      // no empty splits
     const long long tiles_all = static_cast<long long>(g.tiles_m) * g.tiles_n * g.splits;
     plan->slab = !plan->bs && plan->cg == 1 && !(p.flags & GEMM_GEGLU) && (bn == 224 || bn == 256) &&
                  (!g.tma_out || tiles_all <= num_sms) ? 1 : 0;
@@ -1091,6 +1090,55 @@ int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
     cfg.numAttrs = na;
     void* args[1] = {const_cast<GemmDesc*>(&plan.desc)};
     return cudaLaunchKernelExC(&cfg, var->fn, args) == cudaSuccess ? 0 : -2;
+}
+
+// ------------------------------------------------------------------------------------------ split-K
+static long long problem_rows(const GemmProblem& p) {
+    long long rows = 1;
+    for (int d = 0; d < p.nd; ++d) rows *= p.dim[d];
+    return rows;
+}
+
+int gemm_split_count(const GemmProblem& p, int requested) {
+    if (requested <= 1) return 1;
+    const int kt = p.ntaps * ((p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K);
+    const int kps = (kt + requested - 1) / requested;
+    return (kt + kps - 1) / kps;
+}
+
+const char* gemm_splitk_unsupported(const GemmProblem& p) {
+    const auto a16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+    if (p.flags & GEMM_GEGLU) return "GEGLU epilogue";
+    if (p.flags & GEMM_LN) return "LayerNorm-folded epilogue";
+    if (p.flags & GEMM_OUT_F32) return "fp32 output";
+    if (p.b_batch_dim >= 0) return "batched B";
+    if (p.alpha != 1.0f) return "alpha != 1";
+    if (p.N % 8 != 0) return "N % 8 != 0";
+    if ((p.ldo & 7) != 0 || !a16(p.out)) return "output rows not 16-byte aligned";
+    if (p.residual != nullptr && ((p.ldr & 7) != 0 || !a16(p.residual))) return "residual rows not 16-byte aligned";
+    if (p.bias != nullptr && ((p.bias_stride & 7) != 0 || !a16(p.bias))) return "bias rows not 16-byte aligned";
+    return nullptr;
+}
+
+long long gemm_splitk_scratch_elems(const GemmProblem& p, int splits) { return static_cast<long long>(splits) * problem_rows(p) * p.N; }
+
+GemmProblem gemm_splitk_partials(const GemmProblem& p, int splits, float* scratch) {
+    GemmProblem q = p;
+    q.out = scratch;
+    q.ldo = p.N;
+    q.flags |= GEMM_OUT_F32;
+    q.bias = nullptr;
+    q.bias_rows = 0;
+    q.residual = nullptr;
+    q.splits = splits;
+    q.split_stride = problem_rows(p) * p.N;
+    return q;
+}
+
+int gemm_splitk_reduce(const GemmProblem& p, int splits, const float* scratch, cudaStream_t stream) {
+    const long long rows = problem_rows(p);
+    return splitk_reduce(scratch, splits, rows * p.N, rows, p.N, p.bias, p.bias_rows, p.bias_stride, p.residual, p.ldr,
+                         reinterpret_cast<__half*>(p.out), p.ldo, stream);
 }
 
 }  // namespace t2v

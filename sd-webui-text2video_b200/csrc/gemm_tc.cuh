@@ -116,6 +116,23 @@ int gemm_bs_bn(long long tiles_m, int N, int K, int ntaps, bool geglu, int num_s
 // Builds tensor maps / tile shapes for a problem.  Returns 0 on success.
 int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms);
 int gemm_launch(const GemmPlan& plan, cudaStream_t stream);
+
+// ---- split-K (fp16 output of a contraction too small to fill the machine): the kernel writes one fp32 partial per split
+// into scratch [splits][rows][N], then gemm_splitk_reduce folds them in split order and adds bias and residual.
+// Split count the kernel runs for `requested` splits of p: each split owns ceil(kt / requested) of the kt = taps x K-chunk
+// iterations and splits that would be left empty are dropped (kt = 30, 7 requested -> 6 splits of 5).  gemm_plan and the
+// fix-up pass both take the count from here.
+int gemm_split_count(const GemmProblem& p, int requested);
+// Why p cannot be split (nullptr if it can): GEGLU, LayerNorm fold, fp32 output, batched B, alpha != 1, N % 8 != 0, or
+// output / residual / bias rows the fix-up's 16-byte accesses cannot address.
+const char* gemm_splitk_unsupported(const GemmProblem& p);
+// fp32 elements the partials of `splits` splits occupy
+long long gemm_splitk_scratch_elems(const GemmProblem& p, int splits);
+// The partial-sum problem of p: same contraction, fp32 out into scratch, no bias / residual, `splits` = gemm_split_count
+GemmProblem gemm_splitk_partials(const GemmProblem& p, int splits, float* scratch);
+// Folds the partials gemm_splitk_partials(p, splits, scratch) wrote and applies p's bias (per sample with bias_rows) and
+// residual into p.out.
+int gemm_splitk_reduce(const GemmProblem& p, int splits, const float* scratch, cudaStream_t stream);
 // One-time: cudaFuncSetAttribute for all instantiations + driver entry point lookup.
 int gemm_init();
 // fp16 tensor map of rank `rank` with SWIZZLE_128B (box[0] = 64 elements); strides_bytes has rank-1 entries (dims 1..)

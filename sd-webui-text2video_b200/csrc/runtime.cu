@@ -388,38 +388,22 @@ int Builder::gemm(GemmProblem& p) {
     // 23040): each (tile, split) work item accumulates a K range into an fp32 partial, a fix-up kernel folds the partials
     // in a fixed order and applies bias / residual.  Deterministic; chosen only when >= half of the SMs would idle.
     static const bool no_split = getenv("T2V_NO_SPLITK") != nullptr;
-    if (!no_split && p.splits <= 1 && !(p.flags & (GEMM_GEGLU | GEMM_OUT_F32 | GEMM_LN)) && p.b_batch_dim < 0 && (p.N % 8) == 0 &&
-        p.alpha == 1.0f) {
+    if (!no_split && p.splits <= 1 && gemm_splitk_unsupported(p) == nullptr) {
         const long long tiles_m = (static_cast<long long>(rows) + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M;
         const long long tiles = tiles_m * ((p.N + 255) / 256);
         const int kt = p.ntaps * ((p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K);
-        int S = static_cast<int>(std::min<long long>(std::min<long long>(sms_ / std::max<long long>(tiles, 1), kt / 4), 8));
-        if (S >= 2) {       // the kernel never runs empty splits: use the split count gemm_plan will actually produce, the
-            const int kps = (kt + S - 1) / S;      // fix-up pass must not read partials nobody wrote
-            S = (kt + kps - 1) / kps;
-        }
+        // the split count the kernel runs (no empty splits): the fix-up pass must not read partials nobody wrote
+        const int S = gemm_split_count(
+            p, static_cast<int>(std::min<long long>(std::min<long long>(sms_ / std::max<long long>(tiles, 1), kt / 4), 8)));
         // (64-wide tiles without split-K were measured equal within 0.3 % on the whole forward: same MMA time per CTA)
         if (tiles * 2 <= sms_ && S >= 2) {
-            const long long nrows = static_cast<long long>(rows);
-            float* scratch = reinterpret_cast<float*>(arena_->alloc(static_cast<size_t>(S) * nrows * p.N * sizeof(float)));
-            GemmProblem q = p;
-            q.out = scratch;
-            q.ldo = p.N;
-            q.flags |= GEMM_OUT_F32;
-            q.bias = nullptr;
-            q.bias_rows = 0;
-            q.residual = nullptr;
-            q.splits = S;
-            q.split_stride = nrows * p.N;
+            float* scratch = reinterpret_cast<float*>(arena_->alloc(static_cast<size_t>(gemm_splitk_scratch_elems(p, S)) * sizeof(float)));
+            GemmProblem q = gemm_splitk_partials(p, S, scratch);
             q.force_bn = 256;
             const int rc = gemm(q);
             if (rc != 0) return rc;
             const GemmProblem o = p;
-            const int N = p.N;
-            step([=](cudaStream_t s) {
-                return splitk_reduce(scratch, S, nrows * N, nrows, N, o.bias, o.bias_rows, o.bias_stride, o.residual, o.ldr,
-                                     reinterpret_cast<__half*>(o.out), o.ldo, s);
-            }, 1, STEP_OTHER, 0.0, "splitk_reduce");
+            step([=](cudaStream_t s) { return gemm_splitk_reduce(o, S, scratch, s); }, 1, STEP_OTHER, 0.0, "splitk_reduce");
             arena_->free(reinterpret_cast<char*>(scratch));
             return 0;
         }

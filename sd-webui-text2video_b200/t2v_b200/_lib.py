@@ -81,6 +81,10 @@ SIGNATURES = {
     't2v_q_sample_blend': (c_int, [P, C.POINTER(c_ll), P, C.POINTER(c_ll), P, P, P, C.POINTER(c_ll), P, P, C.POINTER(c_int), P]),
     't2v_op_gemm': (c_int, [P, c_ll, c_int, c_int, C.POINTER(c_int), c_int, C.POINTER(c_int), P, c_int, c_int, c_int,
                             c_int, P, c_ll, P, c_int, c_ll, P, c_ll, c_float, c_int, c_int, P]),
+    't2v_op_gemm_splitk': (c_int, [P, c_ll, c_int, c_int, C.POINTER(c_int), c_int, C.POINTER(c_int), P, c_int, c_int, c_int,
+                                   c_int, P, c_ll, P, c_int, c_ll, P, c_ll, c_float, c_int, P, c_ll, C.POINTER(c_int), c_int,
+                                   c_int, P]),
+    't2v_op_ln_linear': (c_int, [P, c_ll, c_ll, c_int, P, P, P, P, c_int, c_int, P, P, P, P, P, c_ll, P, c_ll, c_int, c_int, P]),
     't2v_op_pack_conv_weight': (c_int, [P, c_int, P, c_int, c_int, c_int, c_int, c_int, P]),
     't2v_op_pack_geglu_weight': (c_int, [P, P, c_int, P, P, c_int, c_int, c_int, P]),
     't2v_op_groupnorm': (c_int, [P, c_ll, P, c_ll, c_ll, c_int, c_int, P, P, c_float, c_int, P]),

@@ -44,6 +44,97 @@ def gemm(a, w_packed, N, *, K=None, lda=None, dims=None, taps=None, n_alloc=None
     return out
 
 
+def gemm_splitk(a, w_packed, N, splits, *, scratch=None, K=None, lda=None, dims=None, taps=None, n_alloc=None, b_batch_dim=-1,
+                flags=0, out=None, ldo=None, bias=None, bias_rows=0, bias_stride=0, residual=None, ldr=None, alpha=1.0,
+                force_bn=0, force_cg=0):
+    """gemm's problem through split-K (fp32 partials per split, then a fix-up pass adding bias and residual).
+    scratch: fp32 CUDA tensor, by default [splits, rows, N].  Returns (out, number of splits run)."""
+    l = _lib.lib()
+    rows = a.shape[0]
+    K = K if K is not None else a.shape[1]
+    lda = lda if lda is not None else a.stride(0)
+    dims = list(dims) if dims is not None else [rows]
+    taps = taps if taps is not None else [[0] * len(dims)]
+    flat = [o for t in taps for o in t]
+    n_alloc = n_alloc if n_alloc is not None else w_packed.shape[-2]
+    if out is None:
+        out = torch.empty((rows, N), device=a.device, dtype=torch.float16)
+    if scratch is None:
+        scratch = torch.empty((max(splits, 1), rows, N), device=a.device, dtype=torch.float32)
+    ldo = ldo if ldo is not None else out.stride(0)
+    ldr = ldr if ldr is not None else (residual.stride(0) if residual is not None else 0)
+    used = C.c_int(0)
+    rc = l.t2v_op_gemm_splitk(_lib.ptr(a), lda, K, len(dims), _ia(dims), len(taps), _ia(flat), _lib.ptr(w_packed), n_alloc, N,
+                              b_batch_dim, flags, _lib.ptr(out), ldo, _lib.ptr(bias), bias_rows, bias_stride,
+                              _lib.ptr(residual), ldr, alpha, splits, _lib.ptr(scratch), scratch.numel(), C.byref(used),
+                              force_bn, force_cg, _lib.stream_ptr())
+    _lib.check(rc, 'op_gemm_splitk')
+    return out, used.value
+
+
+def ln_linear(x, w, bias, gamma, beta, *, flags=0, residual=None, out=None, force_bn=0, force_cg=0):
+    """Linear(LayerNorm(x)) (eps 1e-5) with the LayerNorm folded into the GEMM epilogue.  w [N, K] (GEGLU-packed with
+    flags=GEMM_GEGLU).  Returns (out, w_folded [N, K] fp16, colsum [N] fp32, bias32 [N] fp32, rowstat [rows, 2] fp32)."""
+    l = _lib.lib()
+    rows, K = x.shape
+    w = w.reshape(-1, K)
+    N = w.shape[0]
+    ncols = N // 2 if (flags & GEMM_GEGLU) else N
+    if out is None:
+        out = torch.empty((rows, ncols), device=x.device, dtype=torch.float16)
+    wf = torch.empty((N, K), device=x.device, dtype=torch.float16)
+    colsum = torch.empty((N,), device=x.device, dtype=torch.float32)
+    bias32 = torch.empty((N,), device=x.device, dtype=torch.float32)
+    rowstat = torch.empty((rows, 2), device=x.device, dtype=torch.float32)
+    rc = l.t2v_op_ln_linear(_lib.ptr(x), x.stride(0), rows, K, _lib.ptr(w), _lib.ptr(bias), _lib.ptr(gamma), _lib.ptr(beta), N,
+                            flags, _lib.ptr(wf), _lib.ptr(colsum), _lib.ptr(bias32), _lib.ptr(rowstat), _lib.ptr(residual),
+                            residual.stride(0) if residual is not None else 0, _lib.ptr(out), out.stride(0), force_bn, force_cg,
+                            _lib.stream_ptr())
+    _lib.check(rc, 'op_ln_linear')
+    return out, wf, colsum, bias32, rowstat
+
+
+def upsample2x(x):
+    """Nearest 2x upsampling of frames x [nframes, h, w, C] -> [nframes, 2h, 2w, C]."""
+    l = _lib.lib()
+    nf, h, w, Cc = x.shape
+    y = torch.empty((nf, 2 * h, 2 * w, Cc), device=x.device, dtype=torch.float16)
+    _lib.check(l.t2v_op_upsample2x(_lib.ptr(x), _lib.ptr(y), nf, h, w, Cc, _lib.stream_ptr()), 'op_upsample2x')
+    return y
+
+
+def im2col_s2(x):
+    """Stride-2 3x3 gather with padding 1: x [nframes, h, w, C] -> [nframes, ceil(h/2), ceil(w/2), 9 * C], column
+    tap * C + c with tap = ky * 3 + kx."""
+    l = _lib.lib()
+    nf, h, w, Cc = x.shape
+    col = torch.empty((nf, (h + 1) // 2, (w + 1) // 2, 9 * Cc), device=x.device, dtype=torch.float16)
+    _lib.check(l.t2v_op_im2col_s2(_lib.ptr(x), _lib.ptr(col), nf, h, w, Cc, _lib.stream_ptr()), 'op_im2col_s2')
+    return col
+
+
+def time_sinusoid(t, dim):
+    """Timestep embedding [cos(t f_k) | sin(t f_k)], f_k = 10000^(-k / (dim // 2)), fp16 [B, dim] (odd dim: last column 0).
+    t: fp32 CUDA [B]."""
+    l = _lib.lib()
+    out = torch.empty((t.numel(), dim), device=t.device, dtype=torch.float16)
+    _lib.check(l.t2v_op_time_sinusoid(_lib.ptr(t), _lib.ptr(out), t.numel(), dim, _lib.stream_ptr()), 'op_time_sinusoid')
+    return out
+
+
+def small_linear(x, w, bias=None, addend=None, silu_in=False):
+    """y = fp16(fp16(act(x) @ w^T + bias) + addend) for a few rows x [B, K], w [N, K]; act = SiLU rounded to fp16 when
+    silu_in.  Accumulation in fp32."""
+    l = _lib.lib()
+    B, K = x.shape
+    N = w.shape[0]
+    y = torch.empty((B, N), device=x.device, dtype=torch.float16)
+    rc = l.t2v_op_small_linear(_lib.ptr(x), x.stride(0), _lib.ptr(w), _lib.ptr(bias), _lib.ptr(addend), _lib.ptr(y), y.stride(0),
+                               B, N, K, int(silu_in), _lib.stream_ptr())
+    _lib.check(rc, 'op_small_linear')
+    return y
+
+
 def pack_conv_weight(w, n_alloc=None, k_alloc=None):
     """w [Cout, Cin, *k] (fp16/fp32, CUDA) -> [taps, n_alloc, k_alloc] fp16."""
     l = _lib.lib()

@@ -2,7 +2,8 @@
 arithmetic, so the output at each forced width (and with two-CTA clusters) must equal the BN = 64 output bit for bit.  The
 cases cover each epilogue kind ops.gemm reaches: plain, residual, fp32 output, per-sample bias, GEGLU, batched B with
 alpha, multi-dimensional row boxes with ragged (out-of-range) rows, ragged N, and unaligned rows (odd ldo / ldr), which
-store element by element.  The LayerNorm fold and split-K are reached through the UNet and checked by test_model_gpu."""
+store element by element.  The LayerNorm fold and split-K, which ops.gemm does not reach, have their own op-level tests
+(fp64 references, tile-width independence) in test_gemm_ln_splitk_gpu.py."""
 import pytest
 import torch
 
