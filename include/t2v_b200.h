@@ -84,6 +84,8 @@ int t2v_unet_forward_adapter(t2v_unet* u, const void* x, int x_is_f32, const flo
                              int w, int L, void* stream);
 /* 2*MAC flop count of one forward at this shape (for roofline reporting). */
 double t2v_unet_flops(t2v_unet* u, int B, int F, int h, int w, int L);
+/* Activation-slab bytes the plan of this shape allocates (host only: the same dry pass as t2v_unet_flops). */
+int t2v_unet_plan_bytes(t2v_unet* u, int B, int F, int h, int w, int L, size_t* arena);
 int t2v_unet_num_launches(t2v_unet* u);
 /* Measurement aid: replays the plan of this shape once (inputs = whatever the last forward left in the staging
  * buffers) with a CUDA-event pair around every launch on `stream` and sums per kernel family:
@@ -196,6 +198,28 @@ int t2v_vae_decode(t2v_vae* v, const void* z, int z_is_f32, float z_scale, void*
  * mean * 0.18215.  Needs the `encoder.*` / `quant_conv.*` parameters (optional for decode-only use). */
 int t2v_vae_encode(t2v_vae* v, const void* x, int x_is_f32, void* moments_out, int N, int H, int W, void* stream);
 double t2v_vae_flops(t2v_vae* v, int nframes, int h, int w);
+/* Frame chunking of long / high-resolution clips.  A plan's activation arena grows linearly with its frame count (0.83 GB per
+ * 576 x 1024 decoded frame).  t2v_vae_decode / t2v_vae_encode run the whole clip as one plan when that plan is cached or
+ * fits the memory budget -- exactly as without chunking -- and otherwise as ceil(frames / n) consecutive frame ranges
+ * (in (b f) order, a range may cross a sample boundary), n the largest frame count whose plan fits, the last range the
+ * tail; each range is written straight to its place in the caller's output.  A chunked call drops that direction's cached
+ * plans before it starts and after it ends (synchronising the stream): chunk plans are sized to the free memory and would
+ * otherwise starve the next network's plan.  Every op is per frame; only reduction
+ * orders that depend on the frame count (GroupNorm grid, GEMM split-K) can move the last bits (DESIGN.md section 2).
+ * If even one frame does not fit, the call fails (-4) before allocating anything.
+ *   direction: 0 = decode, 1 = encode; h, w as the entry point takes them (latent for decode, image for encode).
+ *   plan_bytes: arena and GroupNorm workspace bytes a plan of this shape would allocate (host only, no GPU needed).
+ *   plan_chunks: the split the policy picks for `budget` bytes (host only); -4 if one frame does not fit.
+ *   set / get_memory_budget: bytes of plan (arena + GroupNorm workspace) one direction may hold; 0 (default) = automatic:
+ *     free device memory + this direction's cached arenas + the GroupNorm workspace - 512 MB.
+ *   last_chunking: how the last call of that direction was split (n_chunks = 1: the whole-clip plan; 0 before any call).
+ *   cached_plans: number of cached plans of that direction and (if non-null) their arena bytes together.            */
+int t2v_vae_plan_bytes(t2v_vae* v, int direction, int frames, int h, int w, size_t* arena, size_t* gn_workspace);
+int t2v_vae_plan_chunks(t2v_vae* v, int direction, int frames, int h, int w, size_t budget, int* chunk_frames, int* n_chunks);
+int t2v_vae_set_memory_budget(t2v_vae* v, size_t bytes);
+size_t t2v_vae_get_memory_budget(t2v_vae* v);
+int t2v_vae_last_chunking(t2v_vae* v, int direction, int* chunk_frames, int* n_chunks);
+int t2v_vae_cached_plans(t2v_vae* v, int direction, size_t* slab_bytes);
 /* VideoCrafter LoRA on the decoder's and the encoder's weights (see "VideoCrafter LoRA" above) */
 int t2v_vae_lora_apply(t2v_vae* v, const char* weight_name, const void* up, const void* down, int dtype, int rank, float alpha,
                        void* stream);

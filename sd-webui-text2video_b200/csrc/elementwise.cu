@@ -20,19 +20,20 @@ inline int grid_for(long long n, int threads, int cap = 132 * 16) {
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < (n); \
          i += static_cast<long long>(gridDim.x) * blockDim.x)
 
-__global__ void ingest_kernel(const void* x, int x_is_f32, __half* tok, long long ld, int cpad, int B, int C, int F,
-                              int h, int w, float scale) {
+// frames [frame0, frame0 + nframes) of the (b f) order of x [B, C, F, h, w] -> tok rows [nframes * h * w][ld]
+__global__ void ingest_kernel(const void* x, int x_is_f32, __half* tok, long long ld, int cpad, int C, int F, int h, int w,
+                              long long frame0, long long nframes, float scale) {
     griddep_wait();
     griddep_launch_small();
     const long long P = static_cast<long long>(h) * w;
-    const long long rows = static_cast<long long>(B) * F * P;
+    const long long rows = nframes * P;
     GRID_STRIDE(i, rows * cpad) {
         const long long r = i / cpad;
         const int c = static_cast<int>(i - r * cpad);
         float v = 0.f;
         if (c < C) {
             const long long p = r % P;
-            const long long bf = r / P;
+            const long long bf = frame0 + r / P;
             const int f = static_cast<int>(bf % F);
             const int b = static_cast<int>(bf / F);
             const long long src = ((static_cast<long long>(b) * C + c) * F + f) * P + p;
@@ -625,8 +626,12 @@ inline int ok() { return launch_status("elementwise launch"); }
 
 int ingest_latent(const void* x, int x_is_f32, __half* tok, long long ld, int cpad, int B, int C, int F, int h, int w,
                   float scale, cudaStream_t stream) {
-    const long long n = static_cast<long long>(B) * F * h * w * cpad;
-    launch_pdl(ingest_kernel, grid_for(n, 256), 256, 0, stream, x, x_is_f32, tok, ld, cpad, B, C, F, h, w, scale);
+    return ingest_latent_frames(x, x_is_f32, tok, ld, cpad, C, F, h, w, 0, static_cast<long long>(B) * F, scale, stream);
+}
+int ingest_latent_frames(const void* x, int x_is_f32, __half* tok, long long ld, int cpad, int C, int F, int h, int w,
+                         long long frame0, long long nframes, float scale, cudaStream_t stream) {
+    const long long n = nframes * h * w * cpad;
+    launch_pdl(ingest_kernel, grid_for(n, 256), 256, 0, stream, x, x_is_f32, tok, ld, cpad, C, F, h, w, frame0, nframes, scale);
     return ok();
 }
 int egress_latent(const __half* tok, long long ld, void* out, int out_is_f32, int B, int C, int F, int h, int w,

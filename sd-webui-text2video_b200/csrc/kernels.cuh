@@ -76,6 +76,10 @@ int attention_tc_launch(const AttnTcPlan& plan, cudaStream_t stream);
 // x [B, C, F, h, w] (fp32 or fp16, NCFHW as the samplers hold it) -> tokens [B*F*h*w, ld] fp16, channels >= C zeroed up to cpad
 int ingest_latent(const void* x, int x_is_f32, __half* tok, long long ld, int cpad, int B, int C, int F, int h, int w,
                   float scale, cudaStream_t stream);
+// the same for frames [frame0, frame0 + nframes) of x in (b f) order (a range may cross a sample boundary; B is implied):
+// tokens [nframes*h*w, ld], read straight from the strided latent
+int ingest_latent_frames(const void* x, int x_is_f32, __half* tok, long long ld, int cpad, int C, int F, int h, int w,
+                         long long frame0, long long nframes, float scale, cudaStream_t stream);
 // tokens [B*F*h*w, ld] -> out [B, C, F, h, w] (fp32 or fp16)
 int egress_latent(const __half* tok, long long ld, void* out, int out_is_f32, int B, int C, int F, int h, int w,
                   cudaStream_t stream);

@@ -513,7 +513,7 @@ long long dry_build(const std::shared_ptr<PlanShard>& shard, bool no_reuse, cons
 int build_plan(Plan* plan, unsigned long long weights_version, bool no_reuse, const char* label, const BuildFn& build) {
     const long long peak = dry_build(plan->shard, no_reuse, build);
     if (peak < 0) return -1;
-    const size_t bytes = static_cast<size_t>(peak) + (1 << 20);
+    const size_t bytes = plan_slab_bytes(peak);
     if (cudaMalloc(&plan->slab, bytes) != cudaSuccess) {
         plan->slab = nullptr;
         set_error("%s activation slab cudaMalloc(%zu MB) failed", label, bytes >> 20);

@@ -223,6 +223,8 @@ using BuildFn = std::function<int(Plan* plan, Arena* arena, bool dry)>;
 // The dry pass alone, on a scratch plan sharing `shard`: returns the peak activation bytes (-1 if the build failed) and
 // stores the plan's algorithmic flop count in *flops.
 long long dry_build(const std::shared_ptr<PlanShard>& shard, bool no_reuse, const BuildFn& build, double* flops = nullptr);
+// The slab build_plan allocates for a dry-pass peak of `peak` bytes.
+inline size_t plan_slab_bytes(long long peak) { return static_cast<size_t>(peak) + (1 << 20); }
 // Builds `plan` (a shell: the caller may have set its shard): the dry pass measures the peak, one slab of peak + 1 MB is
 // allocated, the real pass records the launches against it, and the plan is stamped with `weights_version`.  `label`
 // names the network in the error message of a failed slab allocation.  Returns 0, or < 0 with the error set.
@@ -274,6 +276,12 @@ public:
         if (entries_.empty()) return;
         cudaStreamSynchronize(stream);
         entries_.clear();
+    }
+    size_t size() const { return entries_.size(); }
+    size_t slab_bytes() const {          // activation slabs of the cached plans, together
+        size_t s = 0;
+        for (const Entry& e : entries_) s += e.plan->slab_bytes;
+        return s;
     }
 
 private:

@@ -1180,6 +1180,16 @@ double t2v_unet_flops(t2v_unet* u, int B, int F, int h, int w, int L) {
     return flops;
 }
 
+int t2v_unet_plan_bytes(t2v_unet* u, int B, int F, int h, int w, int L, size_t* arena) {
+    if (!u || !arena) return -1;
+    IO io;
+    const long long peak =
+        dry_build(new_plan_shard(u, F), false, [&](Plan* p, Arena* a, bool dry) { return build(u, p, a, dry, nullptr, B, F, h, w, L, &io); });
+    if (peak < 0) return -1;
+    *arena = plan_slab_bytes(peak);
+    return 0;
+}
+
 int t2v_unet_num_launches(t2v_unet* u) { return u->last_launches; }
 
 int t2v_unet_profile(t2v_unet* u, int B, int F, int h, int w, int L, void* stream_, double* out13) {

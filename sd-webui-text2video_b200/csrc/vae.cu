@@ -38,6 +38,8 @@ struct t2v_vae {
     PlanCache<VIO> plans{3};    // key: "frames,h,w"
     PlanCache<EncIO> enc_plans{3};
     GnWorkspace gn_ws;          // shared by the decoder's and the encoder's plans
+    size_t budget = 0;          // plan bytes (arena + GroupNorm workspace) one direction may hold; 0: automatic
+    int last_chunk[2] = {0, 0}, last_n_chunks[2] = {0, 0};      // how the last decode [0] / encode [1] was split
 };
 
 namespace t2v {
@@ -262,12 +264,17 @@ std::string shape_key(int frames, int h, int w) {
     return std::to_string(frames) + "," + std::to_string(h) + "," + std::to_string(w);
 }
 
+// GroupNorm workspace the decoder's / the encoder's plan of this shape needs (largest and smallest resolution, + 1 MB)
+size_t dec_gn_need(int frames, int h, int w) {
+    return std::max(gn_workspace_bytes(h * w, frames, num_sms()), gn_workspace_bytes(h * w * 64, frames, num_sms())) + (1 << 20);
+}
+size_t enc_gn_need(int frames, int H, int W) { return gn_workspace_bytes(H * W, frames, num_sms()) + (1 << 20); }
+
 PlanCache<VIO>::Entry* get_plan(t2v_vae* v, int frames, int h, int w, cudaStream_t stream) {
     const std::string key = shape_key(frames, h, w);
     if (auto* e = v->plans.find(key, v->params.version())) return e;
     if (!v->params.complete("VAE")) return nullptr;
-    const size_t need = std::max(gn_workspace_bytes(h * w, frames, num_sms()), gn_workspace_bytes(h * w * 64, frames, num_sms()));
-    if (!ensure_gn_ws(v, need + (1 << 20), stream)) return nullptr;
+    if (!ensure_gn_ws(v, dec_gn_need(frames, h, w), stream)) return nullptr;
     return v->plans.build(key, v->params.version(), stream, std::unique_ptr<Plan>(new Plan()), false, "VAE",
                           [&](Plan* p, Arena* a, bool dry, VIO* io) { return build(v, p, a, dry, stream, frames, h, w, io); });
 }
@@ -345,9 +352,122 @@ PlanCache<EncIO>::Entry* get_enc_plan(t2v_vae* v, int frames, int H, int W, cuda
     const std::string key = shape_key(frames, H, W);
     if (auto* e = v->enc_plans.find(key, v->enc_params.version())) return e;
     if (!v->enc_params.complete("VAE encoder")) return nullptr;
-    if (!ensure_gn_ws(v, gn_workspace_bytes(H * W, frames, num_sms()) + (1 << 20), stream)) return nullptr;
+    if (!ensure_gn_ws(v, enc_gn_need(frames, H, W), stream)) return nullptr;
     return v->enc_plans.build(key, v->enc_params.version(), stream, std::unique_ptr<Plan>(new Plan()), false, "VAE encoder",
                               [&](Plan* p, Arena* a, bool dry, EncIO* io) { return build_enc(v, p, a, dry, stream, frames, H, W, io); });
+}
+
+// ---------------------------------------------------------------------------------------------- frame chunking
+// A plan's arena grows linearly with the frame count (0.83 GB per 576 x 1024 decoded frame), so a long or large clip may not
+// fit the device as one plan.  Every op of the decoder and the encoder is per frame, so the clip can run as consecutive
+// frame ranges instead, each through a plan of that many frames.  Chunking starts only where the whole-clip plan does not
+// fit: a clip that fits runs exactly as before.
+enum { DEC = 0, ENC = 1 };
+
+// Automatic budget: free device memory, plus what this direction's cached plans and the GroupNorm workspace already hold
+// (both are dropped or regrown to make room), minus this margin.  The margin covers what a plan build allocates outside its
+// arena: the packed weight copies made on the first build (~100 MB for the SD VAE's decoder in fp16), the instantiated
+// CUDA graph and the 2 MB rounding of each allocation, with room left for the caller's own small allocations meanwhile.
+constexpr size_t kBudgetMargin = size_t(512) << 20;
+
+// Bytes a plan of `frames` frames would allocate: its activation slab (*arena) and the GroupNorm workspace it needs (*gn).
+// Host only (the dry pass).  h, w are what the entry point takes: the latent's for decode, the image's for encode.
+int plan_bytes(t2v_vae* v, int dir, int frames, int h, int w, size_t* arena, size_t* gn) {
+    long long peak;
+    if (dir == DEC) {
+        VIO io;
+        peak = dry_build(nullptr, false, [&](Plan* p, Arena* a, bool dry) { return build(v, p, a, dry, nullptr, frames, h, w, &io); });
+        *gn = dec_gn_need(frames, h, w);
+    } else {
+        EncIO io;
+        peak = dry_build(nullptr, false, [&](Plan* p, Arena* a, bool dry) { return build_enc(v, p, a, dry, nullptr, frames, h, w, &io); });
+        *gn = enc_gn_need(frames, h, w);
+    }
+    if (peak < 0) return -1;
+    *arena = plan_slab_bytes(peak);
+    return 0;
+}
+
+// The largest n <= frames whose plan (arena + GroupNorm workspace) fits `budget`, found by bisection (plan bytes grow with
+// the frame count).  Returns 0 with *n set; -4 if not even one frame fits (*one_frame = its plan bytes, error set); -1 if
+// the dry pass failed.
+int choose_chunk(t2v_vae* v, int dir, int frames, int h, int w, size_t budget, int* n, size_t* one_frame) {
+    auto bytes = [&](int f, size_t* out) {
+        size_t a = 0, g = 0;
+        if (plan_bytes(v, dir, f, h, w, &a, &g) != 0) return false;
+        *out = a + g;
+        return true;
+    };
+    size_t b = 0;
+    if (!bytes(frames, &b)) return -1;
+    if (b <= budget) {
+        *n = frames;
+        return 0;
+    }
+    if (!bytes(1, one_frame)) return -1;
+    if (*one_frame > budget) {
+        set_error("VAE %s of %d frames of %d x %d %s: a one-frame plan needs %.1f MB, more than the memory budget of %.1f MB",
+                  dir == DEC ? "decode" : "encode", frames, h, w, dir == DEC ? "latents" : "pixels", *one_frame / 1048576.0,
+                  budget / 1048576.0);
+        return -4;
+    }
+    int lo = 1, hi = frames;          // lo fits, hi does not
+    while (hi - lo > 1) {
+        const int mid = lo + (hi - lo) / 2;
+        if (!bytes(mid, &b)) return -1;
+        (b <= budget ? lo : hi) = mid;
+    }
+    *n = lo;
+    return 0;
+}
+
+size_t call_budget(t2v_vae* v, size_t cached) {
+    if (v->budget != 0) return v->budget;
+    size_t free_b = 0, total_b = 0;
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) {
+        cudaGetLastError();
+        return SIZE_MAX;              // no reading: the whole-clip path, as before
+    }
+    const size_t avail = free_b + cached + v->gn_ws.bytes;
+    return avail > kBudgetMargin ? avail - kBudgetMargin : 0;
+}
+
+// Runs a clip of `frames` frames through the plans of `cache`: as one plan if it is cached or fits the budget, else as
+// ceil(frames / n) consecutive ranges of n frames (the last one the tail), n the largest that fits.  Before a plan is
+// built, this direction's cached plans are dropped if the new one would not fit beside them.  A chunked call drops this
+// direction's plans when it starts and again when it ends: its chunk plans are sized to the free memory, and keeping them
+// would starve whatever runs next (the UNet after a vid2vid encode, a decode after it).  get(nf) returns the entry of an
+// nf-frame plan (building it), run(entry, f0, nf) stages frames [f0, f0 + nf), replays the plan and writes the result.
+template <class IO, class Get, class Run>
+int run_in_chunks(t2v_vae* v, int dir, PlanCache<IO>& cache, const ParamStore& P, const char* what, int frames, int h, int w,
+                  cudaStream_t stream, Get&& get, Run&& run) {
+    int n = frames;
+    size_t budget = SIZE_MAX;
+    if (!cache.find(shape_key(frames, h, w), P.version())) {
+        if (!P.complete(what)) return -1;
+        budget = call_budget(v, cache.slab_bytes());
+        size_t one = 0;
+        const int rc = choose_chunk(v, dir, frames, h, w, budget, &n, &one);
+        if (rc == -4) return rc;
+        if (rc != 0) n = frames;      // dry pass failed: the build below reports why
+    }
+    const int n_chunks = (frames + n - 1) / n;
+    const int tail = frames - (n_chunks - 1) * n;
+    if (n_chunks > 1) cache.clear(stream);
+    v->last_chunk[dir] = n;
+    v->last_n_chunks[dir] = n_chunks;
+    int rc = 0;
+    for (int c = 0; c < n_chunks && rc == 0; ++c) {
+        const int f0 = c * n, nf = c + 1 < n_chunks ? n : tail;
+        if (budget != SIZE_MAX && !cache.find(shape_key(nf, h, w), P.version())) {
+            size_t a = 0, g = 0;
+            if (plan_bytes(v, dir, nf, h, w, &a, &g) == 0 && cache.slab_bytes() + a + g > budget) cache.clear(stream);
+        }
+        auto* e = get(nf);
+        rc = e ? run(e, f0, nf) : -1;
+    }
+    if (n_chunks > 1) cache.clear(stream);
+    return rc;
 }
 
 }  // namespace
@@ -414,27 +534,25 @@ int t2v_vae_decode(t2v_vae* v, const void* z, int z_is_f32, float z_scale, void*
                    int w, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const int frames = B * F;
-    auto* entry = get_plan(v, frames, h, w, stream);
-    if (!entry) return -1;
-    const VIO& io = entry->io;
-    const int zpad = (v->cfg.z_channels + 7) / 8 * 8;
-    int rc = ingest_latent(z, z_is_f32, io.z_tok, zpad, zpad, B, v->cfg.z_channels, F, h, w, z_scale, stream);
-    if (rc != 0) return rc;
-    rc = run_plan(entry->plan.get(), stream, true);
-    if (rc != 0) {
-        set_error("VAE launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
-        return rc;
-    }
-    const int H = h * 8, W = w * 8;       // 3 upsamples for the 4-level decoder
     int up = 1;
     for (int i = 1; i < v->cfg.n_mult; ++i) up *= 2;
-    const int Ho = h * up, Wo = w * up;
-    (void)H;
-    (void)W;
-    if (out_mode == 1)
-        return frames_to_u8(io.out_tok, io.out_ld, reinterpret_cast<uint8_t*>(out), static_cast<long long>(frames) * Ho * Wo,
-                            stream);
-    return frames_to_f32_nchw(io.out_tok, io.out_ld, reinterpret_cast<float*>(out), frames, Ho, Wo, stream);
+    const long long pix = static_cast<long long>(h * up) * (w * up);      // pixels of one output frame
+    const int zpad = (v->cfg.z_channels + 7) / 8 * 8;
+    return run_in_chunks(
+        v, DEC, v->plans, v->params, "VAE", frames, h, w, stream, [&](int nf) { return get_plan(v, nf, h, w, stream); },
+        [&](PlanCache<VIO>::Entry* entry, int f0, int nf) {
+            const VIO& io = entry->io;
+            int rc = ingest_latent_frames(z, z_is_f32, io.z_tok, zpad, zpad, v->cfg.z_channels, F, h, w, f0, nf, z_scale, stream);
+            if (rc != 0) return rc;
+            rc = run_plan(entry->plan.get(), stream, true);
+            if (rc != 0) {
+                set_error("VAE launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+                return rc;
+            }
+            if (out_mode == 1)
+                return frames_to_u8(io.out_tok, io.out_ld, reinterpret_cast<uint8_t*>(out) + f0 * pix * 3, nf * pix, stream);
+            return frames_to_f32_nchw(io.out_tok, io.out_ld, reinterpret_cast<float*>(out) + f0 * pix * 3, nf, h * up, w * up, stream);
+        });
 }
 
 int t2v_vae_encode(t2v_vae* v, const void* x, int x_is_f32, void* moments_out, int N, int H, int W, void* stream_) {
@@ -445,17 +563,22 @@ int t2v_vae_encode(t2v_vae* v, const void* x, int x_is_f32, void* moments_out, i
         set_error("t2v_vae_encode: H and W must be multiples of %d (got %d x %d)", down, H, W);
         return -3;
     }
-    auto* entry = get_enc_plan(v, N, H, W, stream);
-    if (!entry) return -1;
-    const EncIO& io = entry->io;
-    int rc = ingest_latent(x, x_is_f32, io.x_tok, 8, 8, N, 3, 1, H, W, 1.0f, stream);
-    if (rc != 0) return rc;
-    rc = run_plan(entry->plan.get(), stream, true);
-    if (rc != 0) {
-        set_error("VAE encoder launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
-        return rc;
-    }
-    return egress_latent(io.out_tok, io.out_ld, moments_out, 1, N, 2 * v->cfg.embed_dim, 1, io.ho, io.wo, stream);
+    const long long in_frame = 3LL * H * W * (x_is_f32 ? 4 : 2);          // bytes of one input frame
+    const int M = 2 * v->cfg.embed_dim;
+    return run_in_chunks(
+        v, ENC, v->enc_plans, v->enc_params, "VAE encoder", N, H, W, stream, [&](int nf) { return get_enc_plan(v, nf, H, W, stream); },
+        [&](PlanCache<EncIO>::Entry* entry, int f0, int nf) {
+            const EncIO& io = entry->io;
+            int rc = ingest_latent(static_cast<const char*>(x) + f0 * in_frame, x_is_f32, io.x_tok, 8, 8, nf, 3, 1, H, W, 1.0f, stream);
+            if (rc != 0) return rc;
+            rc = run_plan(entry->plan.get(), stream, true);
+            if (rc != 0) {
+                set_error("VAE encoder launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+                return rc;
+            }
+            float* mom = static_cast<float*>(moments_out) + static_cast<long long>(f0) * M * io.ho * io.wo;
+            return egress_latent(io.out_tok, io.out_ld, mom, 1, nf, M, 1, io.ho, io.wo, stream);
+        });
 }
 
 double t2v_vae_flops(t2v_vae* v, int nframes, int h, int w) {
@@ -464,6 +587,48 @@ double t2v_vae_flops(t2v_vae* v, int nframes, int h, int w) {
     if (dry_build(nullptr, false, [&](Plan* p, Arena* a, bool dry) { return build(v, p, a, dry, nullptr, nframes, h, w, &io); }, &flops) < 0)
         return -1.0;
     return flops;
+}
+
+int t2v_vae_plan_bytes(t2v_vae* v, int direction, int frames, int h, int w, size_t* arena, size_t* gn_workspace) {
+    if (!v || !arena || !gn_workspace || (direction != DEC && direction != ENC) || frames < 1 || h < 1 || w < 1) return -1;
+    if (plan_bytes(v, direction, frames, h, w, arena, gn_workspace) != 0) {
+        set_error("t2v_vae_plan_bytes: the dry pass failed at %d frames of %d x %d", frames, h, w);
+        return -1;
+    }
+    return 0;
+}
+
+int t2v_vae_plan_chunks(t2v_vae* v, int direction, int frames, int h, int w, size_t budget, int* chunk_frames, int* n_chunks) {
+    if (!v || !chunk_frames || !n_chunks || (direction != DEC && direction != ENC) || frames < 1 || h < 1 || w < 1) return -1;
+    int n = 0;
+    size_t one = 0;
+    const int rc = choose_chunk(v, direction, frames, h, w, budget, &n, &one);
+    if (rc != 0) return rc;
+    *chunk_frames = n;
+    *n_chunks = (frames + n - 1) / n;
+    return 0;
+}
+
+int t2v_vae_set_memory_budget(t2v_vae* v, size_t bytes) {
+    if (!v) return -1;
+    v->budget = bytes;
+    return 0;
+}
+
+size_t t2v_vae_get_memory_budget(t2v_vae* v) { return v ? v->budget : 0; }
+
+int t2v_vae_last_chunking(t2v_vae* v, int direction, int* chunk_frames, int* n_chunks) {
+    if (!v || !chunk_frames || !n_chunks || (direction != DEC && direction != ENC)) return -1;
+    *chunk_frames = v->last_chunk[direction];
+    *n_chunks = v->last_n_chunks[direction];
+    return 0;
+}
+
+int t2v_vae_cached_plans(t2v_vae* v, int direction, size_t* slab_bytes) {
+    if (!v || (direction != DEC && direction != ENC)) return -1;
+    const size_t n = direction == DEC ? v->plans.size() : v->enc_plans.size();
+    if (slab_bytes) *slab_bytes = direction == DEC ? v->plans.slab_bytes() : v->enc_plans.slab_bytes();
+    return static_cast<int>(n);
 }
 
 }  // extern "C"

@@ -26,6 +26,7 @@ SIGNATURES = {
     't2v_unet_forward': (c_int, [P, P, c_int, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     't2v_unet_forward_adapter': (c_int, [P, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     't2v_unet_flops': (c_double, [P, c_int, c_int, c_int, c_int, c_int]),
+    't2v_unet_plan_bytes': (c_int, [P, c_int, c_int, c_int, c_int, c_int, C.POINTER(C.c_size_t)]),
     't2v_unet_num_launches': (c_int, [P]),
     't2v_unet_profile': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, C.POINTER(c_double)]),
     't2v_unet_read_tap': (c_ll, [P, c_char_p, P, c_ll, P]),
@@ -62,6 +63,12 @@ SIGNATURES = {
     't2v_vae_decode': (c_int, [P, P, c_int, c_float, P, c_int, c_int, c_int, c_int, c_int, P]),
     't2v_vae_encode': (c_int, [P, P, c_int, P, c_int, c_int, c_int, P]),
     't2v_vae_flops': (c_double, [P, c_int, c_int, c_int]),
+    't2v_vae_plan_bytes': (c_int, [P, c_int, c_int, c_int, c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    't2v_vae_plan_chunks': (c_int, [P, c_int, c_int, c_int, c_int, C.c_size_t, C.POINTER(c_int), C.POINTER(c_int)]),
+    't2v_vae_set_memory_budget': (c_int, [P, C.c_size_t]),
+    't2v_vae_get_memory_budget': (C.c_size_t, [P]),
+    't2v_vae_last_chunking': (c_int, [P, c_int, C.POINTER(c_int), C.POINTER(c_int)]),
+    't2v_vae_cached_plans': (c_int, [P, c_int, C.POINTER(C.c_size_t)]),
     't2v_clip_create': (c_int, [P, C.POINTER(P)]),
     't2v_clip_destroy': (None, [P]),
     't2v_clip_set_param': (c_int, [P, c_char_p, P, c_int, c_int, C.POINTER(C.c_int64), P]),

@@ -356,6 +356,12 @@ class UNetSD(_NativeModule):
     def flops(self, B, F, h, w, L=77):
         return _lib.load_library().t2v_unet_flops(self._handle, B, F, h, w, L)
 
+    def plan_bytes(self, B, F, h, w, L=77):
+        """Activation-arena bytes of the plan of this shape (host only, no GPU needed)."""
+        arena = C.c_size_t(0)
+        _lib.check(_lib.load_library().t2v_unet_plan_bytes(self._handle, B, F, h, w, L, C.byref(arena)), 'unet_plan_bytes')
+        return arena.value
+
     def num_launches(self):
         return _lib.load_library().t2v_unet_num_launches(self._handle)
 
@@ -592,3 +598,44 @@ class AutoencoderKL(_NativeModule):
 
     def flops(self, nframes, h, w):
         return _lib.load_library().t2v_vae_flops(self._handle, nframes, h, w)
+
+    # Frame chunking (include/t2v_b200.h, "Frame chunking"): a clip whose plan does not fit the memory budget is decoded /
+    # encoded as consecutive frame ranges inside decode_video / decode / encode; a clip that fits runs as one plan, as before.
+    @property
+    def memory_budget(self):
+        """Bytes of plan (activation arena + GroupNorm workspace) decode or encode may hold; 0 (the default) = automatic:
+        free device memory + what this module's cached plans of that direction hold - 512 MB."""
+        return int(_lib.load_library().t2v_vae_get_memory_budget(self._handle))
+
+    @memory_budget.setter
+    def memory_budget(self, nbytes):
+        if int(nbytes) < 0:
+            raise ValueError('memory_budget is a byte count (0 = automatic)')
+        _lib.check(_lib.load_library().t2v_vae_set_memory_budget(self._handle, int(nbytes)), 'vae_set_memory_budget')
+
+    def plan_bytes(self, frames, h, w, encode=False):
+        """Bytes one plan of `frames` frames allocates, its arena plus its GroupNorm workspace (host only, no GPU needed).
+        h, w: the latent's size for decode, the image's size for encode (what decode / encode take)."""
+        arena, gn = C.c_size_t(0), C.c_size_t(0)
+        _lib.check(_lib.load_library().t2v_vae_plan_bytes(self._handle, int(encode), frames, h, w, C.byref(arena), C.byref(gn)),
+                   'vae_plan_bytes')
+        return arena.value + gn.value
+
+    def plan_chunks(self, frames, h, w, budget, encode=False):
+        """(frames per chunk, chunks) the library picks for a clip under `budget` bytes (host only); (frames, 1) if it fits."""
+        n, k = C.c_int(0), C.c_int(0)
+        _lib.check(_lib.load_library().t2v_vae_plan_chunks(self._handle, int(encode), frames, h, w, int(budget), C.byref(n),
+                                                           C.byref(k)), 'vae_plan_chunks')
+        return n.value, k.value
+
+    def last_chunking(self, encode=False):
+        """(frames per chunk, chunks) of the last decode (encode=False) or encode; chunks = 1 is the whole-clip plan."""
+        n, k = C.c_int(0), C.c_int(0)
+        _lib.check(_lib.load_library().t2v_vae_last_chunking(self._handle, int(encode), C.byref(n), C.byref(k)), 'vae_last_chunking')
+        return n.value, k.value
+
+    def cached_plans(self, encode=False):
+        """(number, arena bytes together) of the decoder's (encode=False) or the encoder's cached plans."""
+        nbytes = C.c_size_t(0)
+        n = _lib.load_library().t2v_vae_cached_plans(self._handle, int(encode), C.byref(nbytes))
+        return n, nbytes.value

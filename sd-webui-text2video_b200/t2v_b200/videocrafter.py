@@ -129,7 +129,9 @@ class LatentDiffusion(nn.Module):
     @torch.no_grad()
     def decode_first_stage_2DAE(self, z, decode_bs=16, return_cpu=True, **kwargs):
         """z [b, 4, t, h, w] -> video [b, 3, t, 8h, 8w] in [-1, 1]; all frames decoded in one batch (decode_bs only splits
-        work in the reference, the result is identical)."""
+        work in the reference, the result is identical).  `decode_bs` stays ignored: honouring it would change the plan, and
+        possibly the last bits, of clips that fit today.  A clip too large for the device is split into frame chunks by
+        the library instead, sized to the free memory (AutoencoderKL.memory_budget)."""
         b, _, t, _, _ = z.shape
         frames = self.first_stage_model.decode_video(z, z_scale=1.0 / self.scale_factor, as_uint8=False)   # [(b t), 3, H, W]
         out = frames.reshape(b, t, *frames.shape[1:]).permute(0, 2, 1, 3, 4).contiguous()
