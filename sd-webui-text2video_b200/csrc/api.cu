@@ -5,7 +5,6 @@
 #include "kernels.cuh"
 
 #include <cstdarg>
-#include <cstdlib>
 #include <cstdio>
 #include <cstring>
 
@@ -35,10 +34,6 @@ int launch_status(const char* what) {
     if (e == cudaSuccess) return 0;
     set_error("%s: %s (%s)", what, cudaGetErrorString(e), cudaGetErrorName(e));
     return -2;
-}
-bool pdl_enabled() {
-    static const bool on = getenv("T2V_PDL") != nullptr;      // opt-in (common.cuh)
-    return on;
 }
 
 static void* gn_scratch(size_t bytes) {
@@ -332,7 +327,7 @@ int t2v_op_attention_hd(const void* q, const void* k, const void* v, void* o, lo
     p.q_bs = q_bs; p.q_ss = q_ss; p.k_bs = k_bs; p.k_ss = k_ss; p.v_bs = v_bs; p.v_ss = v_ss; p.o_bs = o_bs; p.o_ss = o_ss;
     p.batch = batch; p.heads = heads; p.sq = sq; p.skv = skv; p.head_dim = head_dim; p.kv_batch_div = kv_batch_div;
     p.scale = scale; p.b_inner = 1;
-    return head_dim == 64 ? attention(p, reinterpret_cast<cudaStream_t>(stream)) : attention_hd(p, reinterpret_cast<cudaStream_t>(stream));
+    return attention(p, reinterpret_cast<cudaStream_t>(stream));
 }
 int t2v_op_attention_relpos(const void* q, const void* k, const void* v, void* o, const void* table_k, const void* table_v,
                             long long n_seq, long long seq_inner, long long bs_outer, long long bs_inner, long long ss,

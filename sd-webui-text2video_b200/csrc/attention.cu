@@ -9,7 +9,6 @@
 // P rounded to fp16 for P.V -- the numerics of torch SDPA's fused kernels that the reference dispatches to on the GPU,
 // t2v_model.py:566-569).  It serves the SHORT sequences: temporal attention (S = frames, 32 x 32 tiles), cross-attention
 // (77 keys) and the coarse levels (h*w < 256).  Long spatial sequences go to the wgmma kernel in attention_tc.cu.
-#include <cstdlib>
 
 #include "common.cuh"
 #include "kernels.cuh"
@@ -43,8 +42,6 @@ __device__ __forceinline__ void load_tile(uint32_t smem_tile, const __half* gbas
 
 template <int TS>
 __global__ void __launch_bounds__(2 * TS) attention_kernel(AttnParams p) {
-    griddep_wait();
-    griddep_launch_small();
     constexpr int BM = TS, BNK = TS, NB = TS / 8, KS = TS / 16, TB = TS * 128;   // tile bytes
     // Q | K0 | V0 | K1 | V1: single-tile problems (temporal attention: S = frames <= 32, the gather is latency-bound) are launched with
     // the first three tiles only -> 12 KB instead of 20 KB per 64-thread CTA, 18 instead of 11 resident CTAs per SM
@@ -206,8 +203,9 @@ __global__ void __launch_bounds__(2 * TS) attention_kernel(AttnParams p) {
 }  // namespace
 
 int attention(const AttnParams& p, cudaStream_t stream) {
-    if (p.head_dim != HD || p.sq <= 0 || p.skv <= 0 || p.kv_batch_div <= 0 || p.b_inner <= 0) return -1;
-    if (attention_tc_eligible(p) && !getenv("T2V_ATTN_WARP_MMA")) {
+    if (p.head_dim != HD) return attention_hd(p, stream);
+    if (p.sq <= 0 || p.skv <= 0 || p.kv_batch_div <= 0 || p.b_inner <= 0) return -1;
+    if (attention_tc_eligible(p)) {
         AttnTcPlan plan;
         const int rc = attention_tc_plan(p, &plan);
         if (rc != 0) return rc;
@@ -219,8 +217,8 @@ int attention(const AttnParams& p, cudaStream_t stream) {
     if (grid.z > 65535 || grid.y > 65535) return -3;
     const int n_kv = (p.skv + ts - 1) / ts;
     const size_t smem = static_cast<size_t>(ts) * 128 * (n_kv > 1 ? 5 : 3);
-    if (small) launch_pdl(attention_kernel<32>, grid, 64, smem, stream, p);
-    else launch_pdl(attention_kernel<64>, grid, 128, smem, stream, p);
+    if (small) attention_kernel<32><<<grid, 64, smem, stream>>>(p);
+    else attention_kernel<64><<<grid, 128, smem, stream>>>(p);
     return launch_status("attention launch");
 }
 

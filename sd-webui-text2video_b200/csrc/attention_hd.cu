@@ -55,8 +55,6 @@ __device__ __forceinline__ void load_rows(uint32_t smem_tile, const __half* gbas
 // ------------------------------------------------------------------------------------------------ flash attention, any HD
 template <int HD>
 __global__ void __launch_bounds__(128) attention_hd_kernel(AttnParams p) {
-    griddep_wait();
-    griddep_launch_small();
     using G = Geo<HD>;
     constexpr int TS = 64, NB = TS / 8, KSK = TS / 16, TB = TS * G::PB;
     extern __shared__ __align__(128) uint8_t smem_dyn[];
@@ -224,8 +222,6 @@ struct RelSmem {
 
 template <int HD, int RT>
 __global__ void __launch_bounds__(RP_WARPS * 32) attention_relpos_kernel(RelposParams p) {
-    griddep_wait();
-    griddep_launch_small();
     using G = Geo<HD>;
     using SM = RelSmem<HD, RT>;
     constexpr int NBK = RT / 8;        // 8-wide key blocks
@@ -448,7 +444,7 @@ int launch_hd(const AttnParams& p, cudaStream_t stream) {
     }
     dim3 grid(p.batch, p.heads, (p.sq + 63) / 64);
     if (grid.z > 65535 || grid.y > 65535) return -3;
-    launch_pdl(attention_hd_kernel<HD>, grid, 128, smem, stream, p);
+    attention_hd_kernel<HD><<<grid, 128, smem, stream>>>(p);
     return launch_status("attention_hd launch");
 }
 
@@ -464,7 +460,7 @@ int launch_relpos_rt(const RelposParams& p, cudaStream_t stream) {
     const long long items = static_cast<long long>(p.n_seq) * p.heads;
     const long long want = (items + RP_WARPS - 1) / RP_WARPS;
     const unsigned grid = static_cast<unsigned>(std::min<long long>(want, static_cast<long long>(num_sms()) * 2));
-    launch_pdl(attention_relpos_kernel<HD, RT>, grid, RP_WARPS * 32, SM::kTotal, stream, p);
+    attention_relpos_kernel<HD, RT><<<grid, RP_WARPS * 32, SM::kTotal, stream>>>(p);
     return launch_status("attention_hd launch");
 }
 template <int HD>

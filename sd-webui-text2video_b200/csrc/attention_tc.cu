@@ -84,7 +84,6 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         fence_barrier_init();
     }
     __syncthreads();
-    griddep_wait();        // the prologue above overlaps the previous kernel's tail (PDL, common.cuh)
 
     if (wg == 0) {
         // ------------------------------------------------------------------ TMA producer
@@ -103,7 +102,6 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
                 tma_load_3d(smem + SMEM_K + s * TILE_BYTES, &map_k, &kv_full[s], head * HD, j * BKV, bkv);
                 tma_load_3d(smem + SMEM_V + s * TILE_BYTES, &map_v, &kv_full[s], head * HD, j * BKV, bkv);
             }
-            griddep_launch();          // all loads issued: dependents may be scheduled as SMs drain
         }
         __syncwarp();
     } else {
@@ -277,7 +275,7 @@ int attention_tc_launch(const AttnTcPlan& pl, cudaStream_t stream) {
     a.n_kv = (pl.skv + BKV - 1) / BKV;
     a.sl2 = pl.sl2;
     dim3 grid((pl.sq + BQ - 1) / BQ, pl.heads, pl.batch);
-    launch_pdl(attention_tc_kernel, grid, NTHREADS, SMEM_TOTAL, stream, pl.map_q, pl.map_k, pl.map_v, a);
+    attention_tc_kernel<<<grid, NTHREADS, SMEM_TOTAL, stream>>>(pl.map_q, pl.map_k, pl.map_v, a);
     return launch_status("attention_tc launch");
 }
 

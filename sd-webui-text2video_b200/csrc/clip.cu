@@ -46,8 +46,6 @@ namespace {
 // x[b, l, :] = token_embedding[tokens[b, l], :] + positional_embedding[l, :]
 __global__ void clip_embed_kernel(const int* __restrict__ tokens, const __half* __restrict__ emb, const __half* __restrict__ pos,
                                   __half* __restrict__ x, int rows, int L, int W, int vocab) {
-    griddep_wait();
-    griddep_launch_small();
     const int W8 = W >> 3;
     const long long n = static_cast<long long>(rows) * W8;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -71,8 +69,6 @@ __global__ void clip_embed_kernel(const int* __restrict__ tokens, const __half* 
 
 // y = x * Phi(x) (nn.GELU, erf form), in place on [rows, C] fp16
 __global__ void gelu_kernel(__half* __restrict__ x, long long n8) {
-    griddep_wait();
-    griddep_launch_small();
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n8; i += static_cast<long long>(gridDim.x) * blockDim.x) {
         uint4 v = reinterpret_cast<uint4*>(x)[i];
         __half2* h = reinterpret_cast<__half2*>(&v);
@@ -88,8 +84,6 @@ __global__ void gelu_kernel(__half* __restrict__ x, long long n8) {
 
 // y = x * sigmoid(1.702 x) (transformers' quick_gelu, CLIP ViT-L/14), in place on [rows, C] fp16; fp32 math, one rounding
 __global__ void quick_gelu_kernel(__half* __restrict__ x, long long n8) {
-    griddep_wait();
-    griddep_launch_small();
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n8; i += static_cast<long long>(gridDim.x) * blockDim.x) {
         uint4 v = reinterpret_cast<uint4*>(x)[i];
         __half2* h = reinterpret_cast<__half2*>(&v);
@@ -108,8 +102,6 @@ __global__ void quick_gelu_kernel(__half* __restrict__ x, long long n8) {
 // one warp per query row; lanes own keys l, l+32, ... for the scores and output channels l, l+32 for P V.
 constexpr int kClipD = 64;
 __global__ void __launch_bounds__(128) clip_attention_kernel(const __half* __restrict__ qkv, __half* __restrict__ o, int L, int W, int heads) {
-    griddep_wait();
-    griddep_launch_small();
     extern __shared__ __half sm_kv[];
     const int b = blockIdx.x / heads, hd = blockIdx.x % heads;
     __half* sk = sm_kv;                         // [L][66]
@@ -248,8 +240,8 @@ int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
         const Tok xx = x;
         const int vocab = cfg.vocab;
         bld.step([=](cudaStream_t s) {
-            launch_pdl(clip_embed_kernel, dim3(static_cast<unsigned>((R * (W / 8) + 255) / 256)), dim3(256), 0, s, tokens, emb, pos, xx.p,
-                       static_cast<int>(R), L, W, vocab);
+            clip_embed_kernel<<<dim3(static_cast<unsigned>((R * (W / 8) + 255) / 256)), dim3(256), 0, s>>>(tokens, emb, pos, xx.p,
+                                                                                                           static_cast<int>(R), L, W, vocab);
             return launch_status("clip launch");
         }, 1, STEP_OTHER, 0.0, "clip embed");
     }
@@ -276,7 +268,7 @@ int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
             const Tok q = qkv, oo = o;
             const size_t smem = static_cast<size_t>(2) * L * 66 * sizeof(__half);
             bld.step([=](cudaStream_t s) {
-                launch_pdl(clip_attention_kernel, dim3(static_cast<unsigned>(B * heads)), dim3(128), smem, s, q.p, oo.p, L, W, heads);
+                clip_attention_kernel<<<dim3(static_cast<unsigned>(B * heads)), dim3(128), smem, s>>>(q.p, oo.p, L, W, heads);
                 return launch_status("clip launch");
             }, 1, STEP_ATTN, 4.0 * B * heads * static_cast<double>(L) * L * kClipD / 2, "clip causal attention");
         }
@@ -291,7 +283,7 @@ int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
             const Tok hh = h;
             const long long n8 = R * (4 * W) / 8;
             bld.step([=](cudaStream_t s) {
-                launch_pdl(act, dim3(static_cast<unsigned>((n8 + 255) / 256)), dim3(256), 0, s, hh.p, n8);
+                act<<<dim3(static_cast<unsigned>((n8 + 255) / 256)), dim3(256), 0, s>>>(hh.p, n8);
                 return launch_status("clip launch");
             }, 1, STEP_OTHER, 0.0, act_label);
         }

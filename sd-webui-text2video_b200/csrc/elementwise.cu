@@ -23,8 +23,6 @@ inline int grid_for(long long n, int threads, int cap = 132 * 16) {
 // frames [frame0, frame0 + nframes) of the (b f) order of x [B, C, F, h, w] -> tok rows [nframes * h * w][ld]
 __global__ void ingest_kernel(const void* x, int x_is_f32, __half* tok, long long ld, int cpad, int C, int F, int h, int w,
                               long long frame0, long long nframes, float scale) {
-    griddep_wait();
-    griddep_launch_small();
     const long long P = static_cast<long long>(h) * w;
     const long long rows = nframes * P;
     GRID_STRIDE(i, rows * cpad) {
@@ -46,8 +44,6 @@ __global__ void ingest_kernel(const void* x, int x_is_f32, __half* tok, long lon
 
 __global__ void egress_kernel(const __half* tok, long long ld, void* out, int out_is_f32, int B, int C, int F, int h,
                               int w) {
-    griddep_wait();
-    griddep_launch_small();
     const long long P = static_cast<long long>(h) * w;
     const long long n = static_cast<long long>(B) * C * F * P;
     GRID_STRIDE(i, n) {
@@ -64,8 +60,6 @@ __global__ void egress_kernel(const __half* tok, long long ld, void* out, int ou
 }
 
 __global__ void upsample2x_kernel(const uint4* x, uint4* y, long long nframes, int h, int w, int C8) {
-    griddep_wait();
-    griddep_launch_small();
     const int H = 2 * h, W = 2 * w;
     const long long n = nframes * H * W * C8;
     GRID_STRIDE(i, n) {
@@ -80,8 +74,6 @@ __global__ void upsample2x_kernel(const uint4* x, uint4* y, long long nframes, i
 }
 
 __global__ void im2col_s2_kernel(const uint4* x, uint4* col, long long nframes, int h, int w, int C8, int pad_lo) {
-    griddep_wait();
-    griddep_launch_small();
     // pad_lo = 1: symmetric padding 1 (Conv2d stride 2 padding 1); pad_lo = 0: the ldm Downsample's pad (0,1,0,1) + padding 0
     const int ho = pad_lo ? (h + 1) / 2 : h / 2, wo = pad_lo ? (w + 1) / 2 : w / 2;
     const long long n = nframes * ho * wo * 9 * C8;
@@ -104,8 +96,6 @@ __global__ void im2col_s2_kernel(const uint4* x, uint4* col, long long nframes, 
 
 __global__ void concat_kernel(const __half* a, long long lda, int Ca8, const __half* b, long long ldb, int Cb8,
                               __half* out, long long ldo, long long rows) {
-    griddep_wait();
-    griddep_launch_small();
     const int T8 = Ca8 + Cb8;
     GRID_STRIDE(i, rows * T8) {
         const long long r = i / T8;
@@ -118,8 +108,6 @@ __global__ void concat_kernel(const __half* a, long long lda, int Ca8, const __h
 }
 
 __global__ void time_sinusoid_kernel(const float* t, __half* out, int B, int dim) {
-    griddep_wait();
-    griddep_launch_small();
     const int half_dim = dim / 2;
     GRID_STRIDE(i, static_cast<long long>(B) * dim) {
         const int b = static_cast<int>(i / dim);
@@ -140,8 +128,6 @@ __global__ void time_sinusoid_kernel(const float* t, __half* out, int B, int dim
 __global__ void __launch_bounds__(256) small_linear_kernel(const __half* x, long long ldx, const __half* W,
                                                            const __half* bias, const __half* addend, __half* y,
                                                            long long ldy, int B, int N, int K, int silu_in) {
-    griddep_wait();
-    griddep_launch_small();
     const int lane = threadIdx.x & 31;
     const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (n >= N) return;
@@ -173,8 +159,6 @@ __global__ void __launch_bounds__(256) small_linear_kernel(const __half* x, long
 
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const __half* x, __half* y, long long rows, int cols,
                                                            float scale) {
-    griddep_wait();
-    griddep_launch_small();
     // one warp per row, fp32 math; the scaled logits are rounded to fp16 first (reference: w_ * c^-0.5 in fp16)
     const int lane = threadIdx.x & 31;
     const long long row = blockIdx.x * static_cast<long long>(blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -195,8 +179,6 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const __half* x, __ha
 }
 
 __global__ void transpose_kernel(const __half* x, __half* y, int R, int C) {
-    griddep_wait();
-    griddep_launch_small();
     __shared__ __half tile[32][34];
     const long long base = static_cast<long long>(blockIdx.z) * R * C;
     const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
@@ -212,8 +194,6 @@ __global__ void transpose_kernel(const __half* x, __half* y, int R, int C) {
 }
 
 __global__ void frames_to_u8_kernel(const __half* tok, long long ld, uint8_t* out, long long pixels) {
-    griddep_wait();
-    griddep_launch_small();
     GRID_STRIDE(i, pixels * 3) {
         const long long p = i / 3;
         const int c = static_cast<int>(i - p * 3);
@@ -228,8 +208,6 @@ __global__ void frames_to_u8_kernel(const __half* tok, long long ld, uint8_t* ou
 // nn.PixelUnshuffle(8) of NCHW frames straight into tokens: row (n, y, x), column c*64 + i*8 + j = x[n, c, 8y+i, 8x+j].
 // One thread per 8 consecutive columns (a fixed (c, i), j = 0..7): eight contiguous source pixels, one 16-byte store.
 __global__ void pixel_unshuffle_kernel(const void* x, int x_is_f32, __half* tok, int N, int Cc, int H, int W) {
-    griddep_wait();
-    griddep_launch_small();
     const int h8 = H / 8, w8 = W / 8;
     const int groups = Cc * 8;                  // 8-column groups per row
     const long long n = static_cast<long long>(N) * h8 * w8 * groups;
@@ -253,8 +231,6 @@ __global__ void pixel_unshuffle_kernel(const void* x, int x_is_f32, __half* tok,
 
 // y = max(x, 0) in place on a token matrix (n8 16-byte vectors)
 __global__ void relu_kernel(uint4* x, long long n8) {
-    griddep_wait();
-    griddep_launch_small();
     const __half2 z = __float2half2_rn(0.f);
     GRID_STRIDE(i, n8) {
         uint4 v = x[i];
@@ -268,8 +244,6 @@ __global__ void relu_kernel(uint4* x, long long n8) {
 // 2x2 average pooling, stride 2, floor sizes (nn.AvgPool2d(2, 2)): x [n, h, w, C] -> y [n, h/2, w/2, C]; fp32 sum of the four
 // taps, times 0.25, one fp16 rounding
 __global__ void avgpool2x2_kernel(const uint4* x, uint4* y, long long nframes, int h, int w, int C8) {
-    griddep_wait();
-    griddep_launch_small();
     const int ho = h / 2, wo = w / 2;
     GRID_STRIDE(i, nframes * ho * wo * C8) {
         const int c = static_cast<int>(i % C8);
@@ -301,8 +275,6 @@ __global__ void avgpool2x2_kernel(const uint4* x, uint4* y, long long nframes, i
 // x[r, :] += f[(r / rows_per_sample % f_samples) * rows_per_sample + r % rows_per_sample, :]  in place; fp32 add, one rounding
 __global__ void feature_add_kernel(__half* x, long long ldx, const __half* f, int C8, long long rows, long long rows_per_sample,
                                    int f_samples) {
-    griddep_wait();
-    griddep_launch_small();
     GRID_STRIDE(i, rows * C8) {
         const long long r = i / C8;
         const int c = static_cast<int>(i - r * C8);
@@ -323,8 +295,6 @@ __global__ void feature_add_kernel(__half* x, long long ldx, const __half* f, in
 }
 
 __global__ void frames_to_f32_kernel(const __half* tok, long long ld, float* out, int n, int H, int W) {
-    griddep_wait();
-    griddep_launch_small();
     const long long P = static_cast<long long>(H) * W;
     GRID_STRIDE(i, static_cast<long long>(n) * 3 * P) {
         const long long p = i % P;
@@ -337,8 +307,6 @@ __global__ void frames_to_f32_kernel(const __half* tok, long long ld, float* out
 
 __global__ void pack_conv_kernel(const void* src, int src_is_f32, __half* dst, int Cout, int Cin, int taps, int n_alloc,
                                  int k_alloc) {
-    griddep_wait();
-    griddep_launch_small();
     const long long n = static_cast<long long>(taps) * n_alloc * k_alloc;
     GRID_STRIDE(i, n) {
         const int k = static_cast<int>(i % k_alloc);
@@ -356,8 +324,6 @@ __global__ void pack_conv_kernel(const void* src, int src_is_f32, __half* dst, i
 
 __global__ void pack_geglu_kernel(const void* w, const void* b, int src_is_f32, __half* wdst, __half* bdst, int H, int K,
                                   int bn) {
-    griddep_wait();
-    griddep_launch_small();
     // packed row p: tile = p / bn, j = p % bn ; j < bn/2 -> value channel tile*bn/2 + j ; else gate channel H + tile*bn/2 + (j - bn/2)
     const long long n = static_cast<long long>(2) * H * K;
     const int hb = bn / 2;
@@ -378,8 +344,6 @@ __global__ void pack_geglu_kernel(const void* w, const void* b, int src_is_f32, 
 __global__ void splitk_reduce_kernel(const float* part, int splits, long long split_stride, long long rows, int N8,
                                      const __half* bias, int bias_rows, long long bias_stride, const __half* residual,
                                      long long ldr, __half* out, long long ldo) {
-    griddep_wait();
-    griddep_launch_small();
     GRID_STRIDE(i, rows * N8) {
         const long long r = i / N8;
         const int c = static_cast<int>(i - r * N8) * 8;
@@ -416,8 +380,6 @@ __global__ void splitk_reduce_kernel(const float* part, int splits, long long sp
 // one warp per output row n
 __global__ void __launch_bounds__(256) fold_ln_kernel(const __half* w, const __half* bias, const __half* gamma, const __half* beta,
                                                       __half* wout, float* colsum, float* bias32, int N, int K) {
-    griddep_wait();
-    griddep_launch_small();
     const int lane = threadIdx.x & 31;
     const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (n >= N) return;
@@ -441,8 +403,6 @@ __global__ void __launch_bounds__(256) fold_ln_kernel(const __half* w, const __h
 }
 
 __global__ void convert_kernel(const void* src, int src_is_f32, __half* dst, long long n) {
-    griddep_wait();
-    griddep_launch_small();
     GRID_STRIDE(i, n) {
         dst[i] = src_is_f32 ? __float2half_rn(reinterpret_cast<const float*>(src)[i]) : reinterpret_cast<const __half*>(src)[i];
     }
@@ -463,8 +423,6 @@ __device__ __forceinline__ float load_eps(const void* p, long long i, int is_f32
 }
 
 __global__ void ddim_step_kernel(DdimStepParams p) {
-    griddep_wait();
-    griddep_launch_small();
     GRID_STRIDE(i, p.n) {
         const int ch = static_cast<int>((i / p.chan_stride) % p.C);
         const float c = load_eps(p.eps_c, i, p.eps_is_f32);
@@ -492,8 +450,6 @@ struct LincombArgs {
     int n_src;
 };
 __global__ void lincomb_kernel(float* out, LincombArgs a, long long n) {
-    griddep_wait();
-    griddep_launch_small();
     GRID_STRIDE(i, n) {
         float acc = 0.f;
         for (int s = 0; s < a.n_src; ++s) acc = fmaf(a.coef[s], a.src[s][i], acc);
@@ -503,8 +459,6 @@ __global__ void lincomb_kernel(float* out, LincombArgs a, long long n) {
 
 __global__ void cfg_x0_kernel(const float* x, const void* ec, const void* eu, int eps_f32, float* x0, long long n, float g,
                               float alpha, float sigma, int fp16) {
-    griddep_wait();
-    griddep_launch_small();
     GRID_STRIDE(i, n) {
         float e = load_eps(ec, i, eps_f32);
         if (eu != nullptr) e = cfg_combine(e, load_eps(eu, i, eps_f32), g, fp16);
@@ -517,8 +471,6 @@ __global__ void cfg_x0_kernel(const float* x, const void* ec, const void* eu, in
 __global__ void latent_blend_kernel(const float* __restrict__ img, int img_frames, const double* __restrict__ noise,
                                     const double* __restrict__ w, double* __restrict__ out, double* __restrict__ mask, long long n,
                                     int F, long long hw) {
-    griddep_wait();
-    griddep_launch_small();
     GRID_STRIDE(i, n) {
         const long long bc = i / (static_cast<long long>(F) * hw);
         const long long r = i - bc * F * hw;
@@ -535,8 +487,6 @@ __global__ void latent_blend_kernel(const float* __restrict__ img, int img_frame
 // torch's fp32 op order, no contraction: known = a[b]*x0 + s[b]*noise; out = known*mask + (1 - mask)*img when blending.
 // x0 / noise / mask are read through element strides (0 on a broadcast dimension); img and out are contiguous.
 __global__ void q_sample_blend_kernel(QSampleBlendParams p) {
-    griddep_wait();
-    griddep_launch_small();
     const long long hw = static_cast<long long>(p.shape[3]) * p.shape[4];
     const long long n = static_cast<long long>(p.shape[0]) * p.shape[1] * p.shape[2] * hw;
     GRID_STRIDE(i, n) {
@@ -570,8 +520,6 @@ __global__ void q_sample_blend_kernel(QSampleBlendParams p) {
 // accumulation and rounded to fp16 (torch's autocast matmul), scaled by alpha in fp16, added in fp16.
 __global__ void lora_merge_kernel(__half* __restrict__ w, const __half* __restrict__ A, const __half* __restrict__ B, int out, int cols,
                                   int rank, float alpha, int temporal_mean) {
-    griddep_wait();
-    griddep_launch_small();
     const long long n = static_cast<long long>(out) * cols;
     const int a_cols = temporal_mean ? cols * 3 : cols;
     GRID_STRIDE(i, n) {
@@ -607,8 +555,6 @@ __device__ __forceinline__ float widen(__half v) { return __half2float(v); }
 template <class T>
 __global__ void lora_apply_kernel(__half* __restrict__ w, const T* __restrict__ up, const T* __restrict__ down, int out, int cols,
                                   int rank, float alpha) {
-    griddep_wait();
-    griddep_launch_small();
     const long long n = static_cast<long long>(out) * cols;
     GRID_STRIDE(i, n) {
         const int o = static_cast<int>(i / cols);
@@ -631,120 +577,120 @@ int ingest_latent(const void* x, int x_is_f32, __half* tok, long long ld, int cp
 int ingest_latent_frames(const void* x, int x_is_f32, __half* tok, long long ld, int cpad, int C, int F, int h, int w,
                          long long frame0, long long nframes, float scale, cudaStream_t stream) {
     const long long n = nframes * h * w * cpad;
-    launch_pdl(ingest_kernel, grid_for(n, 256), 256, 0, stream, x, x_is_f32, tok, ld, cpad, C, F, h, w, frame0, nframes, scale);
+    ingest_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, x_is_f32, tok, ld, cpad, C, F, h, w, frame0, nframes, scale);
     return ok();
 }
 int egress_latent(const __half* tok, long long ld, void* out, int out_is_f32, int B, int C, int F, int h, int w,
                   cudaStream_t stream) {
     const long long n = static_cast<long long>(B) * C * F * h * w;
-    launch_pdl(egress_kernel, grid_for(n, 256), 256, 0, stream, tok, ld, out, out_is_f32, B, C, F, h, w);
+    egress_kernel<<<grid_for(n, 256), 256, 0, stream>>>(tok, ld, out, out_is_f32, B, C, F, h, w);
     return ok();
 }
 int upsample2x(const __half* x, __half* y, int nframes, int h, int w, int C, cudaStream_t stream) {
     if (C % 8) return -1;
     const long long n = static_cast<long long>(nframes) * 4 * h * w * (C / 8);
-    launch_pdl(upsample2x_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y),
+    upsample2x_kernel<<<grid_for(n, 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y),
                                                             nframes, h, w, C / 8);
     return ok();
 }
 int im2col_s2(const __half* x, __half* col, int nframes, int h, int w, int C, cudaStream_t stream, int pad_lo) {
     if (C % 8) return -1;
     const long long n = static_cast<long long>(nframes) * ((pad_lo ? (h + 1) / 2 : h / 2)) * ((pad_lo ? (w + 1) / 2 : w / 2)) * 9 * (C / 8);
-    launch_pdl(im2col_s2_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(col),
+    im2col_s2_kernel<<<grid_for(n, 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(col),
                                                            nframes, h, w, C / 8, pad_lo);
     return ok();
 }
 int pixel_unshuffle_ingest(const void* x, int x_is_f32, __half* tok, int N, int Cc, int H, int W, cudaStream_t stream) {
     if (H % 8 || W % 8) return -1;
     const long long n = static_cast<long long>(N) * (H / 8) * (W / 8) * Cc * 8;
-    launch_pdl(pixel_unshuffle_kernel, grid_for(n, 256), 256, 0, stream, x, x_is_f32, tok, N, Cc, H, W);
+    pixel_unshuffle_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, x_is_f32, tok, N, Cc, H, W);
     return ok();
 }
 int relu_inplace(__half* x, long long rows, int C, cudaStream_t stream) {
     if (C % 8) return -1;
     const long long n8 = rows * (C / 8);
-    launch_pdl(relu_kernel, grid_for(n8, 256), 256, 0, stream, reinterpret_cast<uint4*>(x), n8);
+    relu_kernel<<<grid_for(n8, 256), 256, 0, stream>>>(reinterpret_cast<uint4*>(x), n8);
     return ok();
 }
 int avgpool2x2(const __half* x, __half* y, int nframes, int h, int w, int C, cudaStream_t stream) {
     if (C % 8) return -1;
     const long long n = static_cast<long long>(nframes) * (h / 2) * (w / 2) * (C / 8);
-    launch_pdl(avgpool2x2_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y),
-               nframes, h, w, C / 8);
+    avgpool2x2_kernel<<<grid_for(n, 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y),
+                                                            nframes, h, w, C / 8);
     return ok();
 }
 int feature_add(__half* x, long long ldx, const __half* f, int C, long long rows, long long rows_per_sample, int f_samples,
                 cudaStream_t stream) {
     if (C % 8 || ldx % 8 || rows_per_sample < 1 || f_samples < 1) return -1;
     const long long n = rows * (C / 8);
-    launch_pdl(feature_add_kernel, grid_for(n, 256), 256, 0, stream, x, ldx, f, C / 8, rows, rows_per_sample, f_samples);
+    feature_add_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, ldx, f, C / 8, rows, rows_per_sample, f_samples);
     return ok();
 }
 int concat_cols(const __half* a, long long lda, int Ca, const __half* b, long long ldb, int Cb, __half* out,
                 long long ldo, long long rows, cudaStream_t stream) {
     if ((Ca % 8) || (Cb % 8) || (lda % 8) || (ldb % 8) || (ldo % 8)) return -1;
     const long long n = rows * ((Ca + Cb) / 8);
-    launch_pdl(concat_kernel, grid_for(n, 256), 256, 0, stream, a, lda, Ca / 8, b, ldb, Cb / 8, out, ldo, rows);
+    concat_kernel<<<grid_for(n, 256), 256, 0, stream>>>(a, lda, Ca / 8, b, ldb, Cb / 8, out, ldo, rows);
     return ok();
 }
 int time_sinusoid(const float* t, __half* out, int B, int dim, cudaStream_t stream) {
-    launch_pdl(time_sinusoid_kernel, grid_for(static_cast<long long>(B) * dim, 256), 256, 0, stream, t, out, B, dim);
+    time_sinusoid_kernel<<<grid_for(static_cast<long long>(B) * dim, 256), 256, 0, stream>>>(t, out, B, dim);
     return ok();
 }
 int small_linear(const __half* x, long long ldx, const __half* W, const __half* bias, const __half* addend, __half* y,
                  long long ldy, int B, int N, int K, int silu_in, cudaStream_t stream) {
     if ((K % 8) || (ldx % 8)) return -1;
-    launch_pdl(small_linear_kernel, (N + 7) / 8, 256, 0, stream, x, ldx, W, bias, addend, y, ldy, B, N, K, silu_in);
+    small_linear_kernel<<<(N + 7) / 8, 256, 0, stream>>>(x, ldx, W, bias, addend, y, ldy, B, N, K, silu_in);
     return ok();
 }
 int softmax_rows(const __half* x, __half* y, long long rows, int cols, float scale, cudaStream_t stream) {
-    launch_pdl(softmax_rows_kernel, static_cast<unsigned int>((rows + 7) / 8), 256, 0, stream, x, y, rows, cols, scale);
+    softmax_rows_kernel<<<static_cast<unsigned int>((rows + 7) / 8), 256, 0, stream>>>(x, y, rows, cols, scale);
     return ok();
 }
 int transpose_batched(const __half* x, __half* y, int nb, int R, int C, cudaStream_t stream) {
     dim3 grid((C + 31) / 32, (R + 31) / 32, nb);
-    launch_pdl(transpose_kernel, grid, dim3(32, 8), 0, stream, x, y, R, C);
+    transpose_kernel<<<grid, dim3(32, 8), 0, stream>>>(x, y, R, C);
     return ok();
 }
 int frames_to_u8(const __half* tok, long long ld, uint8_t* out, long long pixels, cudaStream_t stream) {
-    launch_pdl(frames_to_u8_kernel, grid_for(pixels * 3, 256), 256, 0, stream, tok, ld, out, pixels);
+    frames_to_u8_kernel<<<grid_for(pixels * 3, 256), 256, 0, stream>>>(tok, ld, out, pixels);
     return ok();
 }
 int frames_to_f32_nchw(const __half* tok, long long ld, float* out, int n, int H, int W, cudaStream_t stream) {
-    launch_pdl(frames_to_f32_kernel, grid_for(static_cast<long long>(n) * 3 * H * W, 256), 256, 0, stream, tok, ld, out, n, H, W);
+    frames_to_f32_kernel<<<grid_for(static_cast<long long>(n) * 3 * H * W, 256), 256, 0, stream>>>(tok, ld, out, n, H, W);
     return ok();
 }
 int pack_conv_weight(const void* src, int src_is_f32, __half* dst, int Cout, int Cin, int taps, int n_alloc, int k_alloc,
                      cudaStream_t stream) {
     const long long n = static_cast<long long>(taps) * n_alloc * k_alloc;
-    launch_pdl(pack_conv_kernel, grid_for(n, 256), 256, 0, stream, src, src_is_f32, dst, Cout, Cin, taps, n_alloc, k_alloc);
+    pack_conv_kernel<<<grid_for(n, 256), 256, 0, stream>>>(src, src_is_f32, dst, Cout, Cin, taps, n_alloc, k_alloc);
     return ok();
 }
 int pack_geglu_weight(const void* w, const void* b, int src_is_f32, __half* wdst, __half* bdst, int H, int K, int bn,
                       cudaStream_t stream) {
     if ((2 * H) % bn) return -1;
-    launch_pdl(pack_geglu_kernel, grid_for(static_cast<long long>(2) * H * K, 256), 256, 0, stream, w, b, src_is_f32, wdst, bdst, H, K, bn);
+    pack_geglu_kernel<<<grid_for(static_cast<long long>(2) * H * K, 256), 256, 0, stream>>>(w, b, src_is_f32, wdst, bdst, H, K, bn);
     return ok();
 }
 int splitk_reduce(const float* part, int splits, long long split_stride, long long rows, int N, const __half* bias,
                   int bias_rows, long long bias_stride, const __half* residual, long long ldr, __half* out, long long ldo,
                   cudaStream_t stream) {
     if ((N & 7) || (ldo & 7) || (residual && (ldr & 7)) || (bias && (bias_stride & 7))) return -1;
-    launch_pdl(splitk_reduce_kernel, grid_for(rows * (N / 8), 256), 256, 0, stream, part, splits, split_stride, rows, N / 8, bias,
+    splitk_reduce_kernel<<<grid_for(rows * (N / 8), 256), 256, 0, stream>>>(part, splits, split_stride, rows, N / 8, bias,
                                                                             bias_rows, bias_stride, residual, ldr, out, ldo);
     return ok();
 }
 int fold_ln_into_linear(const __half* w, const __half* bias, const __half* gamma, const __half* beta, __half* wout,
                         float* colsum, float* bias32, int N, int K, cudaStream_t stream) {
-    launch_pdl(fold_ln_kernel, (N + 7) / 8, 256, 0, stream, w, bias, gamma, beta, wout, colsum, bias32, N, K);
+    fold_ln_kernel<<<(N + 7) / 8, 256, 0, stream>>>(w, bias, gamma, beta, wout, colsum, bias32, N, K);
     return ok();
 }
 int convert_to_f16(const void* src, int src_is_f32, __half* dst, long long n, cudaStream_t stream) {
-    launch_pdl(convert_kernel, grid_for(n, 256), 256, 0, stream, src, src_is_f32, dst, n);
+    convert_kernel<<<grid_for(n, 256), 256, 0, stream>>>(src, src_is_f32, dst, n);
     return ok();
 }
 int ddim_step(const DdimStepParams& p, cudaStream_t stream) {
-    launch_pdl(ddim_step_kernel, grid_for(p.n, 256), 256, 0, stream, p);
+    ddim_step_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p);
     return ok();
 }
 int lincomb(float* out, const float* const* src, const float* coef, int n_src, long long n, cudaStream_t stream) {
@@ -755,43 +701,43 @@ int lincomb(float* out, const float* const* src, const float* coef, int n_src, l
         a.coef[i] = coef[i];
     }
     a.n_src = n_src;
-    launch_pdl(lincomb_kernel, grid_for(n, 256), 256, 0, stream, out, a, n);
+    lincomb_kernel<<<grid_for(n, 256), 256, 0, stream>>>(out, a, n);
     return ok();
 }
 int lora_merge_weight(__half* w, const __half* A, const __half* B, int out, int cols, int rank, float alpha, int temporal_mean,
                       cudaStream_t stream) {
     const long long n = static_cast<long long>(out) * cols;
-    launch_pdl(lora_merge_kernel, grid_for(n, 256), 256, 0, stream, w, A, B, out, cols, rank, alpha, temporal_mean);
+    lora_merge_kernel<<<grid_for(n, 256), 256, 0, stream>>>(w, A, B, out, cols, rank, alpha, temporal_mean);
     return ok();
 }
 int lora_apply_weight(__half* w, const void* up, const void* down, int dtype, int out, int cols, int rank, float alpha,
                       cudaStream_t stream) {
     const long long n = static_cast<long long>(out) * cols;
     if (dtype == 1)
-        launch_pdl(lora_apply_kernel<float>, grid_for(n, 256), 256, 0, stream, w, static_cast<const float*>(up),
-                   static_cast<const float*>(down), out, cols, rank, alpha);
+        lora_apply_kernel<float><<<grid_for(n, 256), 256, 0, stream>>>(w, static_cast<const float*>(up),
+                                                                       static_cast<const float*>(down), out, cols, rank, alpha);
     else
-        launch_pdl(lora_apply_kernel<__half>, grid_for(n, 256), 256, 0, stream, w, static_cast<const __half*>(up),
-                   static_cast<const __half*>(down), out, cols, rank, alpha);
+        lora_apply_kernel<__half><<<grid_for(n, 256), 256, 0, stream>>>(w, static_cast<const __half*>(up),
+                                                                        static_cast<const __half*>(down), out, cols, rank, alpha);
     return ok();
 }
 
 int latent_blend(const float* img, int img_frames, const double* noise, const double* w, double* out, double* mask, int BC, int F,
                  long long hw, cudaStream_t stream) {
     const long long n = static_cast<long long>(BC) * F * hw;
-    launch_pdl(latent_blend_kernel, grid_for(n, 256), 256, 0, stream, img, img_frames, noise, w, out, mask, n, F, hw);
+    latent_blend_kernel<<<grid_for(n, 256), 256, 0, stream>>>(img, img_frames, noise, w, out, mask, n, F, hw);
     return ok();
 }
 
 int q_sample_blend(const QSampleBlendParams& p, cudaStream_t stream) {
     const long long n = static_cast<long long>(p.shape[0]) * p.shape[1] * p.shape[2] * p.shape[3] * p.shape[4];
-    launch_pdl(q_sample_blend_kernel, grid_for(n, 256), 256, 0, stream, p);
+    q_sample_blend_kernel<<<grid_for(n, 256), 256, 0, stream>>>(p);
     return ok();
 }
 
 int cfg_x0(const float* x, const void* eps_c, const void* eps_u, int eps_is_f32, float* x0, long long n, float g,
            float alpha, float sigma, int cfg_fp16, cudaStream_t stream) {
-    launch_pdl(cfg_x0_kernel, grid_for(n, 256), 256, 0, stream, x, eps_c, eps_u, eps_is_f32, x0, n, g, alpha, sigma, cfg_fp16);
+    cfg_x0_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, eps_c, eps_u, eps_is_f32, x0, n, g, alpha, sigma, cfg_fp16);
     return ok();
 }
 

@@ -418,7 +418,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     }
     if constexpr (CG == 2) cluster_sync_all();    // peer barriers are initialised before any multicast / remote arrive
     else __syncthreads();
-    griddep_wait();        // everything above is independent of the previous kernel's output (PDL, common.cuh)
 
     // work items: (pair of consecutive M-tiles, N-tile, K split); CTA `rank` of a cluster owns M-tile CG*pm + rank
     const int pairs_m = (g.tiles_m + CG - 1) / CG;
@@ -515,8 +514,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                     }
                 }
             }
-            // nothing left to fetch: let the next kernel's CTAs be scheduled as SMs drain (PDL)
-            griddep_launch();
         } else if (threadIdx.x >= 32 && threadIdx.x < 64 && col_operands) {
             // Warp 1: the per-column epilogue operands of each tile into `cols`, zero past N.  The consumers release the buffer
             // after step 1 of their epilogue, so the next tile's columns load during the rest of that epilogue and the next
@@ -910,8 +907,7 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
     // wide tiles, even slightly padded ones (N = 1920 -> 9 x 224 instead of 12 x 160), unless the epilogue is the longer leg.
     int bn = p.force_bn;
     const int k_total_sel = p.ntaps * g.k_chunks;
-    static const int model_min_k = getenv("T2V_BN_MODEL_MINK") ? atoi(getenv("T2V_BN_MODEL_MINK")) : 10;      // A/B switch
-    if (bn == 0 && k_total_sel >= model_min_k) {
+    if (bn == 0 && k_total_sel >= 10) {
         // K-heavy tiles (>= 10 K steps): the MMA leg dominates -> time model, padded wide tiles allowed.
         const int cands[7] = {256, 224, 192, 160, 128, 64, 16};
         double best = 1e30;
@@ -1072,22 +1068,13 @@ int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
     cfg.blockDim = dim3(static_cast<unsigned>(kThreads));
     cfg.dynamicSmemBytes = static_cast<size_t>(plan.smem);
     cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    unsigned na = 0;
-    if (plan.cg == 2) {
-        attr[na].id = cudaLaunchAttributeClusterDimension;
-        attr[na].val.clusterDim.x = 2;
-        attr[na].val.clusterDim.y = 1;
-        attr[na].val.clusterDim.z = 1;
-        ++na;
-    }
-    if (pdl_enabled()) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 2;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = plan.cg == 2 ? 1 : 0;
     void* args[1] = {const_cast<GemmDesc*>(&plan.desc)};
     return cudaLaunchKernelExC(&cfg, var->fn, args) == cudaSuccess ? 0 : -2;
 }

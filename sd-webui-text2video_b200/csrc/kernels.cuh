@@ -38,6 +38,8 @@ struct AttnParams {
     long long q_bsi, k_bsi, v_bsi, o_bsi;   // (temporal attention: outer = sample, inner = pixel); b_inner = 1 -> unused
     float scale;
 };
+// Picks the kernel for every caller: head_dim != 64 -> attention_hd; attention_tc when attention_tc_eligible; else the
+// warp-MMA kernel of attention.cu.
 int attention(const AttnParams& p, cudaStream_t stream);
 
 // attention_hd.cu: head dims other than 64 (VideoCrafter: C/8 = 40 / 80 / 160) and temporal attention with
@@ -60,7 +62,7 @@ struct RelposParams {
 int attention_relpos(const RelposParams& p, cudaStream_t stream);
 
 // attention_tc.cu: wgmma / TMA kernel for long self-attention sequences (sq >= 256, skv >= 128, one-level batch).
-// The plan holds the three tensor maps (encoded once per UNet plan, the launch itself is host-side free of driver calls).
+// The plan holds the three tensor maps; attention() encodes them before each launch (a captured graph replays them).
 struct AttnTcPlan {
     CUtensorMap map_q, map_k, map_v;   // rank 3: (heads*64, sequence, batch)
     __half* o;

@@ -6,7 +6,6 @@
 // fp32 math throughout (the reference runs group_norm / layer_norm / SiLU-after-norm in fp32 under autocast and
 // rounds to fp16 only when the value enters the next conv/linear -- exactly where these kernels round).
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 
 #include "common.cuh"
@@ -45,8 +44,6 @@ __global__ void __launch_bounds__(kNormThreads) gn_stats_kernel(const __half* __
                                                                 float eps, float2* __restrict__ partial,
                                                                 unsigned int* __restrict__ counters,
                                                                 float2* __restrict__ stats, const GnShard gs) {
-    griddep_wait();
-    griddep_launch_small();
     extern __shared__ float sm[];          // red[2][RL][C] | s_sum[C] | s_sq[C]
     __shared__ bool is_last;
     const int inst = blockIdx.y;
@@ -229,8 +226,6 @@ __global__ void __launch_bounds__(kNormThreads) gn_apply_kernel(const __half* __
                                                                 const float2* __restrict__ stats,
                                                                 const __half* __restrict__ gamma,
                                                                 const __half* __restrict__ beta) {
-    griddep_wait();
-    griddep_launch_small();
     const int inst = blockIdx.y;
     const int C8 = C >> 3;
     const int cpg = C / kGroups;
@@ -288,7 +283,6 @@ __global__ void __launch_bounds__(kNormThreads) gn_fused_kernel(const __half* __
                                                                 float2* __restrict__ partial, unsigned int* __restrict__ count,
                                                                 unsigned int* __restrict__ gen, const __half* __restrict__ gamma,
                                                                 const __half* __restrict__ beta, int cache) {
-    griddep_wait();
     extern __shared__ __align__(16) float sm[];   // red[2][RL][C] | s_sum[C] | s_sq[C] | fold[8][32][2] doubles | stats[32] float2 | slice
     const int inst = blockIdx.y;
     const int chunk = blockIdx.x;
@@ -429,7 +423,6 @@ __global__ void __launch_bounds__(kNormThreads) gn_fused_kernel(const __half* __
         st[threadIdx.x] = make_float2(static_cast<float>(mean), static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps))));
     }
     __syncthreads();
-    griddep_launch_small();
     if (!m.active) return;
     float a[8], b[8];
     {
@@ -473,8 +466,6 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
                                                         __half* __restrict__ y, long long ldy, long long rows, int C,
                                                         const __half* __restrict__ gamma,
                                                         const __half* __restrict__ beta, float eps) {
-    griddep_wait();
-    griddep_launch_small();
     const int lane = threadIdx.x & 31;
     const long long row = blockIdx.x * static_cast<long long>(blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= rows) return;
@@ -538,8 +529,6 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
 template <int NV>
 __global__ void __launch_bounds__(256) ln_rowstats_kernel(const __half* __restrict__ x, long long ldx, long long rows, int C,
                                                           float eps, float2* __restrict__ out) {
-    griddep_wait();
-    griddep_launch_small();
     const int lane = threadIdx.x & 31;
     const int C8 = C >> 3;
     const float inv_c = 1.0f / static_cast<float>(C);
@@ -647,8 +636,7 @@ int groupnorm_silu(const __half* x, long long ldx, __half* y, long long ldy, lon
     float2* stats = reinterpret_cast<float2*>(ws + kCounterBytes);
     float2* partial = stats + static_cast<size_t>(n_inst) * kGroups;
     // ---- single-launch path (phase 0, no cross-rank statistics): all CTAs of the grid must be co-resident
-    static const bool fused_on = getenv("T2V_NO_FUSED_GN") == nullptr;
-    if (phase == 0 && fused_on && (shard == nullptr || shard->peers.nranks <= 1) && n_inst <= 65536) {
+    if (phase == 0 && (shard == nullptr || shard->peers.nranks <= 1) && n_inst <= 65536) {
         const size_t inst_bytes = static_cast<size_t>(rows_per_inst) * C * sizeof(__half);
         const size_t fixed = stats_smem_bytes(C) + 8 * kGroups * 2 * sizeof(double) + kGroups * sizeof(float2);
         const size_t cache_cap = 200 * 1024 - fixed;                     // slice bytes a lone CTA per SM can keep
@@ -684,11 +672,11 @@ int groupnorm_silu(const __half* x, long long ldx, __half* y, long long ldy, lon
                 attr_done = true;
             }
             if (silu)
-                launch_pdl(gn_fused_kernel<true>, dim3(cpi, n_inst), kNormThreads, smem, stream, x, ldx, y, ldy, C, rows_per_inst, rpc2,
-                           eps, partial, counters, gen, gamma, beta, cache);
+                gn_fused_kernel<true><<<dim3(cpi, n_inst), kNormThreads, smem, stream>>>(x, ldx, y, ldy, C, rows_per_inst, rpc2,
+                                                                                         eps, partial, counters, gen, gamma, beta, cache);
             else
-                launch_pdl(gn_fused_kernel<false>, dim3(cpi, n_inst), kNormThreads, smem, stream, x, ldx, y, ldy, C, rows_per_inst, rpc2,
-                           eps, partial, counters, gen, gamma, beta, cache);
+                gn_fused_kernel<false><<<dim3(cpi, n_inst), kNormThreads, smem, stream>>>(x, ldx, y, ldy, C, rows_per_inst, rpc2,
+                                                                                          eps, partial, counters, gen, gamma, beta, cache);
             return launch_status("norm launch");
         }
     }
@@ -699,8 +687,8 @@ int groupnorm_silu(const __half* x, long long ldx, __half* y, long long ldy, lon
         gs = *shard;
     }
     if (phase != 2)
-        launch_pdl(gn_stats_kernel, dim3(nchunks, n_inst), kNormThreads, stats_smem_bytes(C), stream, x, ldx, C, rows_per_inst,
-                   rpc, nchunks, eps, partial, counters, stats, gs);
+        gn_stats_kernel<<<dim3(nchunks, n_inst), kNormThreads, stats_smem_bytes(C), stream>>>(x, ldx, C, rows_per_inst,
+                                                                                              rpc, nchunks, eps, partial, counters, stats, gs);
     if (phase == 1) return launch_status("norm launch");
     // rows per apply block: ~4 blocks per SM overall, at least 4 rows
     long long want_blocks = static_cast<long long>(num_sms) * 4;
@@ -710,11 +698,11 @@ int groupnorm_silu(const __half* x, long long ldx, __half* y, long long ldy, lon
     if (rpb < 4) rpb = 4;
     const int nblk = static_cast<int>((rows_per_inst + rpb - 1) / rpb);
     if (silu)
-        launch_pdl(gn_apply_kernel<true>, dim3(nblk, n_inst), kNormThreads, 0, stream, x, ldx, y, ldy, C, rows_per_inst,
-                   static_cast<int>(rpb), stats, gamma, beta);
+        gn_apply_kernel<true><<<dim3(nblk, n_inst), kNormThreads, 0, stream>>>(x, ldx, y, ldy, C, rows_per_inst,
+                                                                               static_cast<int>(rpb), stats, gamma, beta);
     else
-        launch_pdl(gn_apply_kernel<false>, dim3(nblk, n_inst), kNormThreads, 0, stream, x, ldx, y, ldy, C, rows_per_inst,
-                   static_cast<int>(rpb), stats, gamma, beta);
+        gn_apply_kernel<false><<<dim3(nblk, n_inst), kNormThreads, 0, stream>>>(x, ldx, y, ldy, C, rows_per_inst,
+                                                                                static_cast<int>(rpb), stats, gamma, beta);
     return launch_status("norm launch");
 }
 
@@ -723,10 +711,10 @@ int layernorm_rowstats(const __half* x, long long ldx, long long rows, int C, fl
     const long long need = (rows + 15) / 16;                           // 8 warps x 2 rows per block pass
     const unsigned int grid = static_cast<unsigned int>(std::min<long long>(need, static_cast<long long>(num_sms()) * 8));
     const int nv = (C / 8 + 31) / 32;
-    if (nv <= 2) launch_pdl(ln_rowstats_kernel<2>, grid, 256, 0, stream, x, ldx, rows, C, eps, out);
-    else if (nv <= 3) launch_pdl(ln_rowstats_kernel<3>, grid, 256, 0, stream, x, ldx, rows, C, eps, out);
-    else if (nv <= 5) launch_pdl(ln_rowstats_kernel<5>, grid, 256, 0, stream, x, ldx, rows, C, eps, out);
-    else launch_pdl(ln_rowstats_kernel<8>, grid, 256, 0, stream, x, ldx, rows, C, eps, out);
+    if (nv <= 2) ln_rowstats_kernel<2><<<grid, 256, 0, stream>>>(x, ldx, rows, C, eps, out);
+    else if (nv <= 3) ln_rowstats_kernel<3><<<grid, 256, 0, stream>>>(x, ldx, rows, C, eps, out);
+    else if (nv <= 5) ln_rowstats_kernel<5><<<grid, 256, 0, stream>>>(x, ldx, rows, C, eps, out);
+    else ln_rowstats_kernel<8><<<grid, 256, 0, stream>>>(x, ldx, rows, C, eps, out);
     return launch_status("norm launch");
 }
 
@@ -734,7 +722,7 @@ int layernorm(const __half* x, long long ldx, __half* y, long long ldy, long lon
               const __half* beta, float eps, cudaStream_t stream) {
     if (C % 8 != 0 || C > 2048) return -1;
     const long long blocks = (rows + 7) / 8;
-    launch_pdl(layernorm_kernel, static_cast<unsigned int>(blocks), 256, 0, stream, x, ldx, y, ldy, rows, C, gamma, beta, eps);
+    layernorm_kernel<<<static_cast<unsigned int>(blocks), 256, 0, stream>>>(x, ldx, y, ldy, rows, C, gamma, beta, eps);
     return launch_status("norm launch");
 }
 

@@ -387,8 +387,7 @@ int Builder::gemm(GemmProblem& p) {
     // Split-K for contractions whose output cannot fill the machine (low-resolution levels: rows = 768 / 3072 with K up to
     // 23040): each (tile, split) work item accumulates a K range into an fp32 partial, a fix-up kernel folds the partials
     // in a fixed order and applies bias / residual.  Deterministic; chosen only when >= half of the SMs would idle.
-    static const bool no_split = getenv("T2V_NO_SPLITK") != nullptr;
-    if (!no_split && p.splits <= 1 && gemm_splitk_unsupported(p) == nullptr) {
+    if (p.splits <= 1 && gemm_splitk_unsupported(p) == nullptr) {
         const long long tiles_m = (static_cast<long long>(rows) + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M;
         const long long tiles = tiles_m * ((p.N + 255) / 256);
         const int kt = p.ntaps * ((p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K);

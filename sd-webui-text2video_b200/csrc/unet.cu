@@ -502,14 +502,7 @@ Tok transformer_block(Ctx& c, Tok x, const std::string& p, int heads, long long 
             const AttnParams apc = ap_;
             const double fl = 4.0 * apc.batch * apc.heads * static_cast<double>(apc.sq) * apc.skv * 64;
             const char* label = temporal ? "attn temporal" : (self_attn ? "attn spatial" : "attn cross");
-            AttnTcPlan tcp;
-            if (!c.b->dry() && attention_tc_eligible(apc) && !getenv("T2V_ATTN_WARP_MMA") &&
-                attention_tc_plan(apc, &tcp) == 0) {
-                // long sequences: wgmma kernel, tensor maps encoded once here
-                c.b->step([tcp](cudaStream_t s) { return attention_tc_launch(tcp, s); }, 1, STEP_ATTN, fl, label);
-            } else {
-                c.b->step([apc](cudaStream_t s) { return attention(apc, s); }, 1, STEP_ATTN, fl, label);
-            }
+            c.b->step([apc](cudaStream_t s) { return attention(apc, s); }, 1, STEP_ATTN, fl, label);
         }
         c.b->free(qkv);
         if (!self_attn) c.b->free(kv);
@@ -689,7 +682,7 @@ Tok stt_block(Ctx& c, const Tok& xin, const Blk& blk, int hcur, int wcur) {
         a.q_ss = a.k_ss = a.v_ss = qkv.ld;
         a.o_bs = P * o.ld;
         a.o_ss = o.ld;
-        c.b->step([a](cudaStream_t s) { return a.head_dim == 64 ? attention(a, s) : attention_hd(a, s); }, 1, STEP_ATTN,
+        c.b->step([a](cudaStream_t s) { return attention(a, s); }, 1, STEP_ATTN,
                   4.0 * a.batch * a.heads * static_cast<double>(a.sq) * a.skv * d, "attn spatial (vc)");
         finish(o, qkv, ap);
     };
@@ -741,7 +734,7 @@ Tok stt_block(Ctx& c, const Tok& xin, const Blk& blk, int hcur, int wcur) {
         a.k_ss = a.v_ss = kv.ld;
         a.kv_batch_div = c.F;
         a.o_bs = P * o.ld; a.o_ss = o.ld;
-        c.b->step([a](cudaStream_t s) { return a.head_dim == 64 ? attention(a, s) : attention_hd(a, s); }, 1, STEP_ATTN,
+        c.b->step([a](cudaStream_t s) { return attention(a, s); }, 1, STEP_ATTN,
                   4.0 * a.batch * a.heads * static_cast<double>(a.sq) * a.skv * d, "attn cross (vc)");
         c.b->free(kv);
         finish(o, q, ap);
