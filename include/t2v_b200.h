@@ -366,22 +366,35 @@ int t2v_op_groupnorm(const void* x, long long ldx, void* y, long long ldy, long 
                      const void* gamma, const void* beta, float eps, int silu, void* stream);
 int t2v_op_layernorm(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, const void* gamma,
                      const void* beta, float eps, void* stream);
+/* softmax(Q K^T * scale) V, head_dim 64, head h at column h * 64; batch b reads Q / O at b * X_bs and K / V at
+ * (b / kv_batch_div) * X_bs.  Strides in elements.  Returns -1 without launching on operands the kernels cannot load:
+ * Q, K, V not 16-byte aligned or a Q / K / V stride not a multiple of 8 (0 is allowed), O not 4-byte aligned or an odd
+ * O stride. */
 int t2v_op_attention(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_ss,
                      long long k_bs, long long k_ss, long long v_bs, long long v_ss, long long o_bs, long long o_ss,
                      int batch, int heads, int sq, int skv, int kv_batch_div, float scale, void* stream);
 /* same for head_dim in {8,16,32,40,80,160} (64 dispatches to t2v_op_attention's kernels): CrossAttention.forward of the
- * VideoCrafter denoiser, videocrafter/lvdm/models/modules/attention_temporal.py:167-190 (8 heads of width C/8). */
+ * VideoCrafter denoiser, videocrafter/lvdm/models/modules/attention_temporal.py:167-190 (8 heads of width C/8), plus a
+ * two-level batch: batch index b -> (b / b_inner) * X_bs + (b % b_inner) * X_bsi for X in q, k, v, o (K / V after the
+ * kv_batch_div division); b_inner = 1 leaves the X_bsi unused.  With head_dim 64 this reaches the ModelScope temporal
+ * attention layout (outer = sample, inner = pixel, sequence = frames).  Same alignment rules as t2v_op_attention. */
 int t2v_op_attention_hd(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_ss,
                         long long k_bs, long long k_ss, long long v_bs, long long v_ss, long long o_bs, long long o_ss,
-                        int batch, int heads, int head_dim, int sq, int skv, int kv_batch_div, float scale, void* stream);
+                        int batch, int heads, int head_dim, int sq, int skv, int kv_batch_div, float scale, int b_inner,
+                        long long q_bsi, long long k_bsi, long long v_bsi, long long o_bsi, void* stream);
 /* TemporalCrossAttention.forward with RelativePosition tables (attention_temporal.py:46-65, :107-144), context = x:
  * sequences of T <= 32 frames; sequence s of n_seq lives at (s / seq_inner) * bs_outer + (s % seq_inner) * bs_inner, its
  * frames `ss` elements apart; head h at column h * head_dim; tables [2*max_rel+1, head_dim] fp16 (2*max_rel+1 <= 48),
- * frame distances beyond +-max_rel use the end rows of the tables, as the reference's clamp. */
+ * frame distances beyond +-max_rel use the end rows of the tables, as the reference's clamp.  Same alignment rules as
+ * t2v_op_attention, and the tables 16-byte aligned. */
 int t2v_op_attention_relpos(const void* q, const void* k, const void* v, void* o, const void* table_k, const void* table_v,
                             long long n_seq, long long seq_inner, long long bs_outer, long long bs_inner, long long ss,
                             long long o_bs_outer, long long o_bs_inner, long long o_ss, int heads, int head_dim, int T,
                             int max_rel, float scale, void* stream);
+/* The CLIP / OpenCLIP text towers' causal self-attention (nn.MultiheadAttention with the causal mask): qkv [B*L, 3W] fp16
+ * as in_proj lays it out (q | k | v, head h at columns h*64 of each part) -> o [B*L, W]; q is scaled by 64^-0.5 before
+ * q.k as nn.MultiheadAttention does.  -1 unless W % 64 == 0, W / heads == 64 and 1 <= L <= 128. */
+int t2v_op_clip_attention(const void* qkv, void* o, int B, int L, int W, int heads, void* stream);
 int t2v_op_upsample2x(const void* x, void* y, int nframes, int h, int w, int C, void* stream);
 int t2v_op_im2col_s2(const void* x, void* col, int nframes, int h, int w, int C, void* stream);
 int t2v_op_time_sinusoid(const float* t, void* out, int B, int dim, void* stream);

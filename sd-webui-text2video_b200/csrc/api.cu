@@ -317,7 +317,8 @@ int t2v_op_attention(const void* q, const void* k, const void* v, void* o, long 
 }
 int t2v_op_attention_hd(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_ss,
                         long long k_bs, long long k_ss, long long v_bs, long long v_ss, long long o_bs, long long o_ss,
-                        int batch, int heads, int head_dim, int sq, int skv, int kv_batch_div, float scale, void* stream) {
+                        int batch, int heads, int head_dim, int sq, int skv, int kv_batch_div, float scale, int b_inner,
+                        long long q_bsi, long long k_bsi, long long v_bsi, long long o_bsi, void* stream) {
     AttnParams p;
     memset(&p, 0, sizeof(p));
     p.q = reinterpret_cast<const __half*>(q);
@@ -326,7 +327,8 @@ int t2v_op_attention_hd(const void* q, const void* k, const void* v, void* o, lo
     p.o = reinterpret_cast<__half*>(o);
     p.q_bs = q_bs; p.q_ss = q_ss; p.k_bs = k_bs; p.k_ss = k_ss; p.v_bs = v_bs; p.v_ss = v_ss; p.o_bs = o_bs; p.o_ss = o_ss;
     p.batch = batch; p.heads = heads; p.sq = sq; p.skv = skv; p.head_dim = head_dim; p.kv_batch_div = kv_batch_div;
-    p.scale = scale; p.b_inner = 1;
+    p.scale = scale; p.b_inner = b_inner;
+    p.q_bsi = q_bsi; p.k_bsi = k_bsi; p.v_bsi = v_bsi; p.o_bsi = o_bsi;
     return attention(p, reinterpret_cast<cudaStream_t>(stream));
 }
 int t2v_op_attention_relpos(const void* q, const void* k, const void* v, void* o, const void* table_k, const void* table_v,

@@ -202,6 +202,27 @@ __global__ void __launch_bounds__(2 * TS) attention_kernel(AttnParams p) {
 
 }  // namespace
 
+bool attention_args_aligned(const AttnParams& p) {
+    const uintptr_t ptrs[] = {reinterpret_cast<uintptr_t>(p.q), reinterpret_cast<uintptr_t>(p.k),
+                              reinterpret_cast<uintptr_t>(p.v)};
+    for (uintptr_t x : ptrs)
+        if (x & 15) {
+            set_error("attention: Q, K and V must be 16-byte aligned");
+            return false;
+        }
+    const long long strides[] = {p.q_bs, p.q_bsi, p.q_ss, p.k_bs, p.k_bsi, p.k_ss, p.v_bs, p.v_bsi, p.v_ss};
+    for (long long s : strides)
+        if (s & 7) {
+            set_error("attention: Q, K and V strides must be multiples of 8 elements");
+            return false;
+        }
+    if ((reinterpret_cast<uintptr_t>(p.o) & 3) || ((p.o_bs | p.o_bsi | p.o_ss) & 1)) {
+        set_error("attention: O must be 4-byte aligned with even strides");
+        return false;
+    }
+    return true;
+}
+
 int attention(const AttnParams& p, cudaStream_t stream) {
     if (p.head_dim != HD) return attention_hd(p, stream);
     if (p.sq <= 0 || p.skv <= 0 || p.kv_batch_div <= 0 || p.b_inner <= 0) return -1;
@@ -211,6 +232,7 @@ int attention(const AttnParams& p, cudaStream_t stream) {
         if (rc != 0) return rc;
         return attention_tc_launch(plan, stream);
     }
+    if (!attention_args_aligned(p)) return -1;
     const bool small = p.sq <= 32 && p.skv <= 32;
     const int ts = small ? 32 : 64;
     dim3 grid(p.batch, p.heads, (p.sq + ts - 1) / ts);

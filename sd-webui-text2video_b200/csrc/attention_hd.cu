@@ -472,6 +472,7 @@ int launch_relpos(const RelposParams& p, cudaStream_t stream) {
 
 int attention_hd(const AttnParams& p, cudaStream_t stream) {
     if (p.sq <= 0 || p.skv <= 0 || p.kv_batch_div <= 0 || p.b_inner <= 0) return -1;
+    if (!attention_args_aligned(p)) return -1;
     switch (p.head_dim) {
         case 8: return launch_hd<8>(p, stream);
         case 16: return launch_hd<16>(p, stream);
@@ -486,6 +487,22 @@ int attention_hd(const AttnParams& p, cudaStream_t stream) {
 int attention_relpos(const RelposParams& p, cudaStream_t stream) {
     if (p.T < 1 || p.T > 32 || p.max_rel < 1 || 2 * p.max_rel + 1 > RJ || p.n_seq <= 0 || p.heads <= 0 || p.seq_inner <= 0)
         return -1;
+    // same operand rules as attention_args_aligned; the tables are cp.async sources too
+    const uintptr_t ptrs[] = {reinterpret_cast<uintptr_t>(p.q), reinterpret_cast<uintptr_t>(p.k), reinterpret_cast<uintptr_t>(p.v),
+                              reinterpret_cast<uintptr_t>(p.table_k), reinterpret_cast<uintptr_t>(p.table_v)};
+    for (uintptr_t x : ptrs)
+        if (x & 15) {
+            set_error("attention_relpos: Q, K, V and the tables must be 16-byte aligned");
+            return -1;
+        }
+    if ((p.bs_outer | p.bs_inner | p.ss) & 7) {
+        set_error("attention_relpos: Q, K and V strides must be multiples of 8 elements");
+        return -1;
+    }
+    if ((reinterpret_cast<uintptr_t>(p.o) & 3) || ((p.o_bs_outer | p.o_bs_inner | p.o_ss) & 1)) {
+        set_error("attention_relpos: O must be 4-byte aligned with even strides");
+        return -1;
+    }
     switch (p.head_dim) {
         case 8: return launch_relpos<8>(p, stream);
         case 16: return launch_relpos<16>(p, stream);

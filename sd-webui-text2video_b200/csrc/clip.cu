@@ -266,11 +266,8 @@ int build(t2v_clip* m, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
         Tok o = bld.alloc(R, W);
         {
             const Tok q = qkv, oo = o;
-            const size_t smem = static_cast<size_t>(2) * L * 66 * sizeof(__half);
-            bld.step([=](cudaStream_t s) {
-                clip_attention_kernel<<<dim3(static_cast<unsigned>(B * heads)), dim3(128), smem, s>>>(q.p, oo.p, L, W, heads);
-                return launch_status("clip launch");
-            }, 1, STEP_ATTN, 4.0 * B * heads * static_cast<double>(L) * L * kClipD / 2, "clip causal attention");
+            bld.step([=](cudaStream_t s) { return clip_attention(q.p, oo.p, B, L, W, heads, s); }, 1, STEP_ATTN,
+                     4.0 * B * heads * static_cast<double>(L) * L * kClipD / 2, "clip causal attention");
         }
         bld.free(qkv);
         Tok y = linear(c, o, prm(c, p + out_proj + ".weight"), W, prm(c, p + out_proj + ".bias"), &x);
@@ -314,9 +311,29 @@ __global__ void clip_out_kernel(const __half* __restrict__ z, void* __restrict__
 }
 
 }  // namespace
+
+int clip_attention(const __half* qkv, __half* o, int B, int L, int W, int heads, cudaStream_t stream) {
+    if (B < 1 || heads < 1 || W % kClipD != 0 || W / heads != kClipD || L < 1 || L > 128) {
+        set_error("clip_attention: needs W %% 64 == 0, W / heads == 64, 1 <= L <= 128 (B %d, L %d, W %d, heads %d)", B, L, W, heads);
+        return -1;
+    }
+    if (reinterpret_cast<uintptr_t>(qkv) & 3) {        // K and V are read as __half2
+        set_error("clip_attention: qkv must be 4-byte aligned");
+        return -1;
+    }
+    const size_t smem = static_cast<size_t>(2) * L * 66 * sizeof(__half);
+    clip_attention_kernel<<<dim3(static_cast<unsigned>(B * heads)), dim3(128), smem, stream>>>(qkv, o, L, W, heads);
+    return launch_status("clip launch");
+}
+
 }  // namespace t2v
 
 extern "C" {
+
+int t2v_op_clip_attention(const void* qkv, void* o, int B, int L, int W, int heads, void* stream) {
+    return clip_attention(reinterpret_cast<const __half*>(qkv), reinterpret_cast<__half*>(o), B, L, W, heads,
+                          reinterpret_cast<cudaStream_t>(stream));
+}
 
 int t2v_clip_create(const t2v_clip_config* cfg, t2v_clip** out) {
     if (!cfg || !out) return -1;

@@ -39,8 +39,12 @@ struct AttnParams {
     float scale;
 };
 // Picks the kernel for every caller: head_dim != 64 -> attention_hd; attention_tc when attention_tc_eligible; else the
-// warp-MMA kernel of attention.cu.
+// warp-MMA kernel of attention.cu.  Returns -1 without launching when attention_args_aligned fails on the warp-MMA route.
 int attention(const AttnParams& p, cudaStream_t stream);
+// What the warp-MMA and any-head-dim kernels need of their operands: 16-byte cp.async loads (Q, K, V 16-byte aligned, every
+// batch, inner-batch and sequence stride a multiple of 8 elements; 0 is a legal broadcast) and __half2 stores (O 4-byte
+// aligned, even strides).  Records the reason with set_error when it returns false.
+bool attention_args_aligned(const AttnParams& p);
 
 // attention_hd.cu: head dims other than 64 (VideoCrafter: C/8 = 40 / 80 / 160) and temporal attention with
 // relative-position tables.  attention_hd takes the same AttnParams (head h at column h*head_dim).
@@ -59,6 +63,7 @@ struct RelposParams {
     int heads, head_dim, T, max_rel;
     float scale;
 };
+// -1 without launching on bad shapes or on operands that break attention_args_aligned's rules (the tables 16-byte aligned too)
 int attention_relpos(const RelposParams& p, cudaStream_t stream);
 
 // attention_tc.cu: wgmma / TMA kernel for long self-attention sequences (sq >= 256, skv >= 128, one-level batch).
@@ -73,6 +78,11 @@ struct AttnTcPlan {
 bool attention_tc_eligible(const AttnParams& p);
 int attention_tc_plan(const AttnParams& p, AttnTcPlan* plan);
 int attention_tc_launch(const AttnTcPlan& plan, cudaStream_t stream);
+
+// clip.cu: causal self-attention of the CLIP / OpenCLIP text towers on nn.MultiheadAttention's fused in_proj output
+// qkv [B*L, 3W] (q | k | v, head h at columns h*64 of each part) -> o [B*L, W]; q scaled by 64^-0.5 before q.k.
+// -1 unless W % 64 == 0, W / heads == 64 and 1 <= L <= 128 (what t2v_clip_create accepts).
+int clip_attention(const __half* qkv, __half* o, int B, int L, int W, int heads, cudaStream_t stream);
 
 // ---------------------------------------------------------------- elementwise.cu
 // x [B, C, F, h, w] (fp32 or fp16, NCFHW as the samplers hold it) -> tokens [B*F*h*w, ld] fp16, channels >= C zeroed up to cpad

@@ -99,9 +99,10 @@ SIGNATURES = {
     't2v_op_attention': (c_int, [P, P, P, P, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_int,
                                  c_int, c_float, P]),
     't2v_op_attention_hd': (c_int, [P, P, P, P, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_int,
-                                    c_int, c_int, c_float, P]),
+                                    c_int, c_int, c_float, c_int, c_ll, c_ll, c_ll, c_ll, P]),
     't2v_op_attention_relpos': (c_int, [P, P, P, P, P, P, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_int, c_int,
                                         c_int, c_int, c_float, P]),
+    't2v_op_clip_attention': (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
     't2v_op_upsample2x': (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
     't2v_op_im2col_s2': (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
     't2v_op_time_sinusoid': (c_int, [P, P, c_int, c_int, P]),

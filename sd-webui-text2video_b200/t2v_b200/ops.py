@@ -203,13 +203,29 @@ def attention(q, k, v, o, q_bs, q_ss, k_bs, k_ss, v_bs, v_ss, o_bs, o_ss, batch,
 
 
 def attention_hd(q, k, v, o, q_bs, q_ss, k_bs, k_ss, v_bs, v_ss, o_bs, o_ss, batch, heads, head_dim, sq, skv, kv_batch_div=1,
-                 scale=None):
-    """softmax(QK^T * scale)V for any supported head_dim (head h at column h*head_dim of the token matrices)."""
+                 scale=None, *, b_inner=1, q_bsi=0, k_bsi=0, v_bsi=0, o_bsi=0):
+    """softmax(QK^T * scale)V for any supported head_dim (head h at column h*head_dim of the token matrices).
+    Two-level batch: batch index b -> (b // b_inner) * X_bs + (b % b_inner) * X_bsi (K / V after the kv_batch_div division)."""
     l = _lib.lib()
     scale = head_dim ** -0.5 if scale is None else scale
     rc = l.t2v_op_attention_hd(_lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(o), q_bs, q_ss, k_bs, k_ss, v_bs, v_ss, o_bs,
-                               o_ss, batch, heads, head_dim, sq, skv, kv_batch_div, scale, _lib.stream_ptr())
+                               o_ss, batch, heads, head_dim, sq, skv, kv_batch_div, scale, b_inner, q_bsi, k_bsi, v_bsi, o_bsi,
+                               _lib.stream_ptr())
     _lib.check(rc, 'op_attention_hd')
+    return o
+
+
+def clip_attention(qkv, L, heads, o=None):
+    """Causal self-attention of the CLIP text towers: qkv [B*L, 3W] (q | k | v, head width 64) -> o [B*L, W]."""
+    l = _lib.lib()
+    rows, W3 = qkv.shape
+    W = W3 // 3
+    if o is None:
+        o = torch.empty((rows, W), device=qkv.device, dtype=torch.float16)
+    if not (qkv.is_contiguous() and o.is_contiguous()) or W3 != 3 * W or rows % L != 0 or tuple(o.shape) != (rows, W):
+        raise ValueError('clip_attention: qkv must be a dense [B*L, 3W] matrix and o a dense [B*L, W] one')
+    rc = l.t2v_op_clip_attention(_lib.ptr(qkv), _lib.ptr(o), rows // L, L, W, heads, _lib.stream_ptr())
+    _lib.check(rc, 'op_clip_attention')
     return o
 
 
