@@ -362,8 +362,18 @@ int t2v_op_pack_conv_weight(const void* src, int src_is_f32, void* dst, int Cout
                             int k_alloc, void* stream);
 int t2v_op_pack_geglu_weight(const void* w, const void* b, int src_is_f32, void* wdst, void* bdst, int H, int K, int bn,
                              void* stream);
+/* GroupNorm (32 groups, + SiLU when silu) of instances of rows_per_inst consecutive rows of x [rows, C] -> y.
+ * phase 0: what the model runs on one GPU (one fused launch where the grid can be co-resident, else statistics + apply).
+ * phase 1: statistics only, with the chunking of the frame-sharded plans; (mean, rstd) per (instance, group) go to
+ *          stats, fp32 [rows / rows_per_inst, 32, 2].  y is not written.
+ * phase 2: apply only, with the caller's stats in the same layout.
+ * Returns -1 without launching on bad arguments: C not a positive multiple of 32 up to 2560, rows not 1 to 65535 whole
+ * instances, x / y / gamma / beta not 16-byte aligned, ldx / ldy not multiples of 8 or below C; -5 if the workspace cannot
+ * be allocated. */
 int t2v_op_groupnorm(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, int rows_per_inst,
-                     const void* gamma, const void* beta, float eps, int silu, void* stream);
+                     const void* gamma, const void* beta, float eps, int silu, int phase, float* stats, void* stream);
+/* LayerNorm over C of every row.  Returns -1 without launching unless C % 8 == 0, 8 <= C <= 2048, 1 <= rows < 2^31, x / y /
+ * gamma / beta are 16-byte aligned and ldx, ldy are multiples of 8 and >= C. */
 int t2v_op_layernorm(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, const void* gamma,
                      const void* beta, float eps, void* stream);
 /* softmax(Q K^T * scale) V, head_dim 64, head h at column h * 64; batch b reads Q / O at b * X_bs and K / V at

@@ -285,16 +285,31 @@ int t2v_op_pack_geglu_weight(const void* w, const void* b, int src_is_f32, void*
                              reinterpret_cast<cudaStream_t>(stream));
 }
 int t2v_op_groupnorm(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, int rows_per_inst,
-                     const void* gamma, const void* beta, float eps, int silu, void* stream) {
+                     const void* gamma, const void* beta, float eps, int silu, int phase, float* stats, void* stream) {
+    const __half* xh = reinterpret_cast<const __half*>(x);
+    __half* yh = reinterpret_cast<__half*>(y);
+    const __half* gh = reinterpret_cast<const __half*>(gamma);
+    const __half* bh = reinterpret_cast<const __half*>(beta);
+    if (phase < 0 || phase > 2 || (phase != 0 && stats == nullptr)) {
+        set_error("op_groupnorm: phase %d must be 0, 1 or 2, and phases 1 and 2 need a stats buffer", phase);
+        return -1;
+    }
+    if (groupnorm_check(xh, ldx, yh, ldy, rows, C, rows_per_inst, gh, bh) != 0) return -1;
     const int n_inst = static_cast<int>(rows / rows_per_inst);
     void* ws = gn_scratch(gn_workspace_bytes(rows_per_inst, n_inst, g_num_sms));
     if (!ws) {
         set_error("groupnorm workspace allocation failed");
-        return -1;
+        return -5;
     }
-    return groupnorm_silu(reinterpret_cast<const __half*>(x), ldx, reinterpret_cast<__half*>(y), ldy, rows, C,
-                          rows_per_inst, reinterpret_cast<const __half*>(gamma), reinterpret_cast<const __half*>(beta),
-                          eps, silu, ws, g_num_sms, reinterpret_cast<cudaStream_t>(stream));
+    const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const size_t stats_bytes = static_cast<size_t>(n_inst) * 32 * sizeof(float2);
+    if (phase == 2 && cudaMemcpyAsync(gn_workspace_stats(ws), stats, stats_bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+        return launch_status("op_groupnorm: statistics copy");
+    const int rc = groupnorm_silu(xh, ldx, yh, ldy, rows, C, rows_per_inst, gh, bh, eps, silu, ws, g_num_sms, s, phase);
+    if (rc != 0 || phase != 1) return rc;
+    if (cudaMemcpyAsync(stats, gn_workspace_stats(ws), stats_bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+        return launch_status("op_groupnorm: statistics copy");
+    return 0;
 }
 int t2v_op_layernorm(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, const void* gamma,
                      const void* beta, float eps, void* stream) {

@@ -12,6 +12,11 @@ struct GnShard;      // shard.cuh: cross-rank part of a 5-D GroupNorm of a frame
 
 // ---------------------------------------------------------------- norm.cu
 size_t gn_workspace_bytes(int rows_per_inst, int n_inst, int num_sms);
+// 0, or -1 (and the reason in t2v_last_error) for arguments groupnorm_silu refuses before touching the workspace
+int groupnorm_check(const __half* x, long long ldx, const __half* y, long long ldy, long long rows, int C, int rows_per_inst,
+                    const __half* gamma, const __half* beta);
+// where the workspace holds the per-(instance, group) (mean, rstd), fp32 [n_inst, 32, 2]: written by phase 1, read by phase 2
+float2* gn_workspace_stats(void* workspace);
 int groupnorm_silu(const __half* x, long long ldx, __half* y, long long ldy, long long rows, int C, int rows_per_inst,
                    const __half* gamma, const __half* beta, float eps, int silu, void* workspace, int num_sms,
                    cudaStream_t stream, int phase = 0,    // phase 0: stats + apply, 1: stats only, 2: apply only

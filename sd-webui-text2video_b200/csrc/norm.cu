@@ -5,6 +5,11 @@
 // (F*h*w rows).  Both are "instances" of `rows_per_inst` consecutive rows here.
 // fp32 math throughout (the reference runs group_norm / layer_norm / SiLU-after-norm in fp32 under autocast and
 // rounds to fp16 only when the value enters the next conv/linear -- exactly where these kernels round).
+// GroupNorm statistics are summed as x - K_g in fp32, with a pivot K_g per (instance, group): the value of the group's first
+// channel in the instance's first row.  Raw fp32 sums of x and x^2 would lose the variance to cancellation once
+// |mean| / std reaches ~100 (E[x^2] - mean^2); shifted by a sample of the group, the sums stay of the size of the spread.
+// The fold turns them back into raw moments in double (sum x = S + nK, sum x^2 = Q + 2KS + nK^2), where the cancellation
+// of var = E[x^2] - mean^2 costs only (mean / std)^2 2^-53.
 #include <algorithm>
 #include <cstring>
 
@@ -18,7 +23,8 @@ namespace {
 
 constexpr int kGroups = 32;
 constexpr int kNormThreads = 320;    // = 8 x 40 = 4 x 80 = 2 x 160 vectors: whole rows of C = 320 / 640 / 1280 per pass
-constexpr size_t kCounterBytes = 1 << 20;   // up to 262144 norm instances (frames x samples) per call
+constexpr int kMaxInst = 65535;             // instances (frames x samples) per call: gridDim.y
+constexpr size_t kCounterBytes = 1 << 20;   // chunk counters [0, kMaxInst) | fused-kernel barrier generations from word 131072
 
 // Thread mapping shared by the statistics and the apply kernel: a block covers RL = 320 / (C/8) consecutive rows per
 // pass; thread (rl, vc) owns the 16-byte vector vc (8 channels) of rows rl, rl + RL, ...  Consecutive threads read
@@ -37,7 +43,34 @@ __device__ __forceinline__ RowMap row_map(int C8) {
     return m;
 }
 
-// partial[(inst * nchunks + chunk) * 32 + g] = (sum, sumsq) ; the last block of an instance folds them (in
+// The pivots K_g of the 8 channels a thread owns: x[first row of the instance, first channel of the channel's group].
+__device__ __forceinline__ void load_pivots(const __half* inst_row0, int vc, int cpg, float (&k)[8]) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) k[e] = __half2float(inst_row0[(vc * 8 + e) / cpg * cpg]);
+}
+
+// Shifted per-thread sums of one 16-byte vector: s += x - K, q += (x - K)^2.
+__device__ __forceinline__ void accum_vec(const uint4& v, const float (&k)[8], float (&s)[8], float (&q)[8]) {
+    const __half2* h2 = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const float2 f = __half22float2(h2[e]);
+        const float d0 = f.x - k[2 * e], d1 = f.y - k[2 * e + 1];
+        s[2 * e] += d0;
+        q[2 * e] = fmaf(d0, d0, q[2 * e]);
+        s[2 * e + 1] += d1;
+        q[2 * e + 1] = fmaf(d1, d1, q[2 * e + 1]);
+    }
+}
+
+// Raw moments (sum x, sum x^2) of a group from its shifted sums (S, Q) over n elements and its pivot K, in double.
+__device__ __forceinline__ void unshift(double& a, double& b, double n, float K) {
+    const double k = K;
+    b += (2.0 * a + n * k) * k;
+    a += n * k;
+}
+
+// partial[(inst * nchunks + chunk) * 32 + g] = (sum, sumsq) of x - K_g; the last block of an instance folds them (in
 // chunk order, double precision) into stats[inst*32+g] = (mean, rstd) -> deterministic, no float atomics in HBM.
 __global__ void __launch_bounds__(kNormThreads) gn_stats_kernel(const __half* __restrict__ x, long long ld, int C,
                                                                 int rows_per_inst, int rows_per_chunk, int nchunks,
@@ -56,10 +89,13 @@ __global__ void __launch_bounds__(kNormThreads) gn_stats_kernel(const __half* __
     const int r0 = chunk * rows_per_chunk;
     const int r1 = min(r0 + rows_per_chunk, rows_per_inst);
     const __half* base = x + static_cast<long long>(inst) * rows_per_inst * ld;
+    const int cpg = C / kGroups;
     float s[8], q[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) s[e] = q[e] = 0.f;
     if (m.active) {
+        float k[8];
+        load_pivots(base, m.vc, cpg, k);
         constexpr int U = 4;               // independent 16-byte loads in flight per thread
         const __half* p = base + static_cast<long long>(r0 + m.rl) * ld + m.vc * 8;
         const long long step = static_cast<long long>(m.RL) * ld;
@@ -70,30 +106,12 @@ __global__ void __launch_bounds__(kNormThreads) gn_stats_kernel(const __half* __
             for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const uint4*>(p + u * step));
             p += U * step;
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const __half2* h2 = reinterpret_cast<const __half2*>(&v[u]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const float2 f = __half22float2(h2[e]);
-                    s[2 * e] += f.x;
-                    q[2 * e] = fmaf(f.x, f.x, q[2 * e]);
-                    s[2 * e + 1] += f.y;
-                    q[2 * e + 1] = fmaf(f.y, f.y, q[2 * e + 1]);
-                }
-            }
+            for (int u = 0; u < U; ++u) accum_vec(v[u], k, s, q);
         }
         for (; r < r1; r += m.RL) {
             const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
             p += step;
-            const __half2* h2 = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h2[e]);
-                s[2 * e] += f.x;
-                q[2 * e] = fmaf(f.x, f.x, q[2 * e]);
-                s[2 * e + 1] += f.y;
-                q[2 * e + 1] = fmaf(f.y, f.y, q[2 * e + 1]);
-            }
+            accum_vec(v, k, s, q);
         }
         // cross-row-lane reduction through smem in a fixed order (no atomics: bit-reproducible run to run)
         float4* d0 = reinterpret_cast<float4*>(red + (0 * m.RL + m.rl) * C + m.vc * 8);
@@ -114,7 +132,6 @@ __global__ void __launch_bounds__(kNormThreads) gn_stats_kernel(const __half* __
         s_sq[c] = b;
     }
     __syncthreads();
-    const int cpg = C / kGroups;
     if (threadIdx.x < kGroups) {
         float a = 0.f, b = 0.f;
         for (int c = 0; c < cpg; ++c) {
@@ -156,6 +173,7 @@ __global__ void __launch_bounds__(kNormThreads) gn_stats_kernel(const __half* __
                 b += fold[part][threadIdx.x][1];
             }
             double n = static_cast<double>(rows_per_inst) * cpg;
+            unshift(a, b, n, __half2float(base[threadIdx.x * cpg]));
             if (gs.peers.nranks > 1) {
                 // 5-D GroupNorm of a frame-sharded clip (pixel-sharded layout): this rank's (sum, sumsq) of the sample go to
                 // every rank over NVLink peer stores; all ranks then fold the P contributions in rank order, so mean / rstd
@@ -198,16 +216,36 @@ __device__ __forceinline__ float silu_f(float v) {
     return v * r;
 }
 
+// Per-channel scale a = rstd * gamma, mean and beta of the 8 channels a thread owns.
+struct GnAffine {
+    float a[8], mean[8], beta[8];
+};
+__device__ __forceinline__ void gn_affine(GnAffine& t, const float2* st, const __half* gamma, const __half* beta, int vc, int cpg) {
+    const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gamma + vc * 8));
+    const uint4 bv = __ldg(reinterpret_cast<const uint4*>(beta + vc * 8));
+    const __half* gh = reinterpret_cast<const __half*>(&gv);
+    const __half* bh = reinterpret_cast<const __half*>(&bv);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        const float2 ms = st[(vc * 8 + e) / cpg];
+        t.mean[e] = ms.x;
+        t.a[e] = ms.y * __half2float(gh[e]);
+        t.beta[e] = __half2float(bh[e]);
+    }
+}
+
+// y = act((x - mean) * a + beta): centring before the scale keeps a constant group at exactly beta, where
+// x * a + (beta - mean * a) would leave the rounding of mean * a (|mean| / sqrt(eps) large) in the output.
 template <bool SILU>
-__device__ __forceinline__ uint4 gn_apply_vec(const uint4& v, const float (&a)[8], const float (&b)[8]) {
+__device__ __forceinline__ uint4 gn_apply_vec(const uint4& v, const GnAffine& t) {
     const __half2* h2 = reinterpret_cast<const __half2*>(&v);
     uint4 o;
     __half2* oh = reinterpret_cast<__half2*>(&o);
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
         const float2 f = __half22float2(h2[e]);
-        float u0 = fmaf(f.x, a[2 * e], b[2 * e]);
-        float u1 = fmaf(f.y, a[2 * e + 1], b[2 * e + 1]);
+        float u0 = fmaf(f.x - t.mean[2 * e], t.a[2 * e], t.beta[2 * e]);
+        float u1 = fmaf(f.y - t.mean[2 * e + 1], t.a[2 * e + 1], t.beta[2 * e + 1]);
         if (SILU) {
             u0 = silu_f(u0);
             u1 = silu_f(u1);
@@ -217,8 +255,8 @@ __device__ __forceinline__ uint4 gn_apply_vec(const uint4& v, const float (&a)[8
     return o;
 }
 
-// grid = (row blocks, instances).  Each thread folds (mean, rstd, gamma, beta) of ITS 8 channels into scale/shift
-// registers, then streams its rows: y = act(x * a[c] + b[c]) -- one FMA (+ SiLU) per element, 16-byte accesses.
+// grid = (row blocks, instances).  Each thread folds (rstd, gamma) of ITS 8 channels into scale registers, then streams
+// its rows: y = act((x - mean[c]) * a[c] + beta[c]) -- one FADD and one FMA (+ SiLU) per element, 16-byte accesses.
 template <bool SILU>
 __global__ void __launch_bounds__(kNormThreads) gn_apply_kernel(const __half* __restrict__ x, long long ldx,
                                                                 __half* __restrict__ y, long long ldy, int C,
@@ -231,19 +269,8 @@ __global__ void __launch_bounds__(kNormThreads) gn_apply_kernel(const __half* __
     const int cpg = C / kGroups;
     const RowMap m = row_map(C8);
     if (!m.active) return;
-    float a[8], b[8];
-    {
-        const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gamma + m.vc * 8));
-        const uint4 bv = __ldg(reinterpret_cast<const uint4*>(beta + m.vc * 8));
-        const __half* gh = reinterpret_cast<const __half*>(&gv);
-        const __half* bh = reinterpret_cast<const __half*>(&bv);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            const float2 ms = __ldg(stats + inst * kGroups + (m.vc * 8 + e) / cpg);
-            a[e] = ms.y * __half2float(gh[e]);
-            b[e] = __half2float(bh[e]) - ms.x * a[e];
-        }
-    }
+    GnAffine t;
+    gn_affine(t, stats + inst * kGroups, gamma, beta, m.vc, cpg);
     const int r0 = blockIdx.x * rows_per_block;
     const int r1 = min(r0 + rows_per_block, rows_per_inst);
     const long long row0 = static_cast<long long>(inst) * rows_per_inst + r0 + m.rl;
@@ -258,13 +285,13 @@ __global__ void __launch_bounds__(kNormThreads) gn_apply_kernel(const __half* __
         for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const uint4*>(px + u * sx));
         px += U * sx;
 #pragma unroll
-        for (int u = 0; u < U; ++u) *reinterpret_cast<uint4*>(py + u * sy) = gn_apply_vec<SILU>(v[u], a, b);
+        for (int u = 0; u < U; ++u) *reinterpret_cast<uint4*>(py + u * sy) = gn_apply_vec<SILU>(v[u], t);
         py += U * sy;
     }
     for (; r < r1; r += m.RL) {
         const uint4 v = __ldg(reinterpret_cast<const uint4*>(px));
         px += sx;
-        *reinterpret_cast<uint4*>(py) = gn_apply_vec<SILU>(v, a, b);
+        *reinterpret_cast<uint4*>(py) = gn_apply_vec<SILU>(v, t);
         py += sy;
     }
 }
@@ -303,6 +330,8 @@ __global__ void __launch_bounds__(kNormThreads) gn_fused_kernel(const __half* __
 #pragma unroll
     for (int e = 0; e < 8; ++e) s[e] = q[e] = 0.f;
     if (m.active) {
+        float k[8];
+        load_pivots(base, m.vc, cpg, k);
         constexpr int U = 4;
         const __half* p = base + static_cast<long long>(r0 + m.rl) * ldx + m.vc * 8;
         const long long step = static_cast<long long>(m.RL) * ldx;
@@ -315,30 +344,14 @@ __global__ void __launch_bounds__(kNormThreads) gn_fused_kernel(const __half* __
 #pragma unroll
             for (int u = 0; u < U; ++u) {
                 if (cache) slice[static_cast<size_t>(r - r0 + u * m.RL) * C8 + m.vc] = v[u];
-                const __half2* h2 = reinterpret_cast<const __half2*>(&v[u]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const float2 f = __half22float2(h2[e]);
-                    s[2 * e] += f.x;
-                    q[2 * e] = fmaf(f.x, f.x, q[2 * e]);
-                    s[2 * e + 1] += f.y;
-                    q[2 * e + 1] = fmaf(f.y, f.y, q[2 * e + 1]);
-                }
+                accum_vec(v[u], k, s, q);
             }
         }
         for (; r < r1; r += m.RL) {
             const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
             p += step;
             if (cache) slice[static_cast<size_t>(r - r0) * C8 + m.vc] = v;
-            const __half2* h2 = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h2[e]);
-                s[2 * e] += f.x;
-                q[2 * e] = fmaf(f.x, f.x, q[2 * e]);
-                s[2 * e + 1] += f.y;
-                q[2 * e + 1] = fmaf(f.y, f.y, q[2 * e + 1]);
-            }
+            accum_vec(v, k, s, q);
         }
         float4* d0 = reinterpret_cast<float4*>(red + (0 * m.RL + m.rl) * C + m.vc * 8);
         float4* d1 = reinterpret_cast<float4*>(red + (1 * m.RL + m.rl) * C + m.vc * 8);
@@ -417,6 +430,7 @@ __global__ void __launch_bounds__(kNormThreads) gn_fused_kernel(const __half* __
             b += fold[(part * kGroups + threadIdx.x) * 2 + 1];
         }
         const double n = static_cast<double>(rows_per_inst) * cpg;
+        unshift(a, b, n, __half2float(base[threadIdx.x * cpg]));
         const double mean = a / n;
         double var = b / n - mean * mean;
         if (var < 0.0) var = 0.0;
@@ -424,19 +438,8 @@ __global__ void __launch_bounds__(kNormThreads) gn_fused_kernel(const __half* __
     }
     __syncthreads();
     if (!m.active) return;
-    float a[8], b[8];
-    {
-        const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gamma + m.vc * 8));
-        const uint4 bv = __ldg(reinterpret_cast<const uint4*>(beta + m.vc * 8));
-        const __half* gh = reinterpret_cast<const __half*>(&gv);
-        const __half* bh = reinterpret_cast<const __half*>(&bv);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            const float2 ms = st[(m.vc * 8 + e) / cpg];
-            a[e] = ms.y * __half2float(gh[e]);
-            b[e] = __half2float(bh[e]) - ms.x * a[e];
-        }
-    }
+    GnAffine t;
+    gn_affine(t, st, gamma, beta, m.vc, cpg);
     const long long row0 = static_cast<long long>(inst) * rows_per_inst + r0 + m.rl;
     const __half* px = x + row0 * ldx + m.vc * 8;
     __half* py = y + row0 * ldy + m.vc * 8;
@@ -450,13 +453,13 @@ __global__ void __launch_bounds__(kNormThreads) gn_fused_kernel(const __half* __
             v[u] = cache ? slice[static_cast<size_t>(r - r0 + u * m.RL) * C8 + m.vc] : __ldg(reinterpret_cast<const uint4*>(px + u * sx));
         px += U * sx;
 #pragma unroll
-        for (int u = 0; u < U; ++u) *reinterpret_cast<uint4*>(py + u * sy) = gn_apply_vec<SILU>(v[u], a, b);
+        for (int u = 0; u < U; ++u) *reinterpret_cast<uint4*>(py + u * sy) = gn_apply_vec<SILU>(v[u], t);
         py += U * sy;
     }
     for (; r < r1; r += m.RL) {
         const uint4 v = cache ? slice[static_cast<size_t>(r - r0) * C8 + m.vc] : __ldg(reinterpret_cast<const uint4*>(px));
         px += sx;
-        *reinterpret_cast<uint4*>(py) = gn_apply_vec<SILU>(v, a, b);
+        *reinterpret_cast<uint4*>(py) = gn_apply_vec<SILU>(v, t);
         py += sy;
     }
 }
@@ -623,20 +626,55 @@ size_t gn_workspace_bytes(int rows_per_inst, int n_inst, int num_sms) {
            (static_cast<size_t>(2 * num_sms) + n_inst) * kGroups * sizeof(float2) + 256;
 }
 
+static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
+int groupnorm_check(const __half* x, long long ldx, const __half* y, long long ldy, long long rows, int C, int rows_per_inst,
+                    const __half* gamma, const __half* beta) {
+    if (C <= 0 || C % 32 != 0 || C / 8 > kNormThreads) {
+        set_error("groupnorm: C = %d must be a positive multiple of 32, at most %d", C, 8 * kNormThreads);
+        return -1;
+    }
+    if (rows_per_inst <= 0 || rows < rows_per_inst || rows % rows_per_inst != 0 || rows / rows_per_inst > kMaxInst) {
+        set_error("groupnorm: rows = %lld must be 1 to %d whole instances of rows_per_inst = %d", rows, kMaxInst, rows_per_inst);
+        return -1;
+    }
+    // 16-byte vector loads and stores of x, y, gamma and beta
+    if (ldx < C || ldy < C || (ldx & 7) != 0 || (ldy & 7) != 0 || misaligned16(x) || misaligned16(y) || misaligned16(gamma) ||
+        misaligned16(beta)) {
+        set_error("groupnorm: x, y, gamma, beta must be 16-byte aligned and ldx = %lld, ldy = %lld multiples of 8, >= C = %d", ldx,
+                  ldy, C);
+        return -1;
+    }
+    return 0;
+}
+
+float2* gn_workspace_stats(void* workspace) { return reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(workspace) + kCounterBytes); }
+
+// the fused kernel's CTAs of one instance meet at a barrier: only launch it when the whole grid fits on the machine at once
+static bool gn_fused_coresident(int silu, size_t smem, long long ctas, int num_sms) {
+    int per_sm = 0;
+    const cudaError_t e = silu ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gn_fused_kernel<true>, kNormThreads, smem)
+                               : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gn_fused_kernel<false>, kNormThreads, smem);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return static_cast<long long>(per_sm) * num_sms >= ctas;
+}
+
 int groupnorm_silu(const __half* x, long long ldx, __half* y, long long ldy, long long rows, int C, int rows_per_inst,
                    const __half* gamma, const __half* beta, float eps, int silu, void* workspace, int num_sms,
                    cudaStream_t stream, int phase, const GnShard* shard) {
-    if (C % 32 != 0 || C % 8 != 0 || C / 8 > kNormThreads || rows % rows_per_inst != 0 || (ldx & 7) != 0 || (ldy & 7) != 0) return -1;
+    if (groupnorm_check(x, ldx, y, ldy, rows, C, rows_per_inst, gamma, beta) != 0) return -1;
     const int n_inst = static_cast<int>(rows / rows_per_inst);
     const int rpc = gn_rows_per_chunk(rows_per_inst, n_inst, num_sms);
     const int nchunks = (rows_per_inst + rpc - 1) / rpc;
-    if (static_cast<size_t>(n_inst) * sizeof(unsigned int) > kCounterBytes) return -3;
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     unsigned int* counters = reinterpret_cast<unsigned int*>(ws);
     float2* stats = reinterpret_cast<float2*>(ws + kCounterBytes);
     float2* partial = stats + static_cast<size_t>(n_inst) * kGroups;
     // ---- single-launch path (phase 0, no cross-rank statistics): all CTAs of the grid must be co-resident
-    if (phase == 0 && (shard == nullptr || shard->peers.nranks <= 1) && n_inst <= 65536) {
+    if (phase == 0 && (shard == nullptr || shard->peers.nranks <= 1)) {
         const size_t inst_bytes = static_cast<size_t>(rows_per_inst) * C * sizeof(__half);
         const size_t fixed = stats_smem_bytes(C) + 8 * kGroups * 2 * sizeof(double) + kGroups * sizeof(float2);
         const size_t cache_cap = 200 * 1024 - fixed;                     // slice bytes a lone CTA per SM can keep
@@ -662,22 +700,24 @@ int groupnorm_silu(const __half* x, long long ldx, __half* y, long long ldy, lon
                 cache = 0;
                 smem = fixed;
             }
-            const size_t need_ws = kCounterBytes + static_cast<size_t>(n_inst) * (kGroups + static_cast<size_t>(cpi) * kGroups) * sizeof(float2);
-            (void)need_ws;
-            unsigned int* gen = counters + (kCounterBytes / sizeof(unsigned int)) / 2;
             static bool attr_done = false;
             if (!attr_done) {
                 cudaFuncSetAttribute(gn_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
                 cudaFuncSetAttribute(gn_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
                 attr_done = true;
             }
-            if (silu)
-                gn_fused_kernel<true><<<dim3(cpi, n_inst), kNormThreads, smem, stream>>>(x, ldx, y, ldy, C, rows_per_inst, rpc2,
-                                                                                         eps, partial, counters, gen, gamma, beta, cache);
-            else
-                gn_fused_kernel<false><<<dim3(cpi, n_inst), kNormThreads, smem, stream>>>(x, ldx, y, ldy, C, rows_per_inst, rpc2,
-                                                                                          eps, partial, counters, gen, gamma, beta, cache);
-            return launch_status("norm launch");
+            // a grid that cannot be co-resident would spin at the barrier: it takes the two kernels below instead
+            if (gn_fused_coresident(silu, smem, static_cast<long long>(cpi) * n_inst, num_sms)) {
+                unsigned int* gen = counters + (kCounterBytes / sizeof(unsigned int)) / 2;
+                if (silu)
+                    gn_fused_kernel<true><<<dim3(cpi, n_inst), kNormThreads, smem, stream>>>(x, ldx, y, ldy, C, rows_per_inst, rpc2, eps,
+                                                                                             partial, counters, gen, gamma, beta, cache);
+                else
+                    gn_fused_kernel<false><<<dim3(cpi, n_inst), kNormThreads, smem, stream>>>(x, ldx, y, ldy, C, rows_per_inst, rpc2,
+                                                                                              eps, partial, counters, gen, gamma, beta,
+                                                                                              cache);
+                return launch_status("norm launch");
+            }
         }
     }
     GnShard gs;
@@ -720,7 +760,17 @@ int layernorm_rowstats(const __half* x, long long ldx, long long rows, int C, fl
 
 int layernorm(const __half* x, long long ldx, __half* y, long long ldy, long long rows, int C, const __half* gamma,
               const __half* beta, float eps, cudaStream_t stream) {
-    if (C % 8 != 0 || C > 2048) return -1;
+    if (C <= 0 || C % 8 != 0 || C > 2048 || rows < 1 || rows >= (1LL << 31)) {
+        set_error("layernorm: C = %d must be a multiple of 8 from 8 to 2048 and rows = %lld from 1 to 2^31 - 1", C, rows);
+        return -1;
+    }
+    // 16-byte vector loads and stores of x, y, gamma and beta
+    if (ldx < C || ldy < C || (ldx & 7) != 0 || (ldy & 7) != 0 || misaligned16(x) || misaligned16(y) || misaligned16(gamma) ||
+        misaligned16(beta)) {
+        set_error("layernorm: x, y, gamma, beta must be 16-byte aligned and ldx = %lld, ldy = %lld multiples of 8, >= C = %d", ldx,
+                  ldy, C);
+        return -1;
+    }
     const long long blocks = (rows + 7) / 8;
     layernorm_kernel<<<static_cast<unsigned int>(blocks), 256, 0, stream>>>(x, ldx, y, ldy, rows, C, gamma, beta, eps);
     return launch_status("norm launch");

@@ -175,18 +175,29 @@ def conv_taps_temporal():
     return [[0, kt - 1, 0] for kt in range(3)]
 
 
-def groupnorm(x, gamma, beta, rows_per_inst, eps, silu):
+def groupnorm(x, gamma, beta, rows_per_inst, eps, silu, phase=0, stats=None, out=None):
+    """GroupNorm (32 groups, + SiLU) over instances of rows_per_inst consecutive rows of x [rows, C] (a row-strided view
+    is fine).  phase 0: the model's single-GPU path, returns y.  phase 1: statistics only (the frame-sharded plans'
+    chunking), returns (mean, rstd) per (instance, group), fp32 [rows // rows_per_inst, 32, 2].  phase 2: apply only with
+    the given `stats` in that layout, returns y.  `out`: where y goes (by default a new dense [rows, C])."""
     l = _lib.lib()
-    y = torch.empty_like(x)
+    n_inst = x.shape[0] // rows_per_inst if rows_per_inst > 0 else 0
+    if phase == 1:
+        stats = torch.empty((n_inst, 32, 2), device=x.device, dtype=torch.float32) if stats is None else stats
+    elif phase == 2 and (stats is None or stats.dtype != torch.float32 or not stats.is_contiguous()
+                         or stats.numel() != n_inst * 64):
+        raise ValueError('groupnorm: phase 2 needs contiguous fp32 stats [rows // rows_per_inst, 32, 2]')
+    y = out if out is not None else torch.empty(x.shape, device=x.device, dtype=x.dtype)
     rc = l.t2v_op_groupnorm(_lib.ptr(x), x.stride(0), _lib.ptr(y), y.stride(0), x.shape[0], x.shape[1], rows_per_inst,
-                            _lib.ptr(gamma), _lib.ptr(beta), eps, int(silu), _lib.stream_ptr())
+                            _lib.ptr(gamma), _lib.ptr(beta), eps, int(silu), phase, _lib.ptr(stats), _lib.stream_ptr())
     _lib.check(rc, 'op_groupnorm')
-    return y
+    return stats if phase == 1 else y
 
 
-def layernorm(x, gamma, beta, eps=1e-5):
+def layernorm(x, gamma, beta, eps=1e-5, out=None):
+    """LayerNorm over the C columns of every row of x [rows, C] (a row-strided view is fine) -> `out` or a new dense matrix."""
     l = _lib.lib()
-    y = torch.empty_like(x)
+    y = out if out is not None else torch.empty(x.shape, device=x.device, dtype=x.dtype)
     rc = l.t2v_op_layernorm(_lib.ptr(x), x.stride(0), _lib.ptr(y), y.stride(0), x.shape[0], x.shape[1], _lib.ptr(gamma),
                             _lib.ptr(beta), eps, _lib.stream_ptr())
     _lib.check(rc, 'op_layernorm')
