@@ -71,6 +71,12 @@ int t2v_unet_param_info(t2v_unet* u, int index, char* name_out, size_t name_cap,
  *   out [B, out_dim, F, h, w] fp16 (out_is_f32 = 0) or fp32                                               */
 int t2v_unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, void* out,
                      int out_is_f32, int B, int F, int h, int w, int L, void* stream);
+/* t2v_unet_forward with a context batch ctx_B that divides B: ctx [ctx_B, L, context_dim], sample j reads prompt
+ * j / (B / ctx_B) -- for n clips guided as one batch, x = [x_1..x_n, x_1..x_n] and ctx = [c, uc] (ctx_B = 2).  The
+ * cross-attention K/V GEMMs project only the ctx_B * L distinct prompt rows, once per forward.  ctx_B = B is exactly
+ * t2v_unet_forward (same plan); ctx_B < B has a plan of its own.  Not available on a frame-sharded denoiser.          */
+int t2v_unet_forward_ctx(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, int ctx_B, void* out,
+                         int out_is_f32, int B, int F, int h, int w, int L, void* stream);
 /* eps = UNetModel.forward(x, t, context, features_adapter) (videocrafter/lvdm/models/modules/openaimodel3d.py:632-670), arch 1
  * only: feature i is added to h after input block id with (id + 1) % 3 == 0 (the i-th such block, counting from 0), before h is
  * pushed on the skip stack.  feats[i] is a device pointer to [feats_B, F, h_i, w_i, C_i] fp16, channels-last: the
@@ -86,6 +92,9 @@ int t2v_unet_forward_adapter(t2v_unet* u, const void* x, int x_is_f32, const flo
 double t2v_unet_flops(t2v_unet* u, int B, int F, int h, int w, int L);
 /* Activation-slab bytes the plan of this shape allocates (host only: the same dry pass as t2v_unet_flops). */
 int t2v_unet_plan_bytes(t2v_unet* u, int B, int F, int h, int w, int L, size_t* arena);
+/* Both of the above for the plan of a forward with context batch ctx_B (t2v_unet_forward_ctx), host only; *cached = 1 if the
+ * denoiser holds that plan for its current weights already (a forward then allocates nothing).  flops, cached may be null. */
+int t2v_unet_plan_info(t2v_unet* u, int B, int ctx_B, int F, int h, int w, int L, size_t* arena, double* flops, int* cached);
 int t2v_unet_num_launches(t2v_unet* u);
 /* Measurement aid: replays the plan of this shape once (inputs = whatever the last forward left in the staging
  * buffers) with a CUDA-event pair around every launch on `stream` and sums per kernel family:

@@ -252,6 +252,11 @@ public:
             }
         return nullptr;
     }
+    // Whether the plan of `key` built for weights `version` is held, without touching the use order.
+    bool holds(const std::string& key, unsigned long long version) const {
+        return std::any_of(entries_.begin(), entries_.end(),
+                           [&](const Entry& e) { return e.key == key && e.plan->weights_version == version; });
+    }
     // Builds the plan of `key` from `shell` with build_plan, `fn(plan, arena, dry, &io)` filling the entry's I/O record, and
     // keeps it as the most recently used.  First drops every plan of an older weights version (versions only grow, so such
     // a plan can never be replayed again) and then the least recently used ones down to the bound.  Null on failure.

@@ -31,7 +31,7 @@ constexpr int kMaxFeat = 8;
 struct IO {
     __half* x_tok;      // [R, 8]
     float* t;           // [B]
-    __half* ctx;        // [B*L, context_dim]
+    __half* ctx;        // [Bc*L, context_dim]
     __half* out_tok;    // [R, 8]
     // adapter features (plans built with feats_B > 0): staging [feats_B * F * h_i * w_i, C_i] per injection point
     int n_feat = 0;
@@ -365,11 +365,12 @@ void expect_params_vc(t2v_unet* u) {
 struct Ctx : NetCtx {
     t2v_unet* u;
     int B, F, h, w, L;
+    int Bc;                   // context batch: sample j reads prompt j / (B / Bc); = B when every sample brings its own
     int Fl;                   // frames held by this rank in the frame-sharded (FS) layout; = F when the clip is not sharded
     int rank, nranks;         // (0, 1) when not sharded
     char* slab;               // base of the plan's activation slab (exchange destinations are published as offsets into it)
     __half* emb;              // [B, E] time embedding (after time_embed MLP)
-    __half* ctx;              // [B*L, ctx_dim] fixed staging of the text conditioning
+    __half* ctx;              // [Bc*L, ctx_dim] fixed staging of the text conditioning
     Plan* plan;
 };
 
@@ -475,10 +476,11 @@ Tok transformer_block(Ctx& c, Tok x, const std::string& p, int heads, long long 
             const Param& wk = c.params->get(ap + ".to_k.weight");
             const int ctx_dim = wk.data ? static_cast<int>(wk.shape[1]) : c.u->cfg.context_dim;
             qkv = ln_linear(c, x, lnp, ap + ".to_q", prm(c, ap + ".to_q.weight"), nullptr, C, nullptr);
-            // K/V of the prompt: identical for every frame (the reference recomputes them per frame, :426,:545-546)
+            // K/V of the prompt: identical for every frame (the reference recomputes them per frame, :426,:545-546) and, with a
+            // context batch Bc < B, for every sample sharing the prompt: only the Bc * L distinct rows are projected
             Tok ctx_tok;
             ctx_tok.p = c.ctx;
-            ctx_tok.rows = static_cast<long long>(c.B) * c.L;
+            ctx_tok.rows = static_cast<long long>(c.Bc) * c.L;
             ctx_tok.C = ctx_dim;
             ctx_tok.ld = ctx_dim;
             const __half* wkv = w_cat(c, {ap + ".to_k.weight", ap + ".to_v.weight"});
@@ -494,7 +496,8 @@ Tok transformer_block(Ctx& c, Tok x, const std::string& p, int heads, long long 
             ap_.q_ss = qkv.ld;
             ap_.k_bs = ap_.v_bs = static_cast<long long>(c.L) * kv.ld;
             ap_.k_ss = ap_.v_ss = kv.ld;
-            ap_.kv_batch_div = c.Fl;          // frames per sample IN THIS MATRIX (frame-sharded clip: this rank's frames)
+            // frames per prompt IN THIS MATRIX: frames per sample (frame-sharded clip: this rank's frames) x samples per prompt
+            ap_.kv_batch_div = c.Fl * (c.B / c.Bc);
             ap_.o_bs = P * o.ld;
             ap_.o_ss = o.ld;
         }
@@ -711,12 +714,12 @@ Tok stt_block(Ctx& c, const Tok& xin, const Blk& blk, int hcur, int wcur) {
     };
     spatial_self(p + ".attn1", p + ".norm1");
     temporal(p + ".attn1_tmp", p + ".norm4");
-    {   // spatial cross-attention on the prompt: K/V projected once per sample (the reference repeats the context per frame, :321-325)
+    {   // spatial cross-attention on the prompt: K/V projected once per prompt (the reference repeats the context per frame, :321-325)
         const std::string ap = p + ".attn2";
         Tok q = ln_linear(c, x, p + ".norm2", ap + ".to_q", prm(c, ap + ".to_q.weight"), nullptr, C, nullptr);
         Tok ctx_tok;
         ctx_tok.p = c.ctx;
-        ctx_tok.rows = static_cast<long long>(c.B) * c.L;
+        ctx_tok.rows = static_cast<long long>(c.Bc) * c.L;
         ctx_tok.C = c.u->cfg.context_dim;
         ctx_tok.ld = ctx_tok.C;
         const __half* wkv = w_cat(c, {ap + ".to_k.weight", ap + ".to_v.weight"});
@@ -732,7 +735,7 @@ Tok stt_block(Ctx& c, const Tok& xin, const Blk& blk, int hcur, int wcur) {
         a.q_bs = P * q.ld; a.q_ss = q.ld;
         a.k_bs = a.v_bs = static_cast<long long>(c.L) * kv.ld;
         a.k_ss = a.v_ss = kv.ld;
-        a.kv_batch_div = c.F;
+        a.kv_batch_div = c.F * (c.B / c.Bc);
         a.o_bs = P * o.ld; a.o_ss = o.ld;
         c.b->step([a](cudaStream_t s) { return attention(a, s); }, 1, STEP_ATTN,
                   4.0 * a.batch * a.heads * static_cast<double>(a.sq) * a.skv * d, "attn cross (vc)");
@@ -786,8 +789,9 @@ int n_feature_blocks(const t2v_unet* u) {
     return n;
 }
 
-// feats_B > 0: the plan variant with adapter features (VideoCrafter only), staged for feats_B samples
-int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, int B, int F, int h, int w, int L,
+// feats_B > 0: the plan variant with adapter features (VideoCrafter only), staged for feats_B samples.
+// Bc: context batch (B % Bc == 0), the prompts staged and projected for the cross-attentions.
+int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, int B, int Bc, int F, int h, int w, int L,
           IO* io, int feats_B = 0) {
     Builder bld(plan, arena, dry, num_sms());
     Ctx c;
@@ -796,7 +800,7 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     c.stream = stream;
     c.gn_ws = u->gn_ws.ptr;
     c.u = u;
-    c.B = B; c.F = F; c.h = h; c.w = w; c.L = L;
+    c.B = B; c.Bc = Bc; c.F = F; c.h = h; c.w = w; c.L = L;
     c.emb = nullptr; c.ctx = nullptr; c.plan = plan;
     c.Fl = F; c.rank = 0; c.nranks = 1; c.slab = plan->slab;
     const bool sharded = u->shard_on && plan->shard != nullptr;
@@ -822,7 +826,7 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     Tok x0 = bld.alloc(R0, cin_pad);
     io->x_tok = x0.p;
     io->t = reinterpret_cast<float*>(bld.alloc_bytes(static_cast<size_t>(B) * sizeof(float)));
-    Tok ctx_tok = bld.alloc(static_cast<long long>(B) * L, cfg.context_dim);
+    Tok ctx_tok = bld.alloc(static_cast<long long>(Bc) * L, cfg.context_dim);
     c.ctx = ctx_tok.p;
     io->ctx = ctx_tok.p;
     io->n_feat = 0;
@@ -966,15 +970,19 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     return bld.error;
 }
 
-// The plan-cache key of a forward shape.  The adapter-feature variant adds its feature batch (a forward without features
-// keeps its plan and key).
-std::string plan_key(const t2v_unet* u, int B, int F, int h, int w, int L, int feats_B) {
-    char key[112];
+// The plan-cache key of a forward shape.  The adapter-feature variant adds its feature batch and a shared context its
+// context batch Bc < B (a forward without features, one prompt per sample, keeps its plan and key).
+std::string plan_key(const t2v_unet* u, int B, int Bc, int F, int h, int w, int L, int feats_B) {
+    char key[128];
     snprintf(key, sizeof(key), "%d,%d,%d,%d,%d,%d,%d/%d", B, F, h, w, L, u->taps_enabled ? 1 : 0, u->shard_on ? u->peers.rank : 0,
              u->shard_on ? u->peers.nranks : 1);
     if (feats_B > 0) {
         const size_t n = strlen(key);
         snprintf(key + n, sizeof(key) - n, ",a%d", feats_B);
+    }
+    if (Bc != B) {
+        const size_t n = strlen(key);
+        snprintf(key + n, sizeof(key) - n, ",c%d", Bc);
     }
     return key;
 }
@@ -988,8 +996,8 @@ std::shared_ptr<PlanShard> new_plan_shard(const t2v_unet* u, int F) {
     return s;
 }
 
-PlanCache<IO>::Entry* get_plan(t2v_unet* u, int B, int F, int h, int w, int L, cudaStream_t stream, int feats_B = 0) {
-    const std::string key = plan_key(u, B, F, h, w, L, feats_B);
+PlanCache<IO>::Entry* get_plan(t2v_unet* u, int B, int Bc, int F, int h, int w, int L, cudaStream_t stream, int feats_B = 0) {
+    const std::string key = plan_key(u, B, Bc, F, h, w, L, feats_B);
     if (auto* e = u->plans.find(key, u->params.version())) return e;
     if (!u->params.complete("UNet")) return nullptr;
     // groupnorm workspace: the largest (rows_per_inst, n_inst) pair is the per-sample 5-D norm at level 0
@@ -1014,7 +1022,7 @@ PlanCache<IO>::Entry* get_plan(t2v_unet* u, int B, int F, int h, int w, int L, c
     shell->shard = new_plan_shard(u, F);
     return u->plans.build(key, u->params.version(), stream, std::move(shell),
                           u->taps_enabled || getenv("T2V_ARENA_NO_REUSE") != nullptr, "UNet",
-                          [&](Plan* p, Arena* a, bool dry, IO* io) { return build(u, p, a, dry, stream, B, F, h, w, L, io, feats_B); });
+                          [&](Plan* p, Arena* a, bool dry, IO* io) { return build(u, p, a, dry, stream, B, Bc, F, h, w, L, io, feats_B); });
 }
 
 // A tap of the most recently used plan: (tokens, (h, w)); null, with the error set, if that plan has no such tap.
@@ -1083,13 +1091,25 @@ int t2v_unet_param_info(t2v_unet* u, int index, char* name_out, size_t name_cap,
 namespace t2v {
 namespace {
 
-int unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, const void* const* feats, int feats_B,
-                 void* out, int out_is_f32, int B, int F, int h, int w, int L, cudaStream_t stream) {
+int check_ctx_batch(const t2v_unet* u, int B, int ctx_B) {
+    if (ctx_B < 1 || B < 1 || B % ctx_B != 0) {
+        set_error("context batch %d does not divide the forward batch %d", ctx_B, B);
+        return -2;
+    }
+    if (u->shard_on && ctx_B != B) {
+        set_error("a shared context batch (%d prompts for %d samples) is not built for the frame-sharded denoiser", ctx_B, B);
+        return -2;
+    }
+    return 0;
+}
+
+int unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, int ctx_B, const void* const* feats,
+                 int feats_B, void* out, int out_is_f32, int B, int F, int h, int w, int L, cudaStream_t stream) {
     if (u->cfg.arch == 1 && F > 32) {
         set_error("VideoCrafter temporal attention kernel: at most 32 frames per clip (got %d)", F);
         return -4;
     }
-    auto* entry = get_plan(u, B, F, h, w, L, stream, feats_B);
+    auto* entry = get_plan(u, B, ctx_B, F, h, w, L, stream, feats_B);
     if (!entry) return -1;
     Plan* plan = entry->plan.get();
     const IO& io = entry->io;
@@ -1107,7 +1127,7 @@ int unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const
     int rc = ingest_latent(x, x_is_f32, io.x_tok, cin_pad, cin_pad, B, cfg.in_dim, F, h, w, 1.0f, stream);
     if (rc != 0) return rc;
     cudaMemcpyAsync(io.t, t, sizeof(float) * B, cudaMemcpyDeviceToDevice, stream);
-    cudaMemcpyAsync(io.ctx, ctx, static_cast<size_t>(B) * L * cfg.context_dim * sizeof(__half), cudaMemcpyDeviceToDevice,
+    cudaMemcpyAsync(io.ctx, ctx, static_cast<size_t>(ctx_B) * L * cfg.context_dim * sizeof(__half), cudaMemcpyDeviceToDevice,
                     stream);
     for (int i = 0; i < io.n_feat; ++i)
         cudaMemcpyAsync(io.feat[i], feats[i], static_cast<size_t>(io.feat_elems[i]) * sizeof(__half), cudaMemcpyDeviceToDevice, stream);
@@ -1130,7 +1150,15 @@ extern "C" {
 int t2v_unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, void* out,
                      int out_is_f32, int B, int F, int h, int w, int L, void* stream_) {
     clear_pending_error("t2v_unet_forward");
-    return unet_forward(u, x, x_is_f32, t, ctx, nullptr, 0, out, out_is_f32, B, F, h, w, L, reinterpret_cast<cudaStream_t>(stream_));
+    return unet_forward(u, x, x_is_f32, t, ctx, B, nullptr, 0, out, out_is_f32, B, F, h, w, L, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+int t2v_unet_forward_ctx(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx, int ctx_B, void* out,
+                         int out_is_f32, int B, int F, int h, int w, int L, void* stream_) {
+    clear_pending_error("t2v_unet_forward_ctx");
+    if (const int rc = check_ctx_batch(u, B, ctx_B)) return rc;
+    return unet_forward(u, x, x_is_f32, t, ctx, ctx_B, nullptr, 0, out, out_is_f32, B, F, h, w, L,
+                        reinterpret_cast<cudaStream_t>(stream_));
 }
 
 int t2v_unet_forward_adapter(t2v_unet* u, const void* x, int x_is_f32, const float* t, const void* ctx,
@@ -1160,24 +1188,31 @@ int t2v_unet_forward_adapter(t2v_unet* u, const void* x, int x_is_f32, const flo
             set_error("adapter features: feature %d is a null pointer", i);
             return -2;
         }
-    return unet_forward(u, x, x_is_f32, t, ctx, feats, feats_B, out, out_is_f32, B, F, h, w, L, reinterpret_cast<cudaStream_t>(stream_));
+    return unet_forward(u, x, x_is_f32, t, ctx, B, feats, feats_B, out, out_is_f32, B, F, h, w, L, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 double t2v_unet_flops(t2v_unet* u, int B, int F, int h, int w, int L) {
     IO io;
     double flops = 0.0;
     // a sharded denoiser counts this rank's share of the clip's work
-    if (dry_build(new_plan_shard(u, F), false, [&](Plan* p, Arena* a, bool dry) { return build(u, p, a, dry, nullptr, B, F, h, w, L, &io); },
+    if (dry_build(new_plan_shard(u, F), false, [&](Plan* p, Arena* a, bool dry) { return build(u, p, a, dry, nullptr, B, B, F, h, w, L, &io); },
                   &flops) < 0)
         return -1.0;
     return flops;
 }
 
 int t2v_unet_plan_bytes(t2v_unet* u, int B, int F, int h, int w, int L, size_t* arena) {
+    return t2v_unet_plan_info(u, B, B, F, h, w, L, arena, nullptr, nullptr);
+}
+
+int t2v_unet_plan_info(t2v_unet* u, int B, int ctx_B, int F, int h, int w, int L, size_t* arena, double* flops, int* cached) {
     if (!u || !arena) return -1;
+    if (const int rc = check_ctx_batch(u, B, ctx_B)) return rc;
+    if (cached) *cached = u->plans.holds(plan_key(u, B, ctx_B, F, h, w, L, 0), u->params.version()) ? 1 : 0;
     IO io;
-    const long long peak =
-        dry_build(new_plan_shard(u, F), false, [&](Plan* p, Arena* a, bool dry) { return build(u, p, a, dry, nullptr, B, F, h, w, L, &io); });
+    const long long peak = dry_build(
+        new_plan_shard(u, F), false, [&](Plan* p, Arena* a, bool dry) { return build(u, p, a, dry, nullptr, B, ctx_B, F, h, w, L, &io); },
+        flops);
     if (peak < 0) return -1;
     *arena = plan_slab_bytes(peak);
     return 0;
@@ -1187,7 +1222,7 @@ int t2v_unet_num_launches(t2v_unet* u) { return u->last_launches; }
 
 int t2v_unet_profile(t2v_unet* u, int B, int F, int h, int w, int L, void* stream_, double* out13) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    auto* entry = get_plan(u, B, F, h, w, L, stream);
+    auto* entry = get_plan(u, B, B, F, h, w, L, stream);
     if (!entry) return -1;
     return profile_plan(entry->plan.get(), stream, out13);
 }
@@ -1222,7 +1257,7 @@ int t2v_unet_shard_prepare(t2v_unet* u, int B, int F, int h, int w, int L, void*
         set_error("shard_prepare: call t2v_unet_shard_setup first");
         return -1;
     }
-    auto* entry = get_plan(u, B, F, h, w, L, stream);
+    auto* entry = get_plan(u, B, B, F, h, w, L, stream);
     if (!entry) return -1;
     Plan* plan = entry->plan.get();
     memset(out, 0, sizeof(*out));
@@ -1248,7 +1283,7 @@ int t2v_unet_shard_connect(t2v_unet* u, int B, int F, int h, int w, int L, const
         set_error("shard_connect: call t2v_unet_shard_setup / t2v_unet_shard_prepare first");
         return -1;
     }
-    auto* entry = get_plan(u, B, F, h, w, L, stream);
+    auto* entry = get_plan(u, B, B, F, h, w, L, stream);
     if (!entry) return -1;
     Plan* plan = entry->plan.get();
     PlanShard* ps = plan->shard.get();
@@ -1292,7 +1327,7 @@ int t2v_unet_shard_connect(t2v_unet* u, int B, int F, int h, int w, int L, const
 
 int t2v_unet_shard_connected(t2v_unet* u, int B, int F, int h, int w, int L) {
     if (!u->shard_on) return 0;
-    auto* entry = u->plans.find(plan_key(u, B, F, h, w, L, 0), u->params.version());
+    auto* entry = u->plans.find(plan_key(u, B, B, F, h, w, L, 0), u->params.version());
     return (entry && entry->plan->shard && entry->plan->shard->connected) ? 1 : 0;
 }
 

@@ -24,9 +24,12 @@ SIGNATURES = {
     't2v_unet_missing_params': (c_int, [P, c_char_p, C.c_size_t]),
     't2v_unet_param_info': (c_int, [P, c_int, c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(c_int)]),
     't2v_unet_forward': (c_int, [P, P, c_int, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
+    't2v_unet_forward_ctx': (c_int, [P, P, c_int, P, P, c_int, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     't2v_unet_forward_adapter': (c_int, [P, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     't2v_unet_flops': (c_double, [P, c_int, c_int, c_int, c_int, c_int]),
     't2v_unet_plan_bytes': (c_int, [P, c_int, c_int, c_int, c_int, c_int, C.POINTER(C.c_size_t)]),
+    't2v_unet_plan_info': (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(C.c_size_t), C.POINTER(c_double),
+                                   C.POINTER(c_int)]),
     't2v_unet_num_launches': (c_int, [P]),
     't2v_unet_profile': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, C.POINTER(c_double)]),
     't2v_unet_read_tap': (c_ll, [P, c_char_p, P, c_ll, P]),

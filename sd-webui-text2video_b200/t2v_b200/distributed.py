@@ -137,10 +137,15 @@ def frame_bounds(F, world_size):
 
 
 def step_noise(like):
-    """Per-step sampler noise (eta > 0).  Frame-sharded: every rank draws the FULL clip's noise from its (identically seeded)
-    CUDA generator and keeps its frames, so the result does not depend on the number of ranks."""
+    """Per-step sampler noise (eta > 0).  A batch of n clips draws one clip-sized tensor per clip, in clip order, from the
+    global CUDA generator: a batched run consumes it step-major (step s of clips 0..n-1, then step s + 1), n sequential runs
+    clip-major, so the two give different per-step noise from the same generator state.
+    Frame-sharded: every rank draws the FULL clip's noise from its (identically seeded) CUDA generator and keeps its frames,
+    so the result does not depend on the number of ranks."""
     fs = _frame_shard
     if fs is None:
+        if like.shape[0] > 1:
+            return pair_shared(torch.cat([torch.randn_like(like[i:i + 1]) for i in range(like.shape[0])], dim=0))
         return pair_shared(torch.randn_like(like))
     full = torch.randn((like.shape[0], like.shape[1], fs.F) + tuple(like.shape[3:]), device=like.device, dtype=like.dtype)
     return full[:, :, fs.f0:fs.f1].contiguous()

@@ -309,6 +309,9 @@ class UNetSD(_NativeModule):
     @torch.no_grad()
     def forward(self, x, t, y, F_total=None, **ignored):
         """eps = UNetSD(x, t, y).  Returns fp16 [B, out_dim, F, h, w] (what the reference returns under autocast).
+        y may hold fewer prompts than x holds samples: with Bc = y.shape[0] dividing B, sample j reads y[j // (B // Bc)]
+        (n clips guided as one batch: x = [x; x], y = [c; uc]).  1 < Bc < B projects each prompt's K/V once per forward
+        (t2v_unet_forward_ctx); Bc = 1 is repeated to B as before.
         Frame-sharded (after shard_setup): x holds this rank's frames of an `F_total`-frame clip, so does the result."""
         if x.dim() != 5:
             raise ValueError('x must be [B, C, F, h, w]')
@@ -328,14 +331,18 @@ class UNetSD(_NativeModule):
         if getattr(self, '_shard', None) is not None:
             self._shard_connect(B, F_total, h, w, y.shape[1])
             F = F_total
-        rc = l.t2v_unet_forward(self._handle, _lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(t), _lib.ptr(y),
-                                _lib.ptr(out), 0, B, F, h, w, y.shape[1], _lib.stream_ptr())
+        if y.shape[0] == B:
+            rc = l.t2v_unet_forward(self._handle, _lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(t), _lib.ptr(y),
+                                    _lib.ptr(out), 0, B, F, h, w, y.shape[1], _lib.stream_ptr())
+        else:
+            rc = l.t2v_unet_forward_ctx(self._handle, _lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(t), _lib.ptr(y),
+                                        y.shape[0], _lib.ptr(out), 0, B, F, h, w, y.shape[1], _lib.stream_ptr())
         _lib.check(rc, 'unet_forward')
         return out
 
     def _stage(self, x, t, y):
-        """The library's forward inputs: x fp16 / fp32 contiguous, t fp32 [B], y fp16 [B, L, context_dim] (t and y of batch
-        1 broadcast to B), and the fp16 eps output [B, out_dim, F, h, w] to write."""
+        """The library's forward inputs: x fp16 / fp32 contiguous, t fp32 [B], y fp16 [Bc, L, context_dim] (t and y of batch
+        1 broadcast to B; any other Bc must divide B), and the fp16 eps output [B, out_dim, F, h, w] to write."""
         B, _, F, h, w = x.shape
         if x.dtype not in (torch.float32, torch.float16):
             x = x.float()
@@ -348,6 +355,8 @@ class UNetSD(_NativeModule):
         if y.shape[0] == 1 and B > 1:
             y = y.expand(B, -1, -1)
         y = y.contiguous()
+        if B % y.shape[0] != 0:
+            raise ValueError(f'{y.shape[0]} prompts do not divide a batch of {B} samples')
         if y.shape[2] != self.context_dim:
             raise ValueError(f'context dim {y.shape[2]} != {self.context_dim}')
         return x, t, y, torch.empty((B, self.out_dim, F, h, w), device=x.device, dtype=torch.float16)
@@ -361,6 +370,14 @@ class UNetSD(_NativeModule):
         arena = C.c_size_t(0)
         _lib.check(_lib.load_library().t2v_unet_plan_bytes(self._handle, B, F, h, w, L, C.byref(arena)), 'unet_plan_bytes')
         return arena.value
+
+    def plan_info(self, B, F, h, w, L=77, ctx_batch=None):
+        """(activation-arena bytes, flop, cached) of the plan of a forward with `ctx_batch` prompts for B samples (default B):
+        the host-only dry pass, and whether this denoiser holds that plan already."""
+        arena, fl, cached = C.c_size_t(0), C.c_double(0.0), C.c_int(0)
+        _lib.check(_lib.load_library().t2v_unet_plan_info(self._handle, B, B if ctx_batch is None else ctx_batch, F, h, w, L,
+                                                          C.byref(arena), C.byref(fl), C.byref(cached)), 'unet_plan_info')
+        return arena.value, fl.value, bool(cached.value)
 
     def num_launches(self):
         return _lib.load_library().t2v_unet_num_launches(self._handle)
@@ -492,6 +509,8 @@ class UNetModel(UNetSD):
         self.sync_weights()
         l = _lib.lib()
         x, t, y, out = self._stage(x, t, context)
+        if y.shape[0] != B:                      # the adapter entry takes one prompt per sample
+            y = y.repeat_interleave(B // y.shape[0], dim=0)
         ptrs = (C.c_void_p * len(staged))(*[s.data_ptr() for s in staged])
         rc = l.t2v_unet_forward_adapter(self._handle, _lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(t), _lib.ptr(y), ptrs,
                                         len(staged), fb, _lib.ptr(out), 0, B, T, h, w, y.shape[1], _lib.stream_ptr())

@@ -3,8 +3,8 @@
 
 Same public surface: `TextToVideoSynthesis(model_dir)`, attributes `.sd_model .autoencoder .clip_encoder .diffusion
 .model_dir .keep_in_vram`, and `infer(prompt, n_prompt, steps, frames, seed, scale, width, height, eta, cpu_vae,
-device, latents, skip_steps, strength, mask, is_vid2vid, sampler) -> (list of HxWx3 uint8 BGR frames, last latent,
-infotext)`.
+device, latents, skip_steps, strength, mask, is_vid2vid, sampler, batch_size=1) -> (list of HxWx3 uint8 BGR frames, last
+latent, infotext)`; with batch_size = n > 1 each of the three is a list of n, clip i seeded seed + i.
 
 Differences that are the point of this repo:
   * UNet + samplers + VAE run through libt2v_b200.so (no autocast, no PyTorch kernels on the hot path);
@@ -20,10 +20,23 @@ import random
 import numpy as np
 import torch
 
+from . import distributed as _dist
 from .modules import UNetSD, AutoencoderKL
 from .samplers import Txt2VideoSampler, available_samplers
 
 SCALE_FACTOR = 0.18215          # t2v_pipeline.py:321
+BUDGET_MARGIN = 512 << 20       # what a plan build allocates outside its arena (the VAE's rule, DESIGN.md section 2)
+
+
+def batch_groups(n, fits):
+    """Splits n clips into consecutive groups of the largest size k <= n with fits(k) (the B = 2k plan fits the memory
+    budget), the last group the remainder.  [] if not even one clip fits."""
+    k = n
+    while k > 0 and not fits(k):
+        k -= 1
+    if k == 0:
+        return []
+    return [k] * (n // k) + ([n % k] if n % k else [])
 
 VAE_DDCONFIG = {'double_z': True, 'z_channels': 4, 'resolution': 256, 'in_channels': 3, 'out_ch': 3, 'ch': 128,
                 'ch_mult': [1, 2, 4, 4], 'num_res_blocks': 2, 'attn_resolutions': [], 'dropout': 0.0}   # :117-128
@@ -93,6 +106,9 @@ class TextToVideoSynthesis(object):
         self.noise_gen = torch.Generator(device='cpu')
         self.last_tensor = None
         self.frame_shard = None
+        # batch_size > 1: bytes of denoiser plan (activation arena) a batch may add; 0 = automatic: free device memory - 512 MB
+        self.batch_memory_budget = 0
+        self.last_batch_groups = None           # clips per B = 2k forward of the last batched infer()
 
     def enable_frame_shard(self, group=None):
         """ONE clip over the ranks of `group` (BASELINE config 4): every rank calls infer() with the same arguments and gets
@@ -113,13 +129,39 @@ class TextToVideoSynthesis(object):
         return enc(prompt), enc(n_prompt)
 
     # ------------------------------------------------------------------------------------------ entry
+    def plan_groups(self, n, frames, height, width, L):
+        """How n clips of one batched infer() are grouped: the largest k whose B = 2k denoiser plan (context batch 2, host
+        dry pass) fits the budget runs first, as many times as it fits, then the remainder.  A cached plan needs no new
+        memory.  Raises if a single clip's B = 2 plan does not fit."""
+        budget = self.batch_memory_budget or max(torch.cuda.mem_get_info(self.device)[0] - BUDGET_MARGIN, 0)
+        h, w = height // 8, width // 8
+        need = {}
+
+        def fits(k):
+            arena, _, cached = self.sd_model.plan_info(2 * k, frames, h, w, L, ctx_batch=2)
+            need[k] = 0 if cached else arena
+            return need[k] <= budget
+        groups = batch_groups(n, fits)
+        if not groups:
+            raise RuntimeError(f'batch of {n} clips of {frames} x {height} x {width}: one clip\'s B = 2 denoiser plan needs '
+                               f'{need[1] / 1e9:.2f} GB, more than the memory budget of {budget / 1e9:.2f} GB')
+        return groups
+
     @torch.no_grad()
     def infer(self, prompt, n_prompt, steps, frames, seed, scale, width=256, height=256, eta=0.0,
               cpu_vae='GPU (half precision)', device=None, latents=None, skip_steps=0, strength=0, mask=None,
-              is_vid2vid=False, sampler=available_samplers[0].name):
+              is_vid2vid=False, sampler=available_samplers[0].name, batch_size=1):
         if 'CPU' in str(cpu_vae):
             raise RuntimeError('the CPU VAE mode of the reference does not exist here: t2v_b200 has no CPU path')
+        if batch_size > 1:
+            if self.frame_shard is not None:
+                raise NotImplementedError('batch_size > 1 with a frame-sharded clip: run the clips one after another')
+            if _dist.cfg_split_enabled():
+                raise NotImplementedError('batch_size > 1 in CFG-split mode (T2V_CFG_SPLIT=1): run the clips one after another')
         seed = seed if seed != -1 else random.randint(0, 2 ** 32 - 1)
+        if batch_size > 1:
+            return self._infer_batch(prompt, n_prompt, steps, frames, seed, scale, width, height, eta, cpu_vae, latents,
+                                     skip_steps, strength, mask, is_vid2vid, sampler, batch_size)
         vars_ = {'steps': steps, 'frames': frames, 'seed': seed, 'scale': scale, 'width': width, 'height': height,
                  'eta': eta, 'sampler': sampler}
         steps = steps - skip_steps
@@ -159,6 +201,50 @@ class TextToVideoSynthesis(object):
         rgb = host.numpy()
         video = [np.ascontiguousarray(f[:, :, ::-1]) for f in rgb]       # cv2.COLOR_RGB2BGR (t2v_pipeline.py:431-434)
         return video, self.last_tensor, create_infotext(prompt, n_prompt, vars_)
+
+    def _infer_batch(self, prompt, n_prompt, steps, frames, seed, scale, width, height, eta, cpu_vae, latents, skip_steps,
+                     strength, mask, is_vid2vid, sampler, n):
+        """infer() of n clips seeded seed, seed + 1, ...: each step guides a group of k clips with ONE B = 2k forward, and
+        the VAE decodes all n * frames frames in one call.  Start latents (vid2vid / img2vid): one per clip ([n, ...]), or
+        one of batch 1 shared by the clips."""
+        seeds = [seed + i for i in range(n)]
+        steps_total = steps
+        steps = steps - skip_steps
+        c, uc = self.preprocess(prompt, n_prompt, steps)
+        strength = None if (strength == 0.0 and not is_vid2vid) else strength
+        if latents is not None:
+            latents = latents.to(self.device)
+            if 'half precision' in str(cpu_vae):
+                latents = latents.half()
+        groups = self.plan_groups(n, frames, height, width, c.shape[1])
+        self.last_batch_groups = groups
+        outs, first = [], 0
+        if latents is not None and latents.shape[0] not in (1, n):
+            raise ValueError(f'{n} clips take start latents of batch 1 or {n}, got {tuple(latents.shape)}')
+        for k in groups:
+            lat = latents[first:first + k] if latents is not None and latents.shape[0] == n else latents
+            mask_k = mask[first:first + k] if mask is not None and mask.shape[0] == n else mask
+            lat_k, noise, shape = self.diffusion.get_noise(k, 4, frames, height, width, latents=lat,
+                                                           seeds=seeds[first:first + k])
+            # a fresh sampler per group, as per infer(): encode_latent rebinds DDIM's .sample for vid2vid
+            self.diffusion.get_sampler(sampler, return_sampler=False)
+            outs.append(self.diffusion.sample_loop(steps=steps, strength=strength, eta=eta, conditioning=c,
+                                                   unconditional_conditioning=uc, batch_size=k, guidance_scale=scale,
+                                                   latents=lat_k, shape=shape, noise=noise, is_vid2vid=is_vid2vid,
+                                                   sampler_name=sampler, mask=mask_k))
+            first += k
+        x0 = torch.cat(outs, dim=0)
+        self.last_tensor = x0
+        frames_u8 = self.autoencoder.decode_video(x0, 1.0 / SCALE_FACTOR, as_uint8=True)        # [n * F, H, W, 3] RGB
+        host = torch.empty(frames_u8.shape, dtype=torch.uint8, pin_memory=True)
+        host.copy_(frames_u8, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        rgb = host.numpy()
+        videos = [[np.ascontiguousarray(f[:, :, ::-1]) for f in rgb[i * frames:(i + 1) * frames]] for i in range(n)]
+        infos = [create_infotext(prompt, n_prompt, {'steps': steps_total, 'frames': frames, 'seed': s, 'scale': scale,
+                                                    'width': width, 'height': height, 'eta': eta, 'sampler': sampler})
+                 for s in seeds]
+        return videos, [x0[i:i + 1] for i in range(n)], infos
 
     @torch.no_grad()
     def compute_latents(self, vd_out, cpu_vae='GPU (half precision)', device=None):

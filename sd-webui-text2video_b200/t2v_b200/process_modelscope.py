@@ -10,6 +10,10 @@ Out of scope by SURVEY.md section 2 rows 5/12: reading / resizing input FILES wi
 image are passed as tensors) and the LoRA UI.  Packaging: `video_encoder(frames, args) -> str` is pluggable (the webui's
 ffmpeg_stitch_video wrapper); the default (video_encode.py) pipes through an `ffmpeg` binary when one exists and otherwise
 returns an uncompressed AVI data URL.  `return_frames=True` in `args_dict` returns the raw BGR frame lists instead.
+`batch_size` (default 1) groups the `batch_count` clips into batches of that many, each sampled as one batched run
+(`infer(batch_size=...)`, clip i of a batch still seeded seed + i).  The encoded vid2vid video is shared by the clips of a
+batch (each clip noises it with its own x_T); img2vid blends one start latent per clip, in clip order, as the sequential
+loop does.
 """
 import ctypes as C
 from types import SimpleNamespace
@@ -26,7 +30,7 @@ pipe = None
 video_encoder = default_video_encoder        # callable(list_of_bgr_frames, args) -> str (data URL)
 
 _DEFAULTS = dict(prompt='', n_prompt='', steps=30, frames=24, seed=-1, cfg_scale=17, width=256, height=256, eta=0.0,
-                 batch_count=1, sampler='DDIM_Gaussian', cpu_vae='GPU (half precision)', keep_pipe_in_vram='None',
+                 batch_count=1, batch_size=1, sampler='DDIM_Gaussian', cpu_vae='GPU (half precision)', keep_pipe_in_vram='None',
                  do_vid2vid=False, model='<modelscope>', inpainting_frames=0,
                  inpainting_weights='0:(t/max_i_f), "max_i_f":(1)')          # T2VArgs defaults (t2v_helpers/args.py:219-236)
 
@@ -86,17 +90,26 @@ def process_modelscope(args_dict, extra_args=None):
         skip_steps = int(np.floor(a.steps * max(0, min(1 - strength, 1))))                                                  # :143
     else:
         strength = 1                                                                                                       # :146
-    for batch in range(a.batch_count):
+    keep_frames = getattr(a, 'return_frames', False) or video_encoder is None
+    for batch, n in batch_sizes(a.batch_count, a.batch_size):
         seed = a.seed + batch if a.seed != -1 else -1
         latents, mask = vid_latents, None
         image = getattr(a, 'inpainting_image_tensor', None)
         if a.inpainting_frames > 0 and image is not None:                                                                  # :170-219
-            latents, mask = inpainting_latents(pipe, image, a.frames, a.height, a.width, a.inpainting_frames, a.inpainting_weights,
-                                               a.seed, a.cpu_vae, getattr(a, 'inpainting_noise', None))
+            # the blended latent IS the clip's x_T: one per clip, drawn in clip order as the sequential loop draws them
+            blends = [inpainting_latents(pipe, image, a.frames, a.height, a.width, a.inpainting_frames, a.inpainting_weights,
+                                         a.seed, a.cpu_vae, getattr(a, 'inpainting_noise', None)) for _ in range(n)]
+            latents, mask = torch.cat([b[0] for b in blends]), torch.cat([b[1] for b in blends])
             strength = 1
-        frames, _, info = pipe.infer(prompt, n_prompt, a.steps, a.frames, seed, a.cfg_scale, a.width, a.height, a.eta,
-                                     a.cpu_vae, torch.device('cuda'), latents, skip_steps, strength, mask,
-                                     bool(getattr(a, 'do_vid2vid', False)), a.sampler)
-        keep_frames = getattr(a, 'return_frames', False) or video_encoder is None
-        outputs.append(frames if keep_frames else video_encoder(frames, a))
+        args = (prompt, n_prompt, a.steps, a.frames, seed, a.cfg_scale, a.width, a.height, a.eta, a.cpu_vae, torch.device('cuda'),
+                latents, skip_steps, strength, mask, bool(getattr(a, 'do_vid2vid', False)), a.sampler)
+        clips = [pipe.infer(*args)[0]] if n == 1 else pipe.infer(*args, batch_size=n)[0]
+        outputs.extend(frames if keep_frames else video_encoder(frames, a) for frames in clips)
     return outputs
+
+
+def batch_sizes(batch_count, batch_size):
+    """[(index of the batch's first clip, clips in it)]: `batch_count` clips in batches of `batch_size`, the last the rest."""
+    if batch_size < 1:
+        raise ValueError(f'batch_size must be >= 1, got {batch_size}')
+    return [(i, min(batch_size, batch_count - i)) for i in range(0, batch_count, batch_size)]

@@ -61,17 +61,19 @@ def _f32(v):
 
 
 def _eval_pair(model, x, t, c, uc):
-    """(eps_cond, eps_uncond).  One B=2 forward for our UNetSD with a single-sample latent, else two calls; in CFG-split
-    mode (distributed.py) this rank evaluates ONE branch and the pair exchanges the results."""
+    """(eps_cond, eps_uncond).  One forward for our UNetSD: B = 2 for a single-sample latent, and for n clips
+    (x [n, ...], one prompt pair) B = 2n of [x; x] with the context batch [c; uc] shared by each half, so every prompt's
+    K/V is projected once.  Anything else makes two calls; in CFG-split mode (distributed.py) this rank evaluates ONE
+    branch and the pair exchanges the results."""
     if _dist.cfg_split_enabled():
         _, role, grp = _dist.cfg_pair()
         return _dist.exchange_eps(model(x, t, c if role == 0 else uc), grp)
-    if isinstance(model, UNetSD) and x.shape[0] == 1 and torch.is_tensor(c) and torch.is_tensor(uc) \
-            and c.shape == uc.shape:
-        xb = x.expand(2, *x.shape[1:])
-        tb = torch.as_tensor(t, device=x.device).reshape(-1)[:1].expand(2)
+    if isinstance(model, UNetSD) and torch.is_tensor(c) and torch.is_tensor(uc) and c.shape == uc.shape and c.shape[0] == 1:
+        n = x.shape[0]
+        xb = x.expand(2, *x.shape[1:]) if n == 1 else torch.cat([x, x], dim=0)
+        tb = torch.as_tensor(t, device=x.device).reshape(-1)[:1].expand(2 * n)
         out = model(xb, tb, torch.cat([c, uc], dim=0))
-        return out[0:1], out[1:2]
+        return out[:n], out[n:]
     return model(x, t, c), model(x, t, uc)
 
 
@@ -468,12 +470,25 @@ class Txt2VideoSampler(object):
         self.sampler_name = sampler_name
         self.sampler = self.get_sampler(sampler_name, betas=self.betas)
 
-    def get_noise(self, num_sample, channels, frames, height, width, latents=None, seed=1):
-        """x_T from a CPU generator seeded per run, batch forced to 1 (samplers_common.py:104-121)."""
+    def get_noise(self, num_sample, channels, frames, height, width, latents=None, seed=1, seeds=None):
+        """x_T from a CPU generator seeded per run, batch forced to 1 (samplers_common.py:104-121).
+        `seeds`: one clip per seed, stacked to a batch of len(seeds); clip i is drawn exactly as a run with seed=seeds[i]
+        draws it.  `latents` (vid2vid / img2vid) hold one start latent per clip, or one of batch 1 shared by the clips."""
         shape = (1, channels, frames, height // 8, width // 8) if latents is None else tuple(latents.shape)
-        self.noise_gen.manual_seed(seed)
-        noise = torch.randn(shape, generator=self.noise_gen).to(self.device)
-        return latents, noise, shape
+        if seeds is None:
+            self.noise_gen.manual_seed(seed)
+            noise = torch.randn(shape, generator=self.noise_gen).to(self.device)
+            return latents, noise, shape
+        if shape[0] not in (1, len(seeds)):
+            raise ValueError(f'{len(seeds)} clips take start latents of batch 1 or {len(seeds)}, got {tuple(shape)}')
+        draws = []
+        for s in seeds:
+            self.noise_gen.manual_seed(s)
+            draws.append(torch.randn((1,) + shape[1:], generator=self.noise_gen))
+        noise = torch.cat(draws, dim=0).to(self.device)
+        if latents is not None:
+            latents = latents.expand(len(seeds), *shape[1:]).contiguous()
+        return latents, noise, tuple(noise.shape)
 
     def encode_latent(self, latent, noise, strength, steps):
         """vid2vid: noise the encoded input video to the schedule's entry point (samplers_common.py:123-145)."""

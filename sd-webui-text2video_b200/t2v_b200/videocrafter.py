@@ -497,7 +497,8 @@ _DEFAULTS = dict(prompt='', n_prompt='', steps=50, frames=16, seed=-1, cfg_scale
 def process_videocrafter(args_dict, model=None):
     """process_videocrafter.py:13-98: batch loop, `noise_gen.manual_seed(seed + batch)`, `sample_text2video(model, prompt,
     n_prompt, 1, 1, sample_type='ddim', sampler=ddim_sampler, ddim_steps=steps, eta=eta, cfg_scale=cfg_scale,
-    decode_frame_bs=1, num_frames=frames)`.  Checkpoint / yaml discovery under the webui models directory, mp4 writing and
+    decode_frame_bs=1, num_frames=frames)`; `batch_size` in `args_dict` (default 1) replaces both 1s, so each batch samples that
+    many clips together and returns one output per clip.  Checkpoint / yaml discovery under the webui models directory, mp4 writing and
     the data-URL are webui plumbing outside the path: pass `model` (a `LatentDiffusion`) or install one in `model_cache`;
     `prompt_embeds` / `n_prompt_embeds` keys may carry pre-encoded conditioning.
 
@@ -520,12 +521,14 @@ def process_videocrafter(args_dict, model=None):
     prompt = a.prompt if prompt is None else prompt
     n_prompt = a.n_prompt if n_prompt is None else n_prompt
     outputs = []
+    bs = int(getattr(a, 'batch_size', 1))          # clips per sample_text2video call, sampled as one batch
     for batch in range(a.batch_count):
         sampler.noise_gen.manual_seed(a.seed + batch if a.seed != -1 else -1)
-        samples = sample_text2video(model, prompt, n_prompt, 1, 1, sample_type='ddim', sampler=sampler, ddim_steps=a.steps,
+        samples = sample_text2video(model, prompt, n_prompt, bs, bs, sample_type='ddim', sampler=sampler, ddim_steps=a.steps,
                                     eta=a.eta, cfg_scale=a.cfg_scale, decode_frame_bs=1, ddp=False,
                                     show_denoising_progress=False, num_frames=a.frames, x_T=getattr(a, 'x_T', None))
-        outputs.append(video_encoder(samples[0:1], a) if video_encoder is not None else samples[0:1])
+        for i in range(samples.shape[0]):
+            outputs.append(video_encoder(samples[i:i + 1], a) if video_encoder is not None else samples[i:i + 1])
     return outputs
 
 
