@@ -343,6 +343,22 @@ int t2v_q_sample_blend(const float* x0, const long long* x0_strides, const float
                        const float* a, const float* s, const float* mask, const long long* mask_strides, const float* img,
                        float* out, const int* shape, void* stream);
 
+/* vid2vid / img2vid frame preparation (process_modelscope.py:115-137, :172-190): PIL's Image.resize((W, H), Image.LANCZOS)
+ * of n uint8 RGB frames src [n, H0, W0, 3], then the reference's normalisation, as numpy and torch round it op by op:
+ * (float32(x) / 255) * 2 - 1.  out [n, 3, H, W] is fp32, or fp16 (round to nearest of that fp32 value) when out_fp16.
+ * Bit-identical to Pillow: a horizontal pass over the rows the vertical pass reads into tmp, a uint8 buffer of at least
+ * n * H0 * W * 3 bytes (tmp_bytes; unused and may be NULL when W == W0), then the vertical pass; a size that does not
+ * change skips its pass.  src, out and tmp are device pointers.  The coefficient tables are built on the host once per
+ * (in, out) size pair and kept on the device.  Returns -1 without launching when n < 1, a size lies outside [1, 32768],
+ * src or out is NULL, out is not aligned to its element size, or tmp is missing or too small. */
+int t2v_frames_resize(const void* src, int n, int H0, int W0, void* out, int H, int W, int out_fp16, void* tmp,
+                      long long tmp_bytes, void* stream);
+/* Host only: those tables for in_size -> out_size pixels.  *ksize = taps per output pixel: 2 * ceil(3 * max(in / out, 1)) + 1,
+ * or 1 when in == out (the identity, for the pass Pillow skips).  bounds [out_size][2] = (first input pixel, taps used);
+ * coeffs [out_size][*ksize] = int32 weights with 22 fractional bits, 0 past the taps used.  bounds and coeffs may be NULL
+ * (query *ksize first).  Returns -1 when a size lies outside [1, 32768] or ksize is NULL. */
+int t2v_resize_coeffs(int in_size, int out_size, int* ksize, int* bounds, int* coeffs);
+
 /* ------------------------------------------------------------------------------------------ kernel-level entry
  * points (used by the parity tests; the model-level calls above are built from exactly these launchers).   */
 int t2v_op_gemm(const void* a, long long lda, int K, int nd, const int* dims, int ntaps, const int* tap_off,

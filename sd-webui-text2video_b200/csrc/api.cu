@@ -274,6 +274,42 @@ int t2v_q_sample_blend(const float* x0, const long long* x0_strides, const float
     return q_sample_blend(p, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int t2v_resize_coeffs(int in_size, int out_size, int* ksize, int* bounds, int* coeffs) {
+    if (ksize == nullptr || resize_table(in_size, out_size, ksize, bounds, coeffs) != 0) {
+        set_error("resize_coeffs: sizes must lie in [1, %d] (in %d, out %d) and ksize must not be null", kResizeMaxSize, in_size,
+                  out_size);
+        return -1;
+    }
+    return 0;
+}
+
+int t2v_frames_resize(const void* src, int n, int H0, int W0, void* out, int H, int W, int out_fp16, void* tmp,
+                      long long tmp_bytes, void* stream) {
+    const int M = kResizeMaxSize;
+    if (n < 1 || H0 < 1 || W0 < 1 || H < 1 || W < 1 || H0 > M || W0 > M || H > M || W > M) {
+        set_error("frames_resize: n must be >= 1 and every size in [1, %d] (n %d, %dx%d -> %dx%d)", M, n, W0, H0, W, H);
+        return -1;
+    }
+    if (src == nullptr || out == nullptr) {
+        set_error("frames_resize: src and out are required");
+        return -1;
+    }
+    const size_t esize = out_fp16 ? sizeof(__half) : sizeof(float);
+    if (reinterpret_cast<uintptr_t>(out) % esize != 0) {
+        set_error("frames_resize: out must be aligned to its element size (%zu bytes)", esize);
+        return -1;
+    }
+    const long long need = W != W0 ? static_cast<long long>(n) * H0 * W * 3 : 0;
+    if (W != W0 && (tmp == nullptr || tmp_bytes < need)) {
+        set_error("frames_resize: resizing %d to %d columns needs a uint8 buffer of %lld bytes, got %lld", W0, W, need,
+                  tmp ? tmp_bytes : 0LL);
+        return -1;
+    }
+    clear_pending_error("frames_resize");
+    return frames_resize(static_cast<const uint8_t*>(src), n, H0, W0, out, H, W, out_fp16, static_cast<uint8_t*>(tmp),
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
 int t2v_op_pack_conv_weight(const void* src, int src_is_f32, void* dst, int Cout, int Cin, int taps, int n_alloc,
                             int k_alloc, void* stream) {
     return pack_conv_weight(src, src_is_f32, reinterpret_cast<__half*>(dst), Cout, Cin, taps, n_alloc, k_alloc,

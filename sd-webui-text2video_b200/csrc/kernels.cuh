@@ -205,4 +205,16 @@ int lincomb(float* out, const float* const* src, const float* coef, int n_src, l
 int cfg_x0(const float* x, const void* eps_c, const void* eps_u, int eps_is_f32, float* x0, long long n, float g,
            float alpha, float sigma, int cfg_fp16, cudaStream_t stream);
 
+// ---------------------------------------------------------------- resize.cu
+// PIL's Image.resize((W, H), LANCZOS) of uint8 RGB frames followed by the reference's x / 255 * 2 - 1, bit for bit.
+constexpr int kResizeMaxSize = 32768;
+// Pillow's tables for in_size -> out_size pixels (in == out: the identity, one tap): *ksize taps per output, bounds [out][2]
+// (first input pixel, taps used), coeffs [out][*ksize] int32 with 22 fractional bits.  bounds / coeffs may be null.
+// -1 for a size outside [1, kResizeMaxSize].
+int resize_table(int in_size, int out_size, int* ksize, int* bounds, int* coeffs);
+// src [n, H0, W0, 3] uint8 -> out [n, 3, H, W] fp32 (or fp16 when out_fp16), through tmp [n, H0, W, 3] uint8 when W != W0.
+// Arguments are checked by the caller (t2v_frames_resize).
+int frames_resize(const uint8_t* src, int n, int H0, int W0, void* out, int H, int W, int out_fp16, uint8_t* tmp,
+                  cudaStream_t stream);
+
 }  // namespace t2v

@@ -89,6 +89,8 @@ SIGNATURES = {
     't2v_lincomb': (c_int, [P, C.POINTER(P), C.POINTER(c_float), c_int, c_ll, P]),
     't2v_latent_blend': (c_int, [P, c_int, P, P, P, P, c_int, c_int, c_ll, P]),
     't2v_q_sample_blend': (c_int, [P, C.POINTER(c_ll), P, C.POINTER(c_ll), P, P, P, C.POINTER(c_ll), P, P, C.POINTER(c_int), P]),
+    't2v_frames_resize': (c_int, [P, c_int, c_int, c_int, P, c_int, c_int, c_int, P, c_ll, P]),
+    't2v_resize_coeffs': (c_int, [c_int, c_int, C.POINTER(c_int), P, P]),
     't2v_op_gemm': (c_int, [P, c_ll, c_int, c_int, C.POINTER(c_int), c_int, C.POINTER(c_int), P, c_int, c_int, c_int,
                             c_int, P, c_ll, P, c_int, c_ll, P, c_ll, c_float, c_int, c_int, P]),
     't2v_op_gemm_splitk': (c_int, [P, c_ll, c_int, c_int, C.POINTER(c_int), c_int, C.POINTER(c_int), P, c_int, c_int, c_int,

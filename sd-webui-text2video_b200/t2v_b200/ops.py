@@ -6,6 +6,7 @@ All tensors are CUDA fp16, channels-last token matrices [rows, C] unless stated 
 """
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -283,3 +284,82 @@ def attention_relpos(q, k, v, o, table_k, table_v, n_seq, seq_inner, bs_outer, b
                                    max_rel, scale, _lib.stream_ptr())
     _lib.check(rc, 'op_attention_relpos')
     return o
+
+
+def resize_coeffs(in_size, out_size):
+    """t2v_resize_coeffs (host only, no GPU needed): Pillow's LANCZOS tables for in_size -> out_size pixels as numpy int32
+    bounds [out_size, 2] (first input pixel, taps used) and coeffs [out_size, ksize] (22 fractional bits)."""
+    l = _lib.load_library()
+    k = C.c_int(0)
+    _lib.check(l.t2v_resize_coeffs(in_size, out_size, C.byref(k), None, None), 'resize_coeffs')
+    bounds = np.zeros((out_size, 2), dtype=np.int32)
+    coeffs = np.zeros((out_size, k.value), dtype=np.int32)
+    _lib.check(l.t2v_resize_coeffs(in_size, out_size, C.byref(k), bounds.ctypes.data_as(C.c_void_p),
+                                   coeffs.ctypes.data_as(C.c_void_p)), 'resize_coeffs')
+    return bounds, coeffs
+
+
+STAGING_BYTES = 64 << 20      # host frames go to the device in chunks of about this many bytes
+
+
+def frames_resize(frames, width, height, dtype=torch.float32, out=None, staging_bytes=STAGING_BYTES):
+    """PIL's Image.resize((width, height), Image.LANCZOS) of uint8 RGB frames, then the reference's x / 255 * 2 - 1, bit for
+    bit (t2v_frames_resize) -> [n, 3, height, width] fp32 or fp16 on the current device, or into `out` (a contiguous CUDA
+    tensor of that shape and dtype).  `frames`: a uint8 CUDA tensor [n, H0, W0, 3], or host frames -- an array
+    [n, H0, W0, 3] or a sequence of [H0, W0, 3] arrays or RGB PIL images -- copied to the device in chunks of about
+    `staging_bytes` through two pinned buffers, so a long high-resolution clip never has its whole uint8 copy on the device
+    and the host copy of one chunk overlaps the device's work on the previous one."""
+    l = _lib.lib()
+    if dtype not in (torch.float32, torch.float16):
+        raise TypeError(f'frames_resize: dtype must be torch.float32 or torch.float16, got {dtype}')
+    n = len(frames)
+    if n == 0:
+        raise ValueError('frames_resize: no frames')
+    on_device = torch.is_tensor(frames) and frames.is_cuda
+    if on_device:
+        if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+            raise ValueError(f'frames_resize: device frames must be uint8 [n, H, W, 3], got {frames.dtype} {list(frames.shape)}')
+        H0, W0 = frames.shape[1], frames.shape[2]
+    else:
+        H0, W0 = _host_frame(frames[0], None).shape[:2]
+    dev = frames.device if on_device else torch.device('cuda', torch.cuda.current_device())
+    if out is None:
+        out = torch.empty((n, 3, height, width), device=dev, dtype=dtype)
+    if tuple(out.shape) != (n, 3, height, width) or out.dtype != dtype or not out.is_contiguous() or out.device != dev:
+        raise ValueError(f'frames_resize: out must be a contiguous {dtype} tensor [{n}, 3, {height}, {width}] on {dev}')
+    chunk = n if on_device else max(1, min(n, staging_bytes // (H0 * W0 * 3)))
+    tmp = torch.empty((chunk * H0 * width * 3,), device=dev, dtype=torch.uint8) if width != W0 else None
+
+    def launch(src, i0, k):
+        rc = l.t2v_frames_resize(_lib.ptr(src), k, H0, W0, _lib.ptr(out[i0]), height, width, int(dtype == torch.float16),
+                                 _lib.ptr(tmp), tmp.numel() if tmp is not None else 0, _lib.stream_ptr())
+        _lib.check(rc, 'frames_resize')
+
+    if on_device:
+        launch(frames.contiguous(), 0, n)
+        return out
+    stream = torch.cuda.current_stream(dev)
+    nbuf = 1 if chunk == n else 2
+    pinned = [torch.empty((chunk, H0, W0, 3), dtype=torch.uint8, pin_memory=True) for _ in range(nbuf)]
+    staged = [torch.empty((chunk, H0, W0, 3), dtype=torch.uint8, device=dev) for _ in range(nbuf)]
+    copied = [None] * nbuf          # event after the upload that last read each pinned buffer
+    for c, i0 in enumerate(range(0, n, chunk)):
+        b, k = c % nbuf, min(chunk, n - i0)
+        if copied[b] is not None:
+            copied[b].synchronize()
+        host = pinned[b].numpy()
+        for j in range(k):
+            host[j] = _host_frame(frames[i0 + j], (H0, W0))
+        staged[b][:k].copy_(pinned[b][:k], non_blocking=True)
+        copied[b] = torch.cuda.Event()
+        copied[b].record(stream)
+        launch(staged[b], i0, k)
+    return out
+
+
+def _host_frame(frame, size):
+    a = np.asarray(frame)
+    if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or (size is not None and a.shape[:2] != size):
+        want = f'[{size[0]}, {size[1]}, 3]' if size is not None else '[H, W, 3]'
+        raise ValueError(f'frames_resize: every frame must be uint8 RGB {want}, got {a.dtype} {list(a.shape)}')
+    return a

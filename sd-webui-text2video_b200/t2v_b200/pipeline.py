@@ -216,7 +216,8 @@ class TextToVideoSynthesis(object):
             latents = latents.to(self.device)
             if 'half precision' in str(cpu_vae):
                 latents = latents.half()
-        groups = self.plan_groups(n, frames, height, width, c.shape[1])
+        F = latents.shape[2] if latents is not None else frames     # a vid2vid clip has its input video's frames
+        groups = self.plan_groups(n, F, height, width, c.shape[1])
         self.last_batch_groups = groups
         outs, first = [], 0
         if latents is not None and latents.shape[0] not in (1, n):
@@ -240,11 +241,23 @@ class TextToVideoSynthesis(object):
         host.copy_(frames_u8, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         rgb = host.numpy()
-        videos = [[np.ascontiguousarray(f[:, :, ::-1]) for f in rgb[i * frames:(i + 1) * frames]] for i in range(n)]
+        videos = [[np.ascontiguousarray(f[:, :, ::-1]) for f in rgb[i * F:(i + 1) * F]] for i in range(n)]
         infos = [create_infotext(prompt, n_prompt, {'steps': steps_total, 'frames': frames, 'seed': s, 'scale': scale,
                                                     'width': width, 'height': height, 'eta': eta, 'sampler': sampler})
                  for s in seeds]
         return videos, [x0[i:i + 1] for i in range(n)], infos
+
+    def prepare_frames(self, frames_u8, width, height, cpu_vae='GPU (half precision)'):
+        """The reference's frame preparation for compute_latents (process_modelscope.py:115-137, :172-190): every uint8 RGB
+        frame ([f, H0, W0, 3] array or CUDA tensor, or a sequence of [H0, W0, 3] arrays / RGB PIL images) resized to
+        width x height with PIL's LANCZOS, then x / 255 * 2 - 1, bit for bit, on the device (t2v_frames_resize) ->
+        [1, 3, f, height, width] (a view of a dense [f, 3, height, width]): fp16 in the half-precision VAE mode, the value
+        compute_latents' `.half()` gives, fp32 otherwise."""
+        from . import ops
+        dtype = torch.float16 if 'half precision' in str(cpu_vae) else torch.float32
+        with torch.cuda.device(self.device):
+            out = ops.frames_resize(frames_u8, width, height, dtype)
+        return out.permute(1, 0, 2, 3).unsqueeze(0)
 
     @torch.no_grad()
     def compute_latents(self, vd_out, cpu_vae='GPU (half precision)', device=None):
