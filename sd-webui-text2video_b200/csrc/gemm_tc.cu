@@ -808,7 +808,9 @@ int tma_encode_f16(CUtensorMap* m, const void* base, int rank, const unsigned lo
     return encode_map(m, base, rank, d, st, bx);
 }
 
-int gemm_bs_bn(long long tiles_m, int N, int K, int ntaps, bool geglu, int num_sms, int force_bn, bool any_k, int* stages_out) {
+// Tile width of the B-stationary variant for this problem (0 = not eligible).  tiles_m = ceil(rows / 128) for plain row
+// matrices; any_k lifts the K limit.
+static int gemm_bs_bn(long long tiles_m, int N, int K, int ntaps, int num_sms, int force_bn, bool any_k, int* stages_out) {
     static const bool bs_off = getenv("T2V_NO_BSTAT") != nullptr;
     // Off by default (not measured faster on the model's layers); opt-in with T2V_BSTAT_KMAX=<max K chunks>, e.g. 5, and taken
     // by the op-level tests (GEMM_DBG_FORCE_BS).
@@ -819,11 +821,9 @@ int gemm_bs_bn(long long tiles_m, int N, int K, int ntaps, bool geglu, int num_s
     for (int i = 0; i < 3; ++i) {
         const int c = cands[i];
         if (force_bn != 0 && force_bn != c) continue;
-        if (geglu && (c != 128 || (N % c) != 0)) continue;
         const int tn = (N + c - 1) / c;
         if (static_cast<double>(N) / (static_cast<double>(tn) * c) < 0.9) continue;
         const long long b_bytes = static_cast<long long>(kt) * c * GEMM_BLOCK_K * 2;
-        if (geglu) continue;      // the GEGLU epilogue gains nothing from resident weights and loses with the 128-wide tiles they need
         if (b_bytes > kSmemBudget - 4 * kABytes || tn > num_sms) continue;
         const int stages = static_cast<int>(std::min<long long>(8, (kSmemBudget - b_bytes) / kABytes));
         const int group = num_sms / tn;                               // CTAs per N-tile
@@ -957,11 +957,12 @@ int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms) {
             }
         }
     }
-    // ---- B-stationary variant (see the kernel): few K chunks, many M-tiles per CTA
+    // ---- B-stationary variant (see the kernel): few K chunks, many M-tiles per CTA.  Never for GEGLU: its epilogue gains
+    // nothing from resident weights and loses with the 128-wide tiles they would need.
     plan->bs = 0;
-    if (p.force_bs >= 0 && p.force_cg <= 1 && p.splits <= 1 && p.b_batch_dim < 0) {
+    if (!(p.flags & GEMM_GEGLU) && p.force_bs >= 0 && p.force_cg <= 1 && p.splits <= 1 && p.b_batch_dim < 0) {
         int stages = 0;
-        const int c = gemm_bs_bn(g.tiles_m, p.N, p.K, p.ntaps, (p.flags & GEMM_GEGLU) != 0, num_sms, p.force_bn, p.force_bs == 1, &stages);
+        const int c = gemm_bs_bn(g.tiles_m, p.N, p.K, p.ntaps, num_sms, p.force_bn, p.force_bs == 1, &stages);
         if (c > 0) {
             bn = c;
             plan->bs = 1;

@@ -109,10 +109,6 @@ struct GemmPlan {
     double flops;
 };
 
-// Tile width the B-stationary variant would use for this problem (0 = not eligible): the model code asks before it packs
-// GEGLU weights, whose interleave depends on the tile width.  tiles_m = ceil(rows / 128) for plain row matrices.
-int gemm_bs_bn(long long tiles_m, int N, int K, int ntaps, bool geglu, int num_sms, int force_bn = 0, bool any_k = false,
-               int* stages_out = nullptr);
 // Builds tensor maps / tile shapes for a problem.  Returns 0 on success.
 int gemm_plan(const GemmProblem& p, GemmPlan* plan, int num_sms);
 int gemm_launch(const GemmPlan& plan, cudaStream_t stream);

@@ -425,100 +425,162 @@ void tap(Ctx& c, const std::string& name, const Tok& t, int h, int w) {
     if (c.u->taps_enabled && !c.b->dry()) c.plan->taps[name] = {t, {h, w}};
 }
 
-// BasicTransformerBlock.forward (t2v_model.py:803-809): x += attn1(LN x); x += attn2(LN x, ctx); x += FF(LN x)
-// `temporal`: sequences run along frames for every pixel (both attentions are self-attention, :684-685);
-// otherwise sequences are the h*w tokens of a frame and attn2 attends to the prompt.
-// P: rows between consecutive frames of a sample = pixels per frame (this rank's pixel range when the clip is sharded and
-// `temporal`: the matrix is then in the pixel-sharded layout)
-Tok transformer_block(Ctx& c, Tok x, const std::string& p, int heads, long long P, bool temporal) {
+// GroupNorm rows per instance of a spatial module over P pixels per frame: ModelScope normalises each frame on its own
+// (4-D input), VideoCrafter's GroupNorm32 takes a sample's statistics over all its frames (5-D input, util.py:271-273)
+long long norm_rows(const Ctx& c, long long P) { return c.u->cfg.arch == 1 ? P * c.F : P; }
+
+// ---- transformer sub-layers of ModelScope's BasicTransformerBlock (t2v_model.py:803-809) and VideoCrafter's
+// BasicTransformerBlockST (attention_temporal.py:301-335): x + to_out(attention(LN x)) and x + FF(LN x), every LayerNorm
+// folded into the GEMM that consumes it.  Each frees what it consumed, x included, and returns the new x.
+// Heads of width d = C / heads, scale d^-0.5 (0.125 at ModelScope's d = 64).
+
+AttnParams attn_params(const Tok& o, int heads) {
+    AttnParams a;
+    memset(&a, 0, sizeof(a));
+    a.o = o.p;
+    a.heads = heads;
+    a.head_dim = o.C / heads;
+    a.scale = 1.0f / std::sqrt(static_cast<float>(a.head_dim));
+    a.kv_batch_div = 1;
+    a.b_inner = 1;
+    return a;
+}
+
+void attn_step(Ctx& c, const AttnParams& a, const char* label) {
+    c.b->step([a](cudaStream_t s) { return attention(a, s); }, 1, STEP_ATTN,
+              4.0 * a.batch * a.heads * static_cast<double>(a.sq) * a.skv * a.head_dim, label);
+}
+
+// the fused q|k|v projection of a self-attention
+Tok qkv_proj(Ctx& c, const Tok& x, const std::string& ap, const std::string& lnp) {
+    const __half* w = w_cat(c, {ap + ".to_q.weight", ap + ".to_k.weight", ap + ".to_v.weight"});
+    return ln_linear(c, x, lnp, ap + ".qkv", w, nullptr, 3 * x.C, nullptr);
+}
+
+// after the attention that read `in` and wrote o: x + to_out(o)
+Tok attn_out(Ctx& c, const Tok& x, const Tok& o, const Tok& in, const std::string& ap) {
+    c.b->free(in);
+    Tok y = linear(c, o, prm(c, ap + ".to_out.0.weight"), x.C, prm(c, ap + ".to_out.0.bias"), &x);
+    c.b->free(o);
+    c.b->free(x);
+    return y;
+}
+
+// spatial self-attention: every sequence is the P tokens of one frame
+Tok attn_spatial(Ctx& c, const Tok& x, const std::string& ap, const std::string& lnp, int heads, long long P, const char* label) {
     const int C = x.C;
-    const long long R = x.rows;
-    const float scale = 0.125f;    // head_dim^-0.5, head_dim = 64 (t2v_model.py:530)
-    for (int a = 0; a < 2; ++a) {
-        const std::string ap = p + (a == 0 ? ".attn1" : ".attn2");
-        const std::string lnp = p + (a == 0 ? ".norm1" : ".norm2");
-        const bool self_attn = (a == 0) || temporal;
-        Tok o = c.b->alloc(R, C);
-        AttnParams ap_;
-        memset(&ap_, 0, sizeof(ap_));
-        ap_.heads = heads;
-        ap_.head_dim = 64;
-        ap_.scale = scale;
-        ap_.kv_batch_div = 1;
-        ap_.b_inner = 1;
-        Tok qkv, kv;
-        if (self_attn) {
-            const __half* wqkv = w_cat(c, {ap + ".to_q.weight", ap + ".to_k.weight", ap + ".to_v.weight"});
-            qkv = ln_linear(c, x, lnp, ap + ".qkv", wqkv, nullptr, 3 * C, nullptr);
-            ap_.q = qkv.p;
-            ap_.k = qkv.p + C;
-            ap_.v = qkv.p + 2 * C;
-            ap_.o = o.p;
-            if (!temporal) {
-                ap_.batch = static_cast<int>(R / P);
-                ap_.sq = ap_.skv = static_cast<int>(P);
-                ap_.q_bs = ap_.k_bs = ap_.v_bs = P * qkv.ld;
-                ap_.q_ss = ap_.k_ss = ap_.v_ss = qkv.ld;
-                ap_.o_bs = P * o.ld;
-                ap_.o_ss = o.ld;
-            } else {
-                ap_.batch = static_cast<int>(c.B * P);
-                ap_.b_inner = static_cast<int>(P);
-                ap_.sq = ap_.skv = c.F;
-                ap_.q_bs = ap_.k_bs = ap_.v_bs = static_cast<long long>(c.F) * P * qkv.ld;
-                ap_.q_bsi = ap_.k_bsi = ap_.v_bsi = qkv.ld;
-                ap_.q_ss = ap_.k_ss = ap_.v_ss = P * qkv.ld;
-                ap_.o_bs = static_cast<long long>(c.F) * P * o.ld;
-                ap_.o_bsi = o.ld;
-                ap_.o_ss = P * o.ld;
-            }
-        } else {
-            const Param& wk = c.params->get(ap + ".to_k.weight");
-            const int ctx_dim = wk.data ? static_cast<int>(wk.shape[1]) : c.u->cfg.context_dim;
-            qkv = ln_linear(c, x, lnp, ap + ".to_q", prm(c, ap + ".to_q.weight"), nullptr, C, nullptr);
-            // K/V of the prompt: identical for every frame (the reference recomputes them per frame, :426,:545-546) and, with a
-            // context batch Bc < B, for every sample sharing the prompt: only the Bc * L distinct rows are projected
-            Tok ctx_tok;
-            ctx_tok.p = c.ctx;
-            ctx_tok.rows = static_cast<long long>(c.Bc) * c.L;
-            ctx_tok.C = ctx_dim;
-            ctx_tok.ld = ctx_dim;
-            const __half* wkv = w_cat(c, {ap + ".to_k.weight", ap + ".to_v.weight"});
-            kv = linear(c, ctx_tok, wkv, 2 * C, nullptr, nullptr);
-            ap_.q = qkv.p;
-            ap_.k = kv.p;
-            ap_.v = kv.p + C;
-            ap_.o = o.p;
-            ap_.batch = static_cast<int>(R / P);
-            ap_.sq = static_cast<int>(P);
-            ap_.skv = c.L;
-            ap_.q_bs = P * qkv.ld;
-            ap_.q_ss = qkv.ld;
-            ap_.k_bs = ap_.v_bs = static_cast<long long>(c.L) * kv.ld;
-            ap_.k_ss = ap_.v_ss = kv.ld;
-            // frames per prompt IN THIS MATRIX: frames per sample (frame-sharded clip: this rank's frames) x samples per prompt
-            ap_.kv_batch_div = c.Fl * (c.B / c.Bc);
-            ap_.o_bs = P * o.ld;
-            ap_.o_ss = o.ld;
-        }
-        {
-            const AttnParams apc = ap_;
-            const double fl = 4.0 * apc.batch * apc.heads * static_cast<double>(apc.sq) * apc.skv * 64;
-            const char* label = temporal ? "attn temporal" : (self_attn ? "attn spatial" : "attn cross");
-            c.b->step([apc](cudaStream_t s) { return attention(apc, s); }, 1, STEP_ATTN, fl, label);
-        }
-        c.b->free(qkv);
-        if (!self_attn) c.b->free(kv);
-        Tok y = linear(c, o, prm(c, ap + ".to_out.0.weight"), C, prm(c, ap + ".to_out.0.bias"), &x);
-        c.b->free(o);
-        c.b->free(x);
-        x = y;
-    }
-    // feed-forward: GEGLU fused into the first GEMM's epilogue (t2v_model.py:813-821, :833-846)
-    const int H = 4 * C;
-    int bn = (2 * H) % 256 == 0 ? 256 : ((2 * H) % 128 == 0 ? 128 : 64);
-    // K = 320 layers: the B-stationary GEMM variant wants 128-wide GEGLU tiles (the weight interleave follows the tile width)
-    if (const int bs = gemm_bs_bn((R + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M, 2 * H, C, 1, true, c.b->sms())) bn = bs;
+    Tok o = c.b->alloc(x.rows, C);
+    Tok qkv = qkv_proj(c, x, ap, lnp);
+    AttnParams a = attn_params(o, heads);
+    a.q = qkv.p;
+    a.k = qkv.p + C;
+    a.v = qkv.p + 2 * C;
+    a.batch = static_cast<int>(x.rows / P);
+    a.sq = a.skv = static_cast<int>(P);
+    a.q_bs = a.k_bs = a.v_bs = P * qkv.ld;
+    a.q_ss = a.k_ss = a.v_ss = qkv.ld;
+    a.o_bs = P * o.ld;
+    a.o_ss = o.ld;
+    attn_step(c, a, label);
+    return attn_out(c, x, o, qkv, ap);
+}
+
+// cross-attention on the prompt, queries as in attn_spatial.  A prompt's K/V are the same for every frame (the reference
+// recomputes them per frame, t2v_model.py:426, :545-546; attention_temporal.py:321-325) and, with a context batch Bc < B,
+// for every sample sharing it: only the Bc * L context rows are projected.
+Tok attn_cross(Ctx& c, const Tok& x, const std::string& ap, const std::string& lnp, int heads, long long P, const char* label) {
+    const int C = x.C;
+    Tok o = c.b->alloc(x.rows, C);
+    Tok q = ln_linear(c, x, lnp, ap + ".to_q", prm(c, ap + ".to_q.weight"), nullptr, C, nullptr);
+    Tok ctx_tok;
+    ctx_tok.p = c.ctx;
+    ctx_tok.rows = static_cast<long long>(c.Bc) * c.L;
+    ctx_tok.C = c.u->cfg.context_dim;
+    ctx_tok.ld = ctx_tok.C;
+    const __half* wkv = w_cat(c, {ap + ".to_k.weight", ap + ".to_v.weight"});
+    Tok kv = linear(c, ctx_tok, wkv, 2 * C, nullptr, nullptr);
+    AttnParams a = attn_params(o, heads);
+    a.q = q.p;
+    a.k = kv.p;
+    a.v = kv.p + C;
+    a.batch = static_cast<int>(x.rows / P);
+    a.sq = static_cast<int>(P);
+    a.skv = c.L;
+    a.q_bs = P * q.ld;
+    a.q_ss = q.ld;
+    a.k_bs = a.v_bs = static_cast<long long>(c.L) * kv.ld;
+    a.k_ss = a.v_ss = kv.ld;
+    // frames per prompt IN THIS MATRIX: frames per sample (frame-sharded clip: this rank's frames) x samples per prompt
+    a.kv_batch_div = c.Fl * (c.B / c.Bc);
+    a.o_bs = P * o.ld;
+    a.o_ss = o.ld;
+    attn_step(c, a, label);
+    c.b->free(kv);
+    return attn_out(c, x, o, q, ap);
+}
+
+// ModelScope's temporal self-attention (TemporalTransformer, t2v_model.py:684-685): a sequence runs along the F frames of
+// one pixel.  Rows (b, f, pixel) with P pixels per frame: in a sharded clip, this rank's pixels of the pixel-sharded layout.
+Tok attn_temporal(Ctx& c, const Tok& x, const std::string& ap, const std::string& lnp, int heads, long long P) {
+    const int C = x.C;
+    Tok o = c.b->alloc(x.rows, C);
+    Tok qkv = qkv_proj(c, x, ap, lnp);
+    AttnParams a = attn_params(o, heads);
+    a.q = qkv.p;
+    a.k = qkv.p + C;
+    a.v = qkv.p + 2 * C;
+    a.batch = static_cast<int>(c.B * P);
+    a.b_inner = static_cast<int>(P);
+    a.sq = a.skv = c.F;
+    a.q_bs = a.k_bs = a.v_bs = static_cast<long long>(c.F) * P * qkv.ld;
+    a.q_bsi = a.k_bsi = a.v_bsi = qkv.ld;
+    a.q_ss = a.k_ss = a.v_ss = P * qkv.ld;
+    a.o_bs = static_cast<long long>(c.F) * P * o.ld;
+    a.o_bsi = o.ld;
+    a.o_ss = P * o.ld;
+    attn_step(c, a, "attn temporal");
+    return attn_out(c, x, o, qkv, ap);
+}
+
+// VideoCrafter's temporal self-attention with relative-position K/V tables (TemporalCrossAttention, RelativePosition,
+// attention_temporal.py:46-65, :107-144): the sequences of attn_temporal; the FLOP count adds 2 * max_rel + 1 keys for the
+// two table products
+Tok attn_relpos(Ctx& c, const Tok& x, const std::string& ap, const std::string& lnp, int heads, long long P) {
+    const int C = x.C, d = C / heads;
+    Tok o = c.b->alloc(x.rows, C);
+    Tok qkv = qkv_proj(c, x, ap, lnp);
+    RelposParams r;
+    memset(&r, 0, sizeof(r));
+    r.q = qkv.p;
+    r.k = qkv.p + C;
+    r.v = qkv.p + 2 * C;
+    r.o = o.p;
+    r.table_k = prm(c, ap + ".relative_position_k.embeddings_table");
+    r.table_v = prm(c, ap + ".relative_position_v.embeddings_table");
+    r.n_seq = static_cast<long long>(c.B) * P;
+    r.seq_inner = P;
+    r.bs_outer = static_cast<long long>(c.F) * P * qkv.ld;
+    r.bs_inner = qkv.ld;
+    r.ss = P * qkv.ld;
+    r.o_bs_outer = static_cast<long long>(c.F) * P * o.ld;
+    r.o_bs_inner = o.ld;
+    r.o_ss = P * o.ld;
+    r.heads = heads;
+    r.head_dim = d;
+    r.T = c.F;
+    r.max_rel = c.u->cfg.temporal_length;
+    r.scale = 1.0f / std::sqrt(static_cast<float>(d));
+    const int nrel = 2 * r.max_rel + 1;
+    c.b->step([r](cudaStream_t s) { return attention_relpos(r, s); }, 1, STEP_ATTN,
+              4.0 * r.n_seq * heads * static_cast<double>(c.F) * (c.F + nrel) * d, "attn temporal relpos (vc)");
+    return attn_out(c, x, o, qkv, ap);
+}
+
+// GEGLU feed-forward (t2v_model.py:813-821, :833-846): x + net.2(GEGLU(net.0.proj(LN x))), the GEGLU fused into the first
+// GEMM's epilogue.  Its packed weight interleaves the two halves per tile, so the tile width is fixed here.
+Tok feed_forward(Ctx& c, const Tok& x, const std::string& p) {
+    const int C = x.C, H = 4 * C;
+    const int bn = (2 * H) % 256 == 0 ? 256 : ((2 * H) % 128 == 0 ? 128 : 64);
     Geglu g = w_geglu(c, p + ".ff.net.0.proj", H, C, bn);
     Tok gg = ln_linear(c, x, p + ".norm3", p + ".ff.net.0.proj#geglu" + std::to_string(bn), g.w, g.b, 2 * H, nullptr, GEMM_GEGLU, bn);
     Tok y = linear(c, gg, prm(c, p + ".ff.net.2.weight"), C, prm(c, p + ".ff.net.2.bias"), &x);
@@ -527,27 +589,51 @@ Tok transformer_block(Ctx& c, Tok x, const std::string& p, int heads, long long 
     return y;
 }
 
-// SpatialTransformer.forward (:639-658, use_linear) / TemporalTransformer.forward (:716-767, Conv1d k=1 projections)
-Tok transformer(Ctx& c, const Tok& x, const Blk& blk, int hcur, int wcur, bool temporal) {
-    // temporal: rows (b, f, own pixels) -- all frames local; the 5-D GroupNorm's statistics span every rank's pixels
+// GroupNorm -> proj_in -> transformer block -> proj_out + x, all on the one token matrix [(b, f, y, x), C] (none of the
+// reference's rearranges exist).  The block:
+//   ST  SpatialTransformer (t2v_model.py:639-658, use_linear): spatial self -> cross -> FF;
+//   TT  TemporalTransformer (:716-767, Conv1d k=1 projections): temporal self twice (only_self_att, :684-685) -> FF;
+//   STT VideoCrafter's SpatialTemporalTransformer (attention_temporal.py:386-399): spatial self -> relpos temporal ->
+//       cross -> relpos temporal again ("attn2_tmp" with context None) -> FF.
+Tok transformer(Ctx& c, const Tok& x, const Blk& blk, int hcur, int wcur) {
+    // TT: rows (b, f, own pixels) -- all frames local; the 5-D GroupNorm's statistics span every rank's pixels
+    const bool temporal = blk.kind == Blk::TT;
     const long long Pfull = static_cast<long long>(hcur) * wcur;
     const long long P = temporal ? own_pixels(c, hcur, wcur) : Pfull;
     const std::string& p = blk.prefix;
-    Tok n = group_norm(c, x, p + ".norm", temporal ? P * c.F : P, 1e-6f, false,
+    Tok n = group_norm(c, x, p + ".norm", temporal ? P * c.F : norm_rows(c, P), 1e-6f, false,
                        (temporal && c.nranks > 1) ? Pfull * c.F : 0);
-    Tok h0 = linear(c, n, prm(c, p + ".proj_in.weight"), blk.inner, prm(c, p + ".proj_in.bias"), nullptr);
+    Tok h = linear(c, n, prm(c, p + ".proj_in.weight"), blk.inner, prm(c, p + ".proj_in.bias"), nullptr);
     c.b->free(n);
-    Tok h3 = transformer_block(c, h0, p + ".transformer_blocks.0", blk.heads, P, temporal);
-    Tok y = linear(c, h3, prm(c, p + ".proj_out.weight"), blk.cin, prm(c, p + ".proj_out.bias"), &x);
-    c.b->free(h3);
+    const std::string t = p + ".transformer_blocks.0";
+    const int heads = blk.heads;
+    switch (blk.kind) {
+        case Blk::ST:
+            h = attn_spatial(c, h, t + ".attn1", t + ".norm1", heads, P, "attn spatial");
+            h = attn_cross(c, h, t + ".attn2", t + ".norm2", heads, P, "attn cross");
+            break;
+        case Blk::TT:
+            h = attn_temporal(c, h, t + ".attn1", t + ".norm1", heads, P);
+            h = attn_temporal(c, h, t + ".attn2", t + ".norm2", heads, P);
+            break;
+        default:        // Blk::STT
+            h = attn_spatial(c, h, t + ".attn1", t + ".norm1", heads, P, "attn spatial (vc)");
+            h = attn_relpos(c, h, t + ".attn1_tmp", t + ".norm4", heads, P);
+            h = attn_cross(c, h, t + ".attn2", t + ".norm2", heads, P, "attn cross (vc)");
+            h = attn_relpos(c, h, t + ".attn2_tmp", t + ".norm5", heads, P);
+            break;
+    }
+    h = feed_forward(c, h, t);
+    Tok y = linear(c, h, prm(c, p + ".proj_out.weight"), blk.cin, prm(c, p + ".proj_out.bias"), &x);
+    c.b->free(h);
     return y;
 }
 
-// ResBlock._forward (:983-1009) + TemporalConvBlock_v2.forward (:1218-1229)
+// ResBlock._forward (t2v_model.py:983-1009; VideoCrafter openaimodel3d.py:244-271, whose Conv3d (1,3,3) are the same
+// per-frame 3x3 convs), then ModelScope's TemporalConvBlock_v2.forward (:1218-1229)
 Tok res_block(Ctx& c, const Tok& x, const Blk& blk, int hcur, int wcur) {
     const std::string& p = blk.prefix;
     const long long P = static_cast<long long>(hcur) * wcur;
-    const long long R = x.rows;
     const int Co = blk.cout;
     const int E = c.u->cfg.dim * 4;
     // emb_layers(SiLU -> Linear) per sample, folded with conv1's bias into a per-sample bias row
@@ -560,10 +646,10 @@ Tok res_block(Ctx& c, const Tok& x, const Blk& blk, int hcur, int wcur) {
         const int B = c.B;
         c.b->step([=](cudaStream_t s) { return small_linear(emb, E, we, be, bc, bias1, Co, B, Co, E, 1, s); });
     }
-    Tok a = group_norm(c, x, p + ".in_layers.0", P, 1e-5f, true);
+    Tok a = group_norm(c, x, p + ".in_layers.0", norm_rows(c, P), 1e-5f, true);
     Tok h = conv3x3(c, a, p + ".in_layers.2.weight", bias1, static_cast<int>(c.Fl * P), Co, Co, hcur, wcur, nullptr);
     c.b->free(a);
-    Tok bn_ = group_norm(c, h, p + ".out_layers.0", P, 1e-5f, true);
+    Tok bn_ = group_norm(c, h, p + ".out_layers.0", norm_rows(c, P), 1e-5f, true);
     c.b->free(h);
     Tok skip = x;
     bool own_skip = false;
@@ -575,6 +661,7 @@ Tok res_block(Ctx& c, const Tok& x, const Blk& blk, int hcur, int wcur) {
     c.b->free(bn_);
     if (own_skip) c.b->free(skip);
     c.b->free_bytes(bias1);
+    if (c.u->cfg.arch == 1) return h2;
     // temporal conv block: 4 x [GN(5-D: statistics over all frames of a sample) -> SiLU -> Conv3d (3,1,1)] + identity.
     // Sharded clip: transpose to the pixel-sharded layout first -- all F frames of this rank's pixels are then local, the
     // 3-tap conv and its zero padding at f = 0, F-1 need no halo; only the GroupNorm sums cross ranks.
@@ -611,150 +698,6 @@ Tok res_block(Ctx& c, const Tok& x, const Blk& blk, int hcur, int wcur) {
         y = y2;
     }
     c.b->free(h2);
-    return y;
-}
-
-
-// ---- VideoCrafter blocks
-// ResBlock._forward (openaimodel3d.py:244-271): every GroupNorm32 takes its statistics over (C/32, T, H, W) of a sample
-// (5-D input, util.py:271-273); the convs are Conv3d (1,3,3) = per-frame 3x3; no temporal conv.
-Tok res_block_vc(Ctx& c, const Tok& x, const Blk& blk, int hcur, int wcur) {
-    const std::string& p = blk.prefix;
-    const long long P = static_cast<long long>(hcur) * wcur;
-    const int Co = blk.cout;
-    const int E = c.u->cfg.dim * 4;
-    __half* bias1 = reinterpret_cast<__half*>(c.b->alloc_bytes(static_cast<size_t>(c.B) * Co * sizeof(__half)));
-    {
-        const __half* we = prm(c, p + ".emb_layers.1.weight");
-        const __half* be = prm(c, p + ".emb_layers.1.bias");
-        const __half* bc = prm(c, p + ".in_layers.2.bias");
-        const __half* emb = c.emb;
-        const int B = c.B;
-        c.b->step([=](cudaStream_t s) { return small_linear(emb, E, we, be, bc, bias1, Co, B, Co, E, 1, s); });
-    }
-    Tok a = group_norm(c, x, p + ".in_layers.0", P * c.F, 1e-5f, true);
-    Tok h = conv3x3(c, a, p + ".in_layers.2.weight", bias1, static_cast<int>(c.F * P), Co, Co, hcur, wcur, nullptr);
-    c.b->free(a);
-    Tok bn_ = group_norm(c, h, p + ".out_layers.0", P * c.F, 1e-5f, true);
-    c.b->free(h);
-    Tok skip = x;
-    bool own_skip = false;
-    if (blk.cin != blk.cout) {
-        skip = linear(c, x, prm(c, p + ".skip_connection.weight"), Co, prm(c, p + ".skip_connection.bias"), nullptr);
-        own_skip = true;
-    }
-    Tok h2 = conv3x3(c, bn_, p + ".out_layers.3.weight", prm(c, p + ".out_layers.3.bias"), 0, 0, Co, hcur, wcur, &skip);
-    c.b->free(bn_);
-    if (own_skip) c.b->free(skip);
-    c.b->free_bytes(bias1);
-    return h2;
-}
-
-// SpatialTemporalTransformer.forward (attention_temporal.py:386-399) around BasicTransformerBlockST._forward (:301-335):
-// spatial self -> temporal self (relative position) -> spatial cross (CLIP) -> temporal self again ("attn2_tmp" with
-// context None) -> GEGLU feed-forward, each with its own LayerNorm and a residual add.  All five run on the ONE token
-// matrix [(b, t, y, x), C]; the reference's five rearranges per block do not exist.
-Tok stt_block(Ctx& c, const Tok& xin, const Blk& blk, int hcur, int wcur) {
-    const std::string& p0 = blk.prefix;
-    const long long P = static_cast<long long>(hcur) * wcur;
-    const long long R = xin.rows;
-    const int C = blk.inner, heads = blk.heads, d = C / heads;
-    const float scale = 1.0f / std::sqrt(static_cast<float>(d));
-    Tok n = group_norm(c, xin, p0 + ".norm", P * c.F, 1e-6f, false);
-    Tok x = linear(c, n, prm(c, p0 + ".proj_in.weight"), C, prm(c, p0 + ".proj_in.bias"), nullptr);
-    c.b->free(n);
-    const std::string p = p0 + ".transformer_blocks.0";
-    auto finish = [&](Tok& o, Tok& qkv, const std::string& ap) {
-        c.b->free(qkv);
-        Tok y = linear(c, o, prm(c, ap + ".to_out.0.weight"), C, prm(c, ap + ".to_out.0.bias"), &x);
-        c.b->free(o);
-        c.b->free(x);
-        x = y;
-    };
-    auto spatial_self = [&](const std::string& ap, const std::string& lnp) {
-        const __half* wqkv = w_cat(c, {ap + ".to_q.weight", ap + ".to_k.weight", ap + ".to_v.weight"});
-        Tok qkv = ln_linear(c, x, lnp, ap + ".qkv", wqkv, nullptr, 3 * C, nullptr);
-        Tok o = c.b->alloc(R, C);
-        AttnParams a;
-        memset(&a, 0, sizeof(a));
-        a.q = qkv.p; a.k = qkv.p + C; a.v = qkv.p + 2 * C; a.o = o.p;
-        a.heads = heads; a.head_dim = d; a.scale = scale; a.kv_batch_div = 1; a.b_inner = 1;
-        a.batch = static_cast<int>(R / P);
-        a.sq = a.skv = static_cast<int>(P);
-        a.q_bs = a.k_bs = a.v_bs = P * qkv.ld;
-        a.q_ss = a.k_ss = a.v_ss = qkv.ld;
-        a.o_bs = P * o.ld;
-        a.o_ss = o.ld;
-        c.b->step([a](cudaStream_t s) { return attention(a, s); }, 1, STEP_ATTN,
-                  4.0 * a.batch * a.heads * static_cast<double>(a.sq) * a.skv * d, "attn spatial (vc)");
-        finish(o, qkv, ap);
-    };
-    auto temporal = [&](const std::string& ap, const std::string& lnp) {
-        const __half* wqkv = w_cat(c, {ap + ".to_q.weight", ap + ".to_k.weight", ap + ".to_v.weight"});
-        Tok qkv = ln_linear(c, x, lnp, ap + ".qkv", wqkv, nullptr, 3 * C, nullptr);
-        Tok o = c.b->alloc(R, C);
-        RelposParams r;
-        memset(&r, 0, sizeof(r));
-        r.q = qkv.p; r.k = qkv.p + C; r.v = qkv.p + 2 * C; r.o = o.p;
-        r.table_k = prm(c, ap + ".relative_position_k.embeddings_table");
-        r.table_v = prm(c, ap + ".relative_position_v.embeddings_table");
-        r.n_seq = static_cast<long long>(c.B) * P;
-        r.seq_inner = P;
-        r.bs_outer = static_cast<long long>(c.F) * P * qkv.ld;
-        r.bs_inner = qkv.ld;
-        r.ss = P * qkv.ld;
-        r.o_bs_outer = static_cast<long long>(c.F) * P * o.ld;
-        r.o_bs_inner = o.ld;
-        r.o_ss = P * o.ld;
-        r.heads = heads; r.head_dim = d; r.T = c.F; r.max_rel = c.u->cfg.temporal_length; r.scale = scale;
-        const int nrel = 2 * r.max_rel + 1;
-        c.b->step([r](cudaStream_t s) { return attention_relpos(r, s); }, 1, STEP_ATTN,
-                  4.0 * r.n_seq * heads * static_cast<double>(c.F) * (c.F + nrel) * d, "attn temporal relpos (vc)");
-        finish(o, qkv, ap);
-    };
-    spatial_self(p + ".attn1", p + ".norm1");
-    temporal(p + ".attn1_tmp", p + ".norm4");
-    {   // spatial cross-attention on the prompt: K/V projected once per prompt (the reference repeats the context per frame, :321-325)
-        const std::string ap = p + ".attn2";
-        Tok q = ln_linear(c, x, p + ".norm2", ap + ".to_q", prm(c, ap + ".to_q.weight"), nullptr, C, nullptr);
-        Tok ctx_tok;
-        ctx_tok.p = c.ctx;
-        ctx_tok.rows = static_cast<long long>(c.Bc) * c.L;
-        ctx_tok.C = c.u->cfg.context_dim;
-        ctx_tok.ld = ctx_tok.C;
-        const __half* wkv = w_cat(c, {ap + ".to_k.weight", ap + ".to_v.weight"});
-        Tok kv = linear(c, ctx_tok, wkv, 2 * C, nullptr, nullptr);
-        Tok o = c.b->alloc(R, C);
-        AttnParams a;
-        memset(&a, 0, sizeof(a));
-        a.q = q.p; a.k = kv.p; a.v = kv.p + C; a.o = o.p;
-        a.heads = heads; a.head_dim = d; a.scale = scale; a.b_inner = 1;
-        a.batch = static_cast<int>(R / P);
-        a.sq = static_cast<int>(P);
-        a.skv = c.L;
-        a.q_bs = P * q.ld; a.q_ss = q.ld;
-        a.k_bs = a.v_bs = static_cast<long long>(c.L) * kv.ld;
-        a.k_ss = a.v_ss = kv.ld;
-        a.kv_batch_div = c.F * (c.B / c.Bc);
-        a.o_bs = P * o.ld; a.o_ss = o.ld;
-        c.b->step([a](cudaStream_t s) { return attention(a, s); }, 1, STEP_ATTN,
-                  4.0 * a.batch * a.heads * static_cast<double>(a.sq) * a.skv * d, "attn cross (vc)");
-        c.b->free(kv);
-        finish(o, q, ap);
-    }
-    temporal(p + ".attn2_tmp", p + ".norm5");
-    {
-        const int H = 4 * C;
-        const int bn = (2 * H) % 256 == 0 ? 256 : ((2 * H) % 128 == 0 ? 128 : 64);
-        Geglu g = w_geglu(c, p + ".ff.net.0.proj", H, C, bn);
-        Tok gg = ln_linear(c, x, p + ".norm3", p + ".ff.net.0.proj#geglu" + std::to_string(bn), g.w, g.b, 2 * H, nullptr, GEMM_GEGLU, bn);
-        Tok y = linear(c, gg, prm(c, p + ".ff.net.2.weight"), C, prm(c, p + ".ff.net.2.bias"), &x);
-        c.b->free(gg);
-        c.b->free(x);
-        x = y;
-    }
-    Tok y = linear(c, x, prm(c, p0 + ".proj_out.weight"), blk.cin, prm(c, p0 + ".proj_out.bias"), &xin);
-    c.b->free(x);
     return y;
 }
 
@@ -897,12 +840,10 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
                 case Blk::STEM:
                     y = conv3x3(c, x, b.prefix + ".weight", prm(c, b.prefix + ".bias"), 0, 0, b.cout, hc, wc, nullptr);
                     break;
-                case Blk::RES:
-                    y = cfg.arch == 1 ? res_block_vc(c, x, b, hc, wc) : res_block(c, x, b, hc, wc);
-                    break;
-                case Blk::STT: y = stt_block(c, x, b, hc, wc); break;
-                case Blk::ST: y = transformer(c, x, b, hc, wc, false); break;
-                case Blk::TT: y = transformer(c, x, b, hc, wc, true); break;
+                case Blk::RES: y = res_block(c, x, b, hc, wc); break;
+                case Blk::ST:
+                case Blk::TT:
+                case Blk::STT: y = transformer(c, x, b, hc, wc); break;
                 case Blk::DOWN:
                     y = downsample(c, x, b, hc, wc);
                     hc = (hc + 1) / 2;
@@ -961,7 +902,7 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
     }
     to_layout(false);
     // head: GN -> SiLU -> Conv3x3 dim -> out_dim (t2v_model.py:321-323)
-    Tok g = group_norm(c, x, "out.0", static_cast<long long>(hc) * wc * (cfg.arch == 1 ? F : 1), 1e-5f, true);
+    Tok g = group_norm(c, x, "out.0", norm_rows(c, static_cast<long long>(hc) * wc), 1e-5f, true);
     bld.free(x);
     Tok o = conv3x3(c, g, "out.2.weight", prm(c, "out.2.bias"), 0, 0, cfg.out_dim, hc, wc, nullptr, 16);
     bld.free(g);
@@ -1115,7 +1056,6 @@ int unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const
     const IO& io = entry->io;
     const t2v_unet_config& cfg = u->cfg;
     const int cin_pad = (cfg.in_dim + 7) / 8 * 8;
-    const int F_total = F;
     if (u->shard_on) {                   // x / out hold this rank's frames only: [B, C, F_local, h, w]
         if (!plan->shard->connected) {
             set_error("frame-sharded forward before t2v_unet_shard_connect for this shape");
@@ -1123,7 +1063,6 @@ int unet_forward(t2v_unet* u, const void* x, int x_is_f32, const float* t, const
         }
         F = plan->shard->fb[u->peers.rank + 1] - plan->shard->fb[u->peers.rank];
     }
-    (void)F_total;
     int rc = ingest_latent(x, x_is_f32, io.x_tok, cin_pad, cin_pad, B, cfg.in_dim, F, h, w, 1.0f, stream);
     if (rc != 0) return rc;
     cudaMemcpyAsync(io.t, t, sizeof(float) * B, cudaMemcpyDeviceToDevice, stream);
