@@ -17,6 +17,9 @@
 //
 // Both consumer warpgroups share every K/V tile (one L2 read per 128 queries).
 //
+// attention() (attention.cu) routes here the calls attention_tc_eligible accepts; attention_tc encodes the three tensor
+// maps and launches.
+//
 // Numerics (= torch SDPA fused kernels the reference dispatches to, t2v_model.py:561-569): fp16 operands, fp32 scores,
 // fp32 online softmax with the scale folded into exp2, P rounded to fp16 for P.V, fp32 output accumulation,
 // normalised by the fp32 row sum at the end.
@@ -227,7 +230,7 @@ bool attention_tc_eligible(const AttnParams& p) {
     return true;
 }
 
-int attention_tc_plan(const AttnParams& p, AttnTcPlan* plan) {
+int attention_tc(const AttnParams& p, cudaStream_t stream) {
     if (!attention_tc_eligible(p)) return -1;
     if (!g_attr_set) {
         if (cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL) != cudaSuccess) {
@@ -236,6 +239,7 @@ int attention_tc_plan(const AttnParams& p, AttnTcPlan* plan) {
         }
         g_attr_set = true;
     }
+    CUtensorMap map_q, map_k, map_v;   // rank 3: (heads*64, sequence, batch)
     const unsigned box[3] = {HD, BQ, 1};
     const int kvb = (p.batch + p.kv_batch_div - 1) / p.kv_batch_div;
     struct {
@@ -243,39 +247,26 @@ int attention_tc_plan(const AttnParams& p, AttnTcPlan* plan) {
         const __half* base;
         long long bs, ss;
         int S, nb;
-    } maps[3] = {{&plan->map_q, p.q, p.q_bs, p.q_ss, p.sq, p.batch},
-                 {&plan->map_k, p.k, p.k_bs, p.k_ss, p.skv, kvb},
-                 {&plan->map_v, p.v, p.v_bs, p.v_ss, p.skv, kvb}};
+    } maps[3] = {{&map_q, p.q, p.q_bs, p.q_ss, p.sq, p.batch},
+                 {&map_k, p.k, p.k_bs, p.k_ss, p.skv, kvb},
+                 {&map_v, p.v, p.v_bs, p.v_ss, p.skv, kvb}};
     for (auto& m : maps) {
         const unsigned long long dims[3] = {static_cast<unsigned long long>(p.heads) * HD, static_cast<unsigned long long>(m.S),
                                             static_cast<unsigned long long>(m.nb)};
         const unsigned long long str[2] = {static_cast<unsigned long long>(m.ss) * 2, static_cast<unsigned long long>(m.bs) * 2};
         if (tma_encode_f16(m.m, m.base, 3, dims, str, box) != 0) return -3;
     }
-    plan->o = p.o;
-    plan->o_bs = p.o_bs;
-    plan->o_ss = p.o_ss;
-    plan->sq = p.sq;
-    plan->skv = p.skv;
-    plan->kv_batch_div = p.kv_batch_div;
-    plan->batch = p.batch;
-    plan->heads = p.heads;
-    plan->sl2 = p.scale * 1.4426950408889634f;
-    return 0;
-}
-
-int attention_tc_launch(const AttnTcPlan& pl, cudaStream_t stream) {
     Args a;
-    a.o = pl.o;
-    a.o_bs = pl.o_bs;
-    a.o_ss = pl.o_ss;
-    a.sq = pl.sq;
-    a.skv = pl.skv;
-    a.kv_batch_div = pl.kv_batch_div;
-    a.n_kv = (pl.skv + BKV - 1) / BKV;
-    a.sl2 = pl.sl2;
-    dim3 grid((pl.sq + BQ - 1) / BQ, pl.heads, pl.batch);
-    attention_tc_kernel<<<grid, NTHREADS, SMEM_TOTAL, stream>>>(pl.map_q, pl.map_k, pl.map_v, a);
+    a.o = p.o;
+    a.o_bs = p.o_bs;
+    a.o_ss = p.o_ss;
+    a.sq = p.sq;
+    a.skv = p.skv;
+    a.kv_batch_div = p.kv_batch_div;
+    a.n_kv = (p.skv + BKV - 1) / BKV;
+    a.sl2 = p.scale * 1.4426950408889634f;
+    dim3 grid((p.sq + BQ - 1) / BQ, p.heads, p.batch);
+    attention_tc_kernel<<<grid, NTHREADS, SMEM_TOTAL, stream>>>(map_q, map_k, map_v, a);
     return launch_status("attention_tc launch");
 }
 

@@ -1,10 +1,11 @@
 // Declarations of the non-GEMM kernels' host launchers (norm.cu, attention.cu, elementwise.cu).
 #pragma once
-#include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
+
+#include <initializer_list>
 
 namespace t2v {
 
@@ -33,7 +34,7 @@ struct AttnParams {
     const __half* k;
     const __half* v;
     __half* o;
-    long long q_bs, q_ss;     // batch / sequence strides in elements (head h lives at column h*64)
+    long long q_bs, q_ss;     // batch / sequence strides in elements (head h lives at column h*head_dim)
     long long k_bs, k_ss;
     long long v_bs, v_ss;
     long long o_bs, o_ss;
@@ -43,17 +44,19 @@ struct AttnParams {
     long long q_bsi, k_bsi, v_bsi, o_bsi;   // (temporal attention: outer = sample, inner = pixel); b_inner = 1 -> unused
     float scale;
 };
-// Picks the kernel for every caller: head_dim != 64 -> attention_hd; attention_tc when attention_tc_eligible; else the
-// warp-MMA kernel of attention.cu.  Returns -1 without launching when attention_args_aligned fails on the warp-MMA route.
+// Picks the kernel for every caller: attention_tc when attention_tc_eligible (head_dim 64, long sequences), else the
+// warp-MMA kernels of attention.cu for head_dim 8 / 16 / 32 / 40 / 64 / 80 / 160 (head h at column h*head_dim).
+// Returns -1 without launching on bad shapes, an unsupported head_dim, or operands that break
+// attention_operands_aligned's rules on the warp-MMA route.
 int attention(const AttnParams& p, cudaStream_t stream);
-// What the warp-MMA and any-head-dim kernels need of their operands: 16-byte cp.async loads (Q, K, V 16-byte aligned, every
-// batch, inner-batch and sequence stride a multiple of 8 elements; 0 is a legal broadcast) and __half2 stores (O 4-byte
-// aligned, even strides).  Records the reason with set_error when it returns false.
-bool attention_args_aligned(const AttnParams& p);
+// What the warp-MMA and relative-position kernels need of their operands: 16-byte cp.async loads (every pointer in
+// `loads` 16-byte aligned, every stride in `load_strides` a multiple of 8 elements; 0 is a legal broadcast) and __half2
+// stores (O 4-byte aligned, even `o_strides`).  Records the reason with set_error, prefixed by `who`, when it returns false.
+bool attention_operands_aligned(const char* who, std::initializer_list<const void*> loads,
+                                std::initializer_list<long long> load_strides, const void* o,
+                                std::initializer_list<long long> o_strides);
 
-// attention_hd.cu: head dims other than 64 (VideoCrafter: C/8 = 40 / 80 / 160) and temporal attention with
-// relative-position tables.  attention_hd takes the same AttnParams (head h at column h*head_dim).
-int attention_hd(const AttnParams& p, cudaStream_t stream);
+// attention_relpos.cu: temporal attention with relative-position tables (VideoCrafter)
 struct RelposParams {
     const __half* q;
     const __half* k;
@@ -68,21 +71,13 @@ struct RelposParams {
     int heads, head_dim, T, max_rel;
     float scale;
 };
-// -1 without launching on bad shapes or on operands that break attention_args_aligned's rules (the tables 16-byte aligned too)
+// -1 without launching on bad shapes or on operands that break attention_operands_aligned's rules (the tables are loads too)
 int attention_relpos(const RelposParams& p, cudaStream_t stream);
 
 // attention_tc.cu: wgmma / TMA kernel for long self-attention sequences (sq >= 256, skv >= 128, one-level batch).
-// The plan holds the three tensor maps; attention() encodes them before each launch (a captured graph replays them).
-struct AttnTcPlan {
-    CUtensorMap map_q, map_k, map_v;   // rank 3: (heads*64, sequence, batch)
-    __half* o;
-    long long o_bs, o_ss;
-    int sq, skv, kv_batch_div, batch, heads;
-    float sl2;
-};
+// attention_tc encodes the three tensor maps before each launch (a captured graph replays them); -1 unless eligible.
 bool attention_tc_eligible(const AttnParams& p);
-int attention_tc_plan(const AttnParams& p, AttnTcPlan* plan);
-int attention_tc_launch(const AttnTcPlan& plan, cudaStream_t stream);
+int attention_tc(const AttnParams& p, cudaStream_t stream);
 
 // clip.cu: causal self-attention of the CLIP / OpenCLIP text towers on nn.MultiheadAttention's fused in_proj output
 // qkv [B*L, 3W] (q | k | v, head h at columns h*64 of each part) -> o [B*L, W]; q scaled by 64^-0.5 before q.k.

@@ -1,6 +1,6 @@
 // Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor, with cluster multicast), wgmma (warpgroup
-// MMA with shared-memory descriptors) and the warp-level mma.sync used by the short-sequence attention kernels.
-// No CUTLASS/CuTe dependency: descriptors are built by hand (bit layouts documented below).
+// MMA with shared-memory descriptors) and the warp-level mma.sync used by the short-sequence attention kernels, with the
+// padded shared-memory tile those kernels load with cp.async.  No CUTLASS/CuTe dependency: descriptors are built by hand (bit layouts documented below).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -320,5 +320,38 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
+
+// fp16 tile of rows x HD in shared memory with a padded row pitch (HDP*2 + 16 bytes, an odd number of 16-byte chunks):
+// ldmatrix stays conflict-free for head widths whose HD/8 is not a power of two, where an XOR swizzle does not fit.
+template <int HD>
+struct PaddedTile {
+    static constexpr int HDP = (HD + 15) / 16 * 16;      // head dim padded to the MMA K step
+    static constexpr int PB = HDP * 2 + 16;              // row pitch in bytes
+    static constexpr int KS = HDP / 16;                  // k-steps over the head dim
+    static constexpr int NBD = HDP / 8;                  // 8-wide output blocks over the head dim
+    static constexpr int CH = HD / 8;                    // valid 16-byte chunks per row
+    static constexpr int CHP = HDP / 8;                  // chunks per row incl. zero padding
+
+    static __device__ __forceinline__ uint32_t off(int row, int chunk) { return row * PB + chunk * 16; }
+
+    // rows x HD from global (row stride `stride` elements) into the tile; rows >= s_len and the pad columns are zero-filled
+    // (src-size 0 cp.async).  `nthreads` threads cooperate.
+    static __device__ __forceinline__ void load_rows(uint32_t smem_tile, const __half* gbase, long long stride, int s0,
+                                                     int s_len, int rows, int tid, int nthreads) {
+        for (int idx = tid; idx < rows * CHP; idx += nthreads) {
+            const int row = idx / CHP;
+            const int chunk = idx - row * CHP;
+            const bool ok = (s0 + row) < s_len && chunk < CH;
+            const __half* src = gbase + static_cast<long long>(ok ? (s0 + row) : 0) * stride + (ok ? chunk * 8 : 0);
+            cp_async16(smem_tile + row * PB + chunk * 16, src, ok);
+        }
+    }
+    // TS rows by the 2*TS threads of a flash-attention CTA
+    template <int TS>
+    static __device__ __forceinline__ void load(uint32_t smem_tile, const __half* gbase, long long stride, int s0,
+                                                int s_len, int tid) {
+        load_rows(smem_tile, gbase, stride, s0, s_len, TS, tid, 2 * TS);
+    }
+};
 
 }  // namespace t2v
