@@ -323,6 +323,30 @@ int t2v_cfg_x0(const float* x, const void* eps_c, const void* eps_u, int eps_is_
                float alpha, float sigma, int cfg_fp16, void* stream);
 int t2v_lincomb(float* out, const float* const* src, const float* coef, int n_src, long long n, void* stream);
 
+/* x0 range restriction of DDIM_Gaussian (gaussian_sampler.py:110-120, :174-178, :199-202): t2v_ddim_step's mode 0 over B
+ * samples of n / B elements each, with x0 restricted before eps is recomputed from it.
+ *   percentile in (0, 1]: dynamic thresholding, per sample: s = the percentile-quantile of |x0| (as t2v_abs_quantile, written
+ *                         to s_out [B]), then x0 = min(s', max(-s', x0)) / s' with s' = max(s, 1);
+ *   percentile == 0:      x0 clamped to [-1, 1] (the reference clamps to +-1 whatever value `clamp` has); s_out and the
+ *                         workspace are unused and may be NULL.
+ * fp32 op by op in the reference's order; NaN propagates as in torch.  x_out holds x0 between the launches, so it must not
+ * overlap x, eps_c, eps_u or noise.  Errors (-1, before any launch): x_out == x, n not a multiple of B, percentile outside
+ * {0} U (0, 1], and with percentile > 0 the t2v_abs_quantile errors for n / B.  No host synchronisation: graph-capturable. */
+int t2v_ddim_step_threshold(const float* x, const void* eps_c, const void* eps_u, int eps_is_f32, float* x_out, long long n,
+                            long long chan_stride, int C, int guided_channels, float g, float a0, float a1, float a2, float a3,
+                            float a4, const float* noise, int cfg_fp16, int B, float percentile, float* s_out, void* workspace,
+                            long long workspace_bytes, void* stream);
+/* out[b] = torch.quantile(|x[b*n : (b+1)*n]|, q) (linear interpolation) for b < B, bit for bit: rank = fp32(q) * (n - 1) in
+ * fp32, the floor(rank)-th and ceil(rank)-th order statistics by an exact radix select on the bit patterns, then torch.lerp's
+ * fp32 arithmetic with weight rank - floor(rank); NaN for a sample that holds a NaN.  x and out are device pointers; the
+ * workspace holds at least t2v_abs_quantile_workspace(B) bytes of device memory and is cleared on the stream by each call.
+ * Deterministic, no host synchronisation (graph-capturable).  Errors (-1, before any launch): B outside [1, 65535], n < 1,
+ * q outside [0, 1], a missing pointer or a short workspace, and n > 2^24 ("quantile() input tensor is too large", as torch). */
+int t2v_abs_quantile(const float* x, int B, long long n, float q, float* out, void* workspace, long long workspace_bytes,
+                     void* stream);
+/* Host only: the workspace bytes t2v_abs_quantile and t2v_ddim_step_threshold need for B samples. */
+long long t2v_abs_quantile_workspace(int B);
+
 /* img2vid inpainting latent of process_modelscope.py:170-219: masked_latents = image_latents * (1 - mask) + latent_noise * mask
  * with mask[:, :, f] = weights[f] (the per-frame schedule of T2VAnimKeys), evaluated in fp64 like the reference's numpy code.
  *   image_latents [BC, image_frames, hw] fp32 (image_frames = 1: one encoded image shared by all frames, or F)

@@ -425,6 +425,63 @@ int t2v_ddim_step(const float* x, const void* eps_c, const void* eps_u, int eps_
     p.mode = mode; p.a0 = a0; p.a1 = a1; p.a2 = a2; p.a3 = a3; p.a4 = a4; p.noise = noise; p.cfg_fp16 = cfg_fp16;
     return ddim_step(p, reinterpret_cast<cudaStream_t>(stream));
 }
+long long t2v_abs_quantile_workspace(int B) { return static_cast<long long>(abs_quantile_workspace(B)); }
+static int check_quantile_args(const char* what, const float* x, int B, long long n, const float* out, const void* ws,
+                               long long ws_bytes) {
+    if (B < 1 || B > 65535 || n < 1) {
+        set_error("%s: need 1 <= B <= 65535 samples of n >= 1 elements (B %d, n %lld)", what, B, n);
+        return -1;
+    }
+    if (n > kQuantileMaxN) {
+        set_error("quantile() input tensor is too large");
+        return -1;
+    }
+    if (x == nullptr || out == nullptr) {
+        set_error("%s: x and the quantile output are required", what);
+        return -1;
+    }
+    const long long need = t2v_abs_quantile_workspace(B);
+    if (ws == nullptr || ws_bytes < need) {
+        set_error("%s: %d samples need a workspace of %lld bytes, got %lld", what, B, need, ws ? ws_bytes : 0LL);
+        return -1;
+    }
+    return 0;
+}
+int t2v_abs_quantile(const float* x, int B, long long n, float q, float* out, void* workspace, long long workspace_bytes,
+                     void* stream) {
+    if (check_quantile_args("abs_quantile", x, B, n, out, workspace, workspace_bytes) != 0) return -1;
+    if (!(q >= 0.f && q <= 1.f)) {
+        set_error("abs_quantile: q must lie in [0, 1], got %g", static_cast<double>(q));
+        return -1;
+    }
+    clear_pending_error("abs_quantile");
+    return abs_quantile(x, B, n, q, out, workspace, reinterpret_cast<cudaStream_t>(stream));
+}
+int t2v_ddim_step_threshold(const float* x, const void* eps_c, const void* eps_u, int eps_is_f32, float* x_out, long long n,
+                            long long chan_stride, int C, int guided_channels, float g, float a0, float a1, float a2, float a3,
+                            float a4, const float* noise, int cfg_fp16, int B, float percentile, float* s_out, void* workspace,
+                            long long workspace_bytes, void* stream) {
+    if (x == nullptr || eps_c == nullptr || x_out == nullptr || x_out == x || n < 1 || chan_stride < 1 || C < 1) {
+        set_error("ddim_step_threshold: x, eps_c and a distinct x_out are required, with n, chan_stride and C >= 1");
+        return -1;
+    }
+    if (B < 1 || n % B != 0) {
+        set_error("ddim_step_threshold: %lld elements do not split into %d samples", n, B);
+        return -1;
+    }
+    if (!(percentile >= 0.f && percentile <= 1.f)) {
+        set_error("ddim_step_threshold: percentile must be 0 (clamp) or lie in (0, 1], got %g", static_cast<double>(percentile));
+        return -1;
+    }
+    if (percentile > 0.f && check_quantile_args("ddim_step_threshold", x, B, n / B, s_out, workspace, workspace_bytes) != 0)
+        return -1;
+    DdimStepParams p;
+    p.x = x; p.eps_c = eps_c; p.eps_u = eps_u; p.eps_is_f32 = eps_is_f32;
+    p.x_out = x_out; p.n = n; p.chan_stride = chan_stride; p.C = C; p.guided_channels = guided_channels; p.g = g;
+    p.mode = 0; p.a0 = a0; p.a1 = a1; p.a2 = a2; p.a3 = a3; p.a4 = a4; p.noise = noise; p.cfg_fp16 = cfg_fp16;
+    clear_pending_error("ddim_step_threshold");
+    return ddim_threshold_step(p, B, percentile, s_out, workspace, reinterpret_cast<cudaStream_t>(stream));
+}
 int t2v_cfg_x0(const float* x, const void* eps_c, const void* eps_u, int eps_is_f32, float* x0, long long n, float g, float alpha,
                float sigma, int cfg_fp16, void* stream) {
     return cfg_x0(x, eps_c, eps_u, eps_is_f32, x0, n, g, alpha, sigma,

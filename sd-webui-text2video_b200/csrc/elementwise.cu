@@ -444,6 +444,44 @@ __global__ void ddim_step_kernel(DdimStepParams p) {
     }
 }
 
+// torch.maximum / torch.minimum / torch.clamp: a NaN operand gives NaN
+__device__ __forceinline__ float nan_max(float a, float b) { return isnan(a) ? a : (isnan(b) ? b : fmaxf(a, b)); }
+__device__ __forceinline__ float nan_min(float a, float b) { return isnan(a) ? a : (isnan(b) ? b : fminf(a, b)); }
+
+// DDIM_Gaussian's x0 (mode 0 of ddim_step_kernel) -> x_out, the input of the dynamic-thresholding quantile
+__global__ void ddim_x0_kernel(DdimStepParams p) {
+    GRID_STRIDE(i, p.n) {
+        const int ch = static_cast<int>((i / p.chan_stride) % p.C);
+        const float c = load_eps(p.eps_c, i, p.eps_is_f32);
+        float e = c;
+        if (p.eps_u != nullptr && ch < p.guided_channels) e = cfg_combine(c, load_eps(p.eps_u, i, p.eps_is_f32), p.g, p.cfg_fp16);
+        p.x_out[i] = __fsub_rn(__fmul_rn(p.a0, p.x[i]), __fmul_rn(p.a1, e));
+    }
+}
+
+// Mode 0 with x0 restricted before eps is recomputed from it (gaussian_sampler.py:110-120, :174-178, :199-202):
+// s != null: x0 = min(s', max(-s', x0)) / s' with s' = max(s[sample], 1); s == null: x0 = clamp(x0, -1, 1).
+__global__ void ddim_threshold_kernel(DdimStepParams p, const float* s, long long sample_n) {
+    GRID_STRIDE(i, p.n) {
+        const int ch = static_cast<int>((i / p.chan_stride) % p.C);
+        const float c = load_eps(p.eps_c, i, p.eps_is_f32);
+        float e = c;
+        if (p.eps_u != nullptr && ch < p.guided_channels) e = cfg_combine(c, load_eps(p.eps_u, i, p.eps_is_f32), p.g, p.cfg_fp16);
+        const float x = p.x[i];
+        const float nz = (p.noise != nullptr && p.a4 != 0.f) ? __fmul_rn(p.a4, p.noise[i]) : 0.f;
+        const float ax = __fmul_rn(p.a0, x);
+        float x0 = __fsub_rn(ax, __fmul_rn(p.a1, e));
+        if (s != nullptr) {
+            const float si = nan_max(s[i / sample_n], 1.f);
+            x0 = __fdiv_rn(nan_min(si, nan_max(-si, x0)), si);
+        } else {
+            x0 = nan_min(nan_max(x0, -1.f), 1.f);
+        }
+        const float eps = __fdiv_rn(__fsub_rn(ax, x0), p.a1);
+        p.x_out[i] = __fadd_rn(__fadd_rn(__fmul_rn(p.a2, x0), __fmul_rn(p.a3, eps)), nz);
+    }
+}
+
 struct LincombArgs {
     const float* src[8];
     float coef[8];
@@ -691,6 +729,16 @@ int convert_to_f16(const void* src, int src_is_f32, __half* dst, long long n, cu
 }
 int ddim_step(const DdimStepParams& p, cudaStream_t stream) {
     ddim_step_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p);
+    return ok();
+}
+int ddim_threshold_step(const DdimStepParams& p, int B, float percentile, float* s, void* ws, cudaStream_t stream) {
+    if (percentile > 0.f) {
+        ddim_x0_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p);
+        int rc = ok();
+        if (rc != 0) return rc;
+        if ((rc = abs_quantile(p.x_out, B, p.n / B, percentile, s, ws, stream)) != 0) return rc;
+    }
+    ddim_threshold_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p, percentile > 0.f ? s : nullptr, p.n / B);
     return ok();
 }
 int lincomb(float* out, const float* const* src, const float* coef, int n_src, long long n, cudaStream_t stream) {

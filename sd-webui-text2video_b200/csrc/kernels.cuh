@@ -194,6 +194,18 @@ struct DdimStepParams {
     int cfg_fp16;             // 1: CFG combine rounded to fp16 op by op, as under the reference's autocast
 };
 int ddim_step(const DdimStepParams& p, cudaStream_t stream);
+// DDIM_Gaussian's step (mode 0) with x0 restricted as gaussian_sampler.py:110-120 does, for B samples of p.n / B elements:
+// percentile > 0: s[b] = the percentile-quantile of |x0| of sample b (abs_quantile, written to s; x_out holds x0 meanwhile),
+// then x0 = min(s', max(-s', x0)) / s', s' = max(s[b], 1); percentile == 0: x0 clamped to [-1, 1] (s, ws unused).
+// Arguments are checked by the caller (t2v_ddim_step_threshold).
+int ddim_threshold_step(const DdimStepParams& p, int B, float percentile, float* s, void* ws, cudaStream_t stream);
+
+// ---------------------------------------------------------------- quantile.cu
+// out[b] = torch.quantile(|x[b * n, (b + 1) * n)|, q) with linear interpolation, exactly; NaN for a sample holding a NaN.
+// ws: abs_quantile_workspace(B) bytes, cleared on the stream by every call.  Arguments are checked by the caller.
+constexpr long long kQuantileMaxN = 1LL << 24;      // torch.quantile's limit
+size_t abs_quantile_workspace(int B);
+int abs_quantile(const float* x, int B, long long n, float q, float* out, void* ws, cudaStream_t stream);
 // out = sum_i coef[i] * src[i]  (fp32), n_src <= 8  -- UniPC predictor/corrector combinations
 int lincomb(float* out, const float* const* src, const float* coef, int n_src, long long n, cudaStream_t stream);
 // CFG combine for UniPC: eps = u + g (c - u) in fp16 rounding, then x0 = (x - sigma*eps)/alpha  -> fp32

@@ -87,6 +87,10 @@ SIGNATURES = {
                               c_float, P, c_int, P]),
     't2v_cfg_x0': (c_int, [P, P, P, c_int, P, c_ll, c_float, c_float, c_float, c_int, P]),
     't2v_lincomb': (c_int, [P, C.POINTER(P), C.POINTER(c_float), c_int, c_ll, P]),
+    't2v_ddim_step_threshold': (c_int, [P, P, P, c_int, P, c_ll, c_ll, c_int, c_int, c_float, c_float, c_float, c_float, c_float,
+                                        c_float, P, c_int, c_int, c_float, P, P, c_ll, P]),
+    't2v_abs_quantile': (c_int, [P, c_int, c_ll, c_float, P, P, c_ll, P]),
+    't2v_abs_quantile_workspace': (c_ll, [c_int]),
     't2v_latent_blend': (c_int, [P, c_int, P, P, P, P, c_int, c_int, c_ll, P]),
     't2v_q_sample_blend': (c_int, [P, C.POINTER(c_ll), P, C.POINTER(c_ll), P, P, P, C.POINTER(c_ll), P, P, C.POINTER(c_int), P]),
     't2v_frames_resize': (c_int, [P, c_int, c_int, c_int, P, c_int, c_int, c_int, P, c_ll, P]),

@@ -241,6 +241,24 @@ def clip_attention(qkv, L, heads, o=None):
     return o
 
 
+def abs_quantile(x, q, out=None, workspace=None):
+    """torch.quantile(x.abs(), q, dim=1) of an fp32 CUDA tensor x [B, n] (t2v_abs_quantile), bit for bit, by an exact radix
+    select: no sort and no host synchronisation.  NaN for a row holding a NaN; RuntimeError for a row above 2^24 elements.
+    `workspace`: a CUDA uint8 tensor of at least t2v_abs_quantile_workspace(B) bytes (allocated when None)."""
+    l = _lib.lib()
+    if x.dim() != 2 or x.dtype != torch.float32 or not x.is_cuda:
+        raise TypeError('abs_quantile: x must be a 2-D fp32 CUDA tensor [B, n]')
+    x = x.contiguous()
+    B = x.shape[0]
+    out = torch.empty(B, device=x.device, dtype=torch.float32) if out is None else out
+    if workspace is None:
+        workspace = torch.empty(l.t2v_abs_quantile_workspace(B), device=x.device, dtype=torch.uint8)
+    rc = l.t2v_abs_quantile(_lib.ptr(x), B, x.shape[1], float(q), _lib.ptr(out), _lib.ptr(workspace), workspace.numel(),
+                            _lib.stream_ptr())
+    _lib.check(rc, 'abs_quantile')
+    return out
+
+
 def q_sample_blend(x0, noise, a, s, mask=None, img=None, out=None):
     """t2v_q_sample_blend on fp32 CUDA tensors: a[b] * x0 + s[b] * noise (q_sample), or, with `mask` and `img`,
     that * mask + (1 - mask) * img (the masked-DDIM blend), rounded as torch's fp32 ops.  The output has img's shape

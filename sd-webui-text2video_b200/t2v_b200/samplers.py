@@ -14,7 +14,9 @@ What changed underneath (GPU-first):
     (the reference's UniPC calls torch.linalg.solve on the device every step, uni_pc.py:603-613);
   * quirks that affect results are reproduced: DDIM_Gaussian guides only the first half of the latent channels
     (`learned_range` split, gaussian_sampler.py:93-95,125-136), DDIM guides all of them (ddim/sampler.py:181), the last
-    DDIM step uses alpha_prev = alphas_cumprod[0], UniPC runs `steps` model evaluations with float timesteps.
+    DDIM step uses alpha_prev = alphas_cumprod[0], UniPC runs `steps` model evaluations with float timesteps;
+  * DDIM_Gaussian's `clamp=` / `percentile=` restrict x0 inside the step (t2v_ddim_step_threshold); the per-sample
+    quantile of dynamic thresholding is an exact radix select on the device, again without a host sync.
 The callback contract is unchanged: it is called on the host once per step and may raise to interrupt.
 """
 import ctypes as C
@@ -97,6 +99,32 @@ def _step_kernel(x, e_c, e_u, g, guided_channels, mode, a, noise, cfg_fp16):
     return out
 
 
+def _threshold_step_kernel(x, e_c, e_u, g, guided_channels, a, noise, cfg_fp16, percentile):
+    """DDIM_Gaussian's step with x0 restricted (t2v_ddim_step_threshold): `percentile` thresholds each sample of x by its own
+    quantile of |x0|, 0 clamps x0 to [-1, 1].  Returns (x_{t-1}, s): s [B] holds the per-sample quantiles (None when clamping)."""
+    l = _lib.lib()
+    x = x.contiguous()
+    out = torch.empty_like(x)
+    if e_c.dtype not in (torch.float16, torch.float32):
+        e_c = e_c.float()
+    e_c = e_c.contiguous()
+    if e_u is not None:
+        e_u = e_u.to(e_c.dtype).contiguous()
+    B, Cc = x.shape[0], x.shape[1]
+    s = ws = None
+    if percentile > 0:
+        s = torch.empty(B, dtype=torch.float32, device=x.device)
+        ws = torch.empty(l.t2v_abs_quantile_workspace(B), dtype=torch.uint8, device=x.device)
+    rc = l.t2v_ddim_step_threshold(_lib.ptr(x), _lib.ptr(e_c), _lib.ptr(e_u), int(e_c.dtype == torch.float32), _lib.ptr(out),
+                                   x.numel(), x.numel() // (B * Cc), Cc, guided_channels, float(g),
+                                   float(a[0]), float(a[1]), float(a[2]), float(a[3]), float(a[4]),
+                                   _lib.ptr(noise) if (noise is not None and float(a[4]) != 0.0) else C.c_void_p(0),
+                                   int(cfg_fp16), B, float(percentile), _lib.ptr(s), _lib.ptr(ws),
+                                   0 if ws is None else ws.numel(), _lib.stream_ptr())
+    _lib.check(rc, 'ddim_step_threshold')
+    return out, s
+
+
 def _need_cuda(x):
     if not x.is_cuda:
         raise RuntimeError('t2v_b200 samplers run on the GPU only (latent is on %s)' % x.device)
@@ -141,8 +169,19 @@ class GaussianDiffusion(object):
     def sample(self, x_T=None, S=5, shape=None, conditioning=None, unconditional_conditioning=None, model_kwargs={},
                clamp=None, percentile=None, condition_fn=None, unconditional_guidance_scale=None, eta=0.0,
                callback=None, mask=None, **kwargs):
-        if clamp is not None or percentile is not None or condition_fn is not None:
-            raise NotImplementedError('x0 clamping / classifier guidance are unused by the pipeline')
+        """x0 range restriction (gaussian_sampler.py:110-120, :174-178): `percentile` (dynamic thresholding) rescales each
+        sample's x0 by max(1, its percentile-quantile of |x0|) and takes precedence over `clamp`; any `clamp` that is not None
+        clamps x0 to [-1, 1] whatever its value, as the reference does (it passes clamp=True).  A batch of n clips thresholds
+        each clip by its own quantile, as n sequential runs would."""
+        if condition_fn is not None:
+            raise NotImplementedError('classifier guidance (condition_fn) is not supported')
+        if percentile is not None:
+            assert percentile > 0 and percentile <= 1
+            if _dist._frame_shard is not None:
+                raise NotImplementedError('percentile thresholding of a frame-sharded clip: the quantile spans the ranks')
+            restrict = float(percentile)
+        else:
+            restrict = None if clamp is None else 0.0            # 0: clamp x0 to [-1, 1]
         device = getattr(self.model, 'device', None)
         xt = torch.randn(shape, device=device) if x_T is None else x_T.clone()
         _need_cuda(xt)
@@ -167,9 +206,13 @@ class GaussianDiffusion(object):
             direction = torch.sqrt(1 - alp - sig ** 2)
             nz_mask = 1.0 if tv != 0 else 0.0
             noise = _dist.step_noise(xt)                      # drawn every step, as the reference does (:279)
-            xt = _step_kernel(xt, e_c, e_u, 1.0 if unguided else g, self.guided_channels(xt.shape[1]), 0,
-                              (sr, srm1, torch.sqrt(alp), direction, nz_mask * sig), noise,
-                              cfg_fp16=(e_c.dtype == torch.float16))
+            coefs = (sr, srm1, torch.sqrt(alp), direction, nz_mask * sig)
+            if restrict is None:
+                xt = _step_kernel(xt, e_c, e_u, 1.0 if unguided else g, self.guided_channels(xt.shape[1]), 0, coefs, noise,
+                                  cfg_fp16=(e_c.dtype == torch.float16))
+            else:
+                xt, _ = _threshold_step_kernel(xt, e_c, e_u, 1.0 if unguided else g, self.guided_channels(xt.shape[1]), coefs,
+                                               noise, e_c.dtype == torch.float16, restrict)
             if hasattr(self, 'inpaint_masking'):
                 # the reference overwrites `mask` with t.ne(0)... (:281), so its inpaint hook runs -- and draws one more
                 # randn_like -- on EVERY step whenever the hook is attached, whether or not the caller passed a mask (:285-291)
