@@ -455,10 +455,45 @@ int t2v_op_attention_relpos(const void* q, const void* k, const void* v, void* o
  * q.k as nn.MultiheadAttention does.  -1 unless W % 64 == 0, W / heads == 64 and 1 <= L <= 128. */
 int t2v_op_clip_attention(const void* qkv, void* o, int B, int L, int W, int heads, void* stream);
 int t2v_op_upsample2x(const void* x, void* y, int nframes, int h, int w, int C, void* stream);
-int t2v_op_im2col_s2(const void* x, void* col, int nframes, int h, int w, int C, void* stream);
+/* 3x3 stride-2 gather x [n, h, w, C] -> col [n*ho*wo, 9*C] (tap-major, tap = ky*3+kx), zeros outside x.  pad_lo = 1:
+ * Conv2d(stride 2, padding 1), ho = ceil(h/2); pad_lo = 0: the ldm Downsample's pad (0,1,0,1) + padding 0, ho = floor(h/2).
+ * -1 unless C % 8 == 0 and pad_lo is 0 or 1. */
+int t2v_op_im2col_s2(const void* x, void* col, int nframes, int h, int w, int C, int pad_lo, void* stream);
 int t2v_op_time_sinusoid(const float* t, void* out, int B, int dim, void* stream);
 int t2v_op_small_linear(const void* x, long long ldx, const void* W, const void* bias, const void* addend, void* y,
                         long long ldy, int B, int N, int K, int silu_in, void* stream);
+/* Frames [frame0, frame0 + nframes) in (b f) order of x [B, C, F, h, w] (fp32 or fp16) -> tok [nframes*h*w, ld] fp16:
+ * column c < C = fp16(x * scale) (fp32 product, one rounding), columns C..cpad-1 = 0, columns >= cpad untouched. */
+int t2v_op_ingest_latent(const void* x, int x_is_f32, void* tok, long long ld, int cpad, int C, int F, int h, int w,
+                         long long frame0, long long nframes, float scale, void* stream);
+/* tok [B*F*h*w, ld] fp16 (columns 0..C-1) -> out [B, C, F, h, w] fp32 (exact) or fp16 (copied). */
+int t2v_op_egress_latent(const void* tok, long long ld, void* out, int out_is_f32, int B, int C, int F, int h, int w,
+                         void* stream);
+/* nn.AvgPool2d(2, 2) of x [n, h, w, C] -> y [n, h/2, w/2, C] (floor sizes): fp32 sum of the four taps in row-major order,
+ * times 0.25, one fp16 rounding.  -1 unless C % 8 == 0. */
+int t2v_op_avgpool2x2(const void* x, void* y, int nframes, int h, int w, int C, void* stream);
+/* nn.PixelUnshuffle(8) of x [N, Cc, H, W] (fp32 rounded once, or fp16) -> tok [N*(H/8)*(W/8), 64*Cc] fp16.
+ * -1 unless H % 8 == 0 and W % 8 == 0. */
+int t2v_op_pixel_unshuffle(const void* x, int x_is_f32, void* tok, int N, int Cc, int H, int W, void* stream);
+/* nn.ReLU in place on a dense fp16 matrix [rows, C]; NaN stays NaN.  -1 unless C % 8 == 0. */
+int t2v_op_relu(void* x, long long rows, int C, void* stream);
+/* x[r, :C] = fp16(x[r, :C] + f[(s % f_samples) * rows_per_sample + r % rows_per_sample, :]) with s = r / rows_per_sample, f dense
+ * [., C]; fp32 add, one rounding.  -1 unless C and ldx are multiples of 8 and rows_per_sample, f_samples >= 1. */
+int t2v_op_feature_add(void* x, long long ldx, const void* f, int C, long long rows, long long rows_per_sample, int f_samples,
+                       void* stream);
+/* out[r, :Ca + Cb] = a[r, :Ca] | b[r, :Cb], copied.  -1 unless Ca, Cb, lda, ldb and ldo are multiples of 8. */
+int t2v_op_concat_cols(const void* a, long long lda, int Ca, const void* b, long long ldb, int Cb, void* out, long long ldo,
+                       long long rows, void* stream);
+/* y = softmax over each dense row of x [rows, cols] of fp16(x * scale): fp32 math with __expf, one output rounding. */
+int t2v_op_softmax_rows(const void* x, void* y, long long rows, int cols, float scale, void* stream);
+/* x [nb, R, C] -> y [nb, C, R] fp16, copied. */
+int t2v_op_transpose_batched(const void* x, void* y, int nb, int R, int C, void* stream);
+/* tok [pixels, ld] fp16, RGB in columns 0..2 -> out [pixels, 3] uint8 = trunc(clamp(v * 0.5 + 0.5, 0, 1) * 255) in fp32; NaN -> 0. */
+int t2v_op_frames_to_u8(const void* tok, long long ld, void* out, long long pixels, void* stream);
+/* tok [n*H*W, ld] fp16, RGB in columns 0..2 -> out [n, 3, H, W] fp32 (exact). */
+int t2v_op_frames_to_f32(const void* tok, long long ld, float* out, int n, int H, int W, void* stream);
+/* dst [n] fp16 = src (fp32 rounded to nearest even, or fp16 copied). */
+int t2v_op_convert_to_f16(const void* src, int src_is_f32, void* dst, long long n, void* stream);
 
 #ifdef __cplusplus
 }

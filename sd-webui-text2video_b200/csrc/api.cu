@@ -403,9 +403,78 @@ int t2v_op_upsample2x(const void* x, void* y, int nframes, int h, int w, int C, 
     return upsample2x(reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(y), nframes, h, w, C,
                       reinterpret_cast<cudaStream_t>(stream));
 }
-int t2v_op_im2col_s2(const void* x, void* col, int nframes, int h, int w, int C, void* stream) {
-    return im2col_s2(reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(col), nframes, h, w, C,
-                     reinterpret_cast<cudaStream_t>(stream));
+int t2v_op_im2col_s2(const void* x, void* col, int nframes, int h, int w, int C, int pad_lo, void* stream) {
+    if (pad_lo != 0 && pad_lo != 1) {
+        set_error("op_im2col_s2: pad_lo must be 0 or 1 (got %d)", pad_lo);
+        return -1;
+    }
+    const int rc = im2col_s2(reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(col), nframes, h, w, C,
+                             reinterpret_cast<cudaStream_t>(stream), pad_lo);
+    if (rc == -1) set_error("op_im2col_s2: C = %d must be a multiple of 8", C);
+    return rc;
+}
+int t2v_op_ingest_latent(const void* x, int x_is_f32, void* tok, long long ld, int cpad, int C, int F, int h, int w,
+                         long long frame0, long long nframes, float scale, void* stream) {
+    return ingest_latent_frames(x, x_is_f32, reinterpret_cast<__half*>(tok), ld, cpad, C, F, h, w, frame0, nframes, scale,
+                                reinterpret_cast<cudaStream_t>(stream));
+}
+int t2v_op_egress_latent(const void* tok, long long ld, void* out, int out_is_f32, int B, int C, int F, int h, int w,
+                         void* stream) {
+    return egress_latent(reinterpret_cast<const __half*>(tok), ld, out, out_is_f32, B, C, F, h, w,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+int t2v_op_avgpool2x2(const void* x, void* y, int nframes, int h, int w, int C, void* stream) {
+    const int rc = avgpool2x2(reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(y), nframes, h, w, C,
+                              reinterpret_cast<cudaStream_t>(stream));
+    if (rc == -1) set_error("op_avgpool2x2: C = %d must be a multiple of 8", C);
+    return rc;
+}
+int t2v_op_pixel_unshuffle(const void* x, int x_is_f32, void* tok, int N, int Cc, int H, int W, void* stream) {
+    const int rc = pixel_unshuffle_ingest(x, x_is_f32, reinterpret_cast<__half*>(tok), N, Cc, H, W,
+                                          reinterpret_cast<cudaStream_t>(stream));
+    if (rc == -1) set_error("op_pixel_unshuffle: H = %d and W = %d must be multiples of 8", H, W);
+    return rc;
+}
+int t2v_op_relu(void* x, long long rows, int C, void* stream) {
+    const int rc = relu_inplace(reinterpret_cast<__half*>(x), rows, C, reinterpret_cast<cudaStream_t>(stream));
+    if (rc == -1) set_error("op_relu: C = %d must be a multiple of 8", C);
+    return rc;
+}
+int t2v_op_feature_add(void* x, long long ldx, const void* f, int C, long long rows, long long rows_per_sample, int f_samples,
+                       void* stream) {
+    const int rc = feature_add(reinterpret_cast<__half*>(x), ldx, reinterpret_cast<const __half*>(f), C, rows, rows_per_sample,
+                               f_samples, reinterpret_cast<cudaStream_t>(stream));
+    if (rc == -1)
+        set_error("op_feature_add: C = %d and ldx = %lld must be multiples of 8, rows_per_sample = %lld and f_samples = %d >= 1", C,
+                  ldx, rows_per_sample, f_samples);
+    return rc;
+}
+int t2v_op_concat_cols(const void* a, long long lda, int Ca, const void* b, long long ldb, int Cb, void* out, long long ldo,
+                       long long rows, void* stream) {
+    const int rc = concat_cols(reinterpret_cast<const __half*>(a), lda, Ca, reinterpret_cast<const __half*>(b), ldb, Cb,
+                               reinterpret_cast<__half*>(out), ldo, rows, reinterpret_cast<cudaStream_t>(stream));
+    if (rc == -1)
+        set_error("op_concat_cols: Ca = %d, Cb = %d, lda = %lld, ldb = %lld and ldo = %lld must be multiples of 8", Ca, Cb, lda, ldb,
+                  ldo);
+    return rc;
+}
+int t2v_op_softmax_rows(const void* x, void* y, long long rows, int cols, float scale, void* stream) {
+    return softmax_rows(reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(y), rows, cols, scale,
+                        reinterpret_cast<cudaStream_t>(stream));
+}
+int t2v_op_transpose_batched(const void* x, void* y, int nb, int R, int C, void* stream) {
+    return transpose_batched(reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(y), nb, R, C,
+                             reinterpret_cast<cudaStream_t>(stream));
+}
+int t2v_op_frames_to_u8(const void* tok, long long ld, void* out, long long pixels, void* stream) {
+    return frames_to_u8(reinterpret_cast<const __half*>(tok), ld, reinterpret_cast<uint8_t*>(out), pixels,
+                        reinterpret_cast<cudaStream_t>(stream));
+}
+int t2v_op_frames_to_f32(const void* tok, long long ld, float* out, int n, int H, int W, void* stream) {
+    return frames_to_f32_nchw(reinterpret_cast<const __half*>(tok), ld, out, n, H, W, reinterpret_cast<cudaStream_t>(stream));
+}
+int t2v_op_convert_to_f16(const void* src, int src_is_f32, void* dst, long long n, void* stream) {
+    return convert_to_f16(src, src_is_f32, reinterpret_cast<__half*>(dst), n, reinterpret_cast<cudaStream_t>(stream));
 }
 int t2v_op_time_sinusoid(const float* t, void* out, int B, int dim, void* stream) {
     return time_sinusoid(t, reinterpret_cast<__half*>(out), B, dim, reinterpret_cast<cudaStream_t>(stream));

@@ -229,14 +229,14 @@ __global__ void pixel_unshuffle_kernel(const void* x, int x_is_f32, __half* tok,
     }
 }
 
-// y = max(x, 0) in place on a token matrix (n8 16-byte vectors)
+// y = max(x, 0) in place on a token matrix (n8 16-byte vectors); a NaN stays NaN, as nn.ReLU (__hmax2 would give 0)
 __global__ void relu_kernel(uint4* x, long long n8) {
     const __half2 z = __float2half2_rn(0.f);
     GRID_STRIDE(i, n8) {
         uint4 v = x[i];
         __half2* h = reinterpret_cast<__half2*>(&v);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) h[k] = __hmax2(h[k], z);
+        for (int k = 0; k < 4; ++k) h[k] = __hmax2_nan(h[k], z);
         x[i] = v;
     }
 }

@@ -101,7 +101,7 @@ int im2col_s2(const __half* x, __half* col, int nframes, int h, int w, int C, cu
 // T2I-Adapter glue (adapter.cu, unet.cu).  nn.PixelUnshuffle(8): x [N, Cc, H, W] (fp32 or fp16, H, W multiples of 8) ->
 // tokens [N*(H/8)*(W/8), 64*Cc] fp16, column c*64 + i*8 + j = x[n, c, 8y+i, 8x+j]
 int pixel_unshuffle_ingest(const void* x, int x_is_f32, __half* tok, int N, int Cc, int H, int W, cudaStream_t stream);
-// max(x, 0) in place on a dense token matrix [rows, C]
+// max(x, 0) in place on a dense token matrix [rows, C]; NaN propagates (nn.ReLU)
 int relu_inplace(__half* x, long long rows, int C, cudaStream_t stream);
 // nn.AvgPool2d(2, 2) (floor sizes): x [n, h, w, C] -> y [n, h/2, w/2, C]; fp32 sum, one fp16 rounding
 int avgpool2x2(const __half* x, __half* y, int nframes, int h, int w, int C, cudaStream_t stream);

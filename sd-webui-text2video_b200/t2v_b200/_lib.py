@@ -113,9 +113,21 @@ SIGNATURES = {
                                         c_int, c_int, c_float, P]),
     't2v_op_clip_attention': (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
     't2v_op_upsample2x': (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
-    't2v_op_im2col_s2': (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
+    't2v_op_im2col_s2': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P]),
     't2v_op_time_sinusoid': (c_int, [P, P, c_int, c_int, P]),
     't2v_op_small_linear': (c_int, [P, c_ll, P, P, P, P, c_ll, c_int, c_int, c_int, c_int, P]),
+    't2v_op_ingest_latent': (c_int, [P, c_int, P, c_ll, c_int, c_int, c_int, c_int, c_int, c_ll, c_ll, c_float, P]),
+    't2v_op_egress_latent': (c_int, [P, c_ll, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
+    't2v_op_avgpool2x2': (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
+    't2v_op_pixel_unshuffle': (c_int, [P, c_int, P, c_int, c_int, c_int, c_int, P]),
+    't2v_op_relu': (c_int, [P, c_ll, c_int, P]),
+    't2v_op_feature_add': (c_int, [P, c_ll, P, c_int, c_ll, c_ll, c_int, P]),
+    't2v_op_concat_cols': (c_int, [P, c_ll, c_int, P, c_ll, c_int, P, c_ll, c_ll, P]),
+    't2v_op_softmax_rows': (c_int, [P, P, c_ll, c_int, c_float, P]),
+    't2v_op_transpose_batched': (c_int, [P, P, c_int, c_int, c_int, P]),
+    't2v_op_frames_to_u8': (c_int, [P, c_ll, P, c_ll, P]),
+    't2v_op_frames_to_f32': (c_int, [P, c_ll, P, c_int, c_int, c_int, P]),
+    't2v_op_convert_to_f16': (c_int, [P, c_int, P, c_ll, P]),
 }
 
 

@@ -104,14 +104,125 @@ def upsample2x(x):
     return y
 
 
-def im2col_s2(x):
-    """Stride-2 3x3 gather with padding 1: x [nframes, h, w, C] -> [nframes, ceil(h/2), ceil(w/2), 9 * C], column
-    tap * C + c with tap = ky * 3 + kx."""
+def im2col_s2(x, pad_lo=1, out=None):
+    """Stride-2 3x3 gather: x [nframes, h, w, C] -> [nframes, ho, wo, 9 * C], column tap * C + c with tap = ky * 3 + kx.
+    pad_lo = 1: padding 1, ho = ceil(h/2); pad_lo = 0: the ldm Downsample's pad (0,1,0,1), ho = floor(h/2)."""
     l = _lib.lib()
     nf, h, w, Cc = x.shape
-    col = torch.empty((nf, (h + 1) // 2, (w + 1) // 2, 9 * Cc), device=x.device, dtype=torch.float16)
-    _lib.check(l.t2v_op_im2col_s2(_lib.ptr(x), _lib.ptr(col), nf, h, w, Cc, _lib.stream_ptr()), 'op_im2col_s2')
+    ho, wo = ((h + 1) // 2, (w + 1) // 2) if pad_lo else (h // 2, w // 2)
+    col = torch.empty((nf, ho, wo, 9 * Cc), device=x.device, dtype=torch.float16) if out is None else out
+    _lib.check(l.t2v_op_im2col_s2(_lib.ptr(x), _lib.ptr(col), nf, h, w, Cc, pad_lo, _lib.stream_ptr()), 'op_im2col_s2')
     return col
+
+
+def ingest_latent(x, tok, cpad, frame0=0, nframes=None, scale=1.0):
+    """Frames [frame0, frame0 + nframes) in (b f) order of the latent x [B, C, F, h, w] (fp32 or fp16, contiguous) into the
+    rows of tok [nframes*h*w, ld] fp16 (a row-strided view is fine): fp16(x * scale), columns C..cpad-1 zeroed."""
+    l = _lib.lib()
+    B, Cc, Fr, h, w = x.shape
+    nframes = B * Fr - frame0 if nframes is None else nframes
+    rc = l.t2v_op_ingest_latent(_lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(tok), tok.stride(0), cpad, Cc, Fr, h, w,
+                                frame0, nframes, scale, _lib.stream_ptr())
+    _lib.check(rc, 'op_ingest_latent')
+    return tok
+
+
+def egress_latent(tok, out):
+    """Token rows tok [B*F*h*w, ld] fp16 -> out [B, C, F, h, w] (fp32 or fp16, contiguous)."""
+    l = _lib.lib()
+    B, Cc, Fr, h, w = out.shape
+    rc = l.t2v_op_egress_latent(_lib.ptr(tok), tok.stride(0), _lib.ptr(out), int(out.dtype == torch.float32), B, Cc, Fr, h, w,
+                                _lib.stream_ptr())
+    _lib.check(rc, 'op_egress_latent')
+    return out
+
+
+def avgpool2x2(x, out=None):
+    """nn.AvgPool2d(2, 2) of frames x [nframes, h, w, C] -> [nframes, h // 2, w // 2, C] (fp32 sum, one fp16 rounding)."""
+    l = _lib.lib()
+    nf, h, w, Cc = x.shape
+    y = torch.empty((nf, h // 2, w // 2, Cc), device=x.device, dtype=torch.float16) if out is None else out
+    _lib.check(l.t2v_op_avgpool2x2(_lib.ptr(x), _lib.ptr(y), nf, h, w, Cc, _lib.stream_ptr()), 'op_avgpool2x2')
+    return y
+
+
+def pixel_unshuffle(x, out=None):
+    """nn.PixelUnshuffle(8) of x [N, Cc, H, W] (fp32 or fp16, contiguous) as tokens [N * H/8 * W/8, 64 * Cc] fp16."""
+    l = _lib.lib()
+    N, Cc, H, W = x.shape
+    tok = torch.empty((N * (H // 8) * (W // 8), 64 * Cc), device=x.device, dtype=torch.float16) if out is None else out
+    rc = l.t2v_op_pixel_unshuffle(_lib.ptr(x), int(x.dtype == torch.float32), _lib.ptr(tok), N, Cc, H, W, _lib.stream_ptr())
+    _lib.check(rc, 'op_pixel_unshuffle')
+    return tok
+
+
+def relu_(x):
+    """nn.ReLU in place on a dense fp16 matrix x [rows, C]."""
+    l = _lib.lib()
+    _lib.check(l.t2v_op_relu(_lib.ptr(x), x.shape[0], x.shape[1], _lib.stream_ptr()), 'op_relu')
+    return x
+
+
+def feature_add_(x, f, rows_per_sample, f_samples):
+    """x[r] += f[(r // rows_per_sample % f_samples) * rows_per_sample + r % rows_per_sample] in place (fp32 add, one rounding);
+    x [rows, C] may be a row-strided view, f is dense [f_samples * rows_per_sample, C]."""
+    l = _lib.lib()
+    rows, Cc = x.shape
+    rc = l.t2v_op_feature_add(_lib.ptr(x), x.stride(0), _lib.ptr(f), Cc, rows, rows_per_sample, f_samples, _lib.stream_ptr())
+    _lib.check(rc, 'op_feature_add')
+    return x
+
+
+def concat_cols(a, b, out):
+    """out[:, :Ca + Cb] = a | b for row-strided fp16 matrices a [rows, Ca], b [rows, Cb], out [rows, >= Ca + Cb]."""
+    l = _lib.lib()
+    rc = l.t2v_op_concat_cols(_lib.ptr(a), a.stride(0), a.shape[1], _lib.ptr(b), b.stride(0), b.shape[1], _lib.ptr(out),
+                              out.stride(0), a.shape[0], _lib.stream_ptr())
+    _lib.check(rc, 'op_concat_cols')
+    return out
+
+
+def softmax_rows(x, scale, out=None):
+    """Row softmax of fp16(x * scale) for a dense fp16 matrix x [rows, cols]."""
+    l = _lib.lib()
+    y = torch.empty_like(x) if out is None else out
+    _lib.check(l.t2v_op_softmax_rows(_lib.ptr(x), _lib.ptr(y), x.shape[0], x.shape[1], scale, _lib.stream_ptr()), 'op_softmax_rows')
+    return y
+
+
+def transpose_batched(x, out=None):
+    """x [nb, R, C] fp16 (contiguous) -> [nb, C, R]."""
+    l = _lib.lib()
+    nb, R, Cc = x.shape
+    y = torch.empty((nb, Cc, R), device=x.device, dtype=torch.float16) if out is None else out
+    _lib.check(l.t2v_op_transpose_batched(_lib.ptr(x), _lib.ptr(y), nb, R, Cc, _lib.stream_ptr()), 'op_transpose_batched')
+    return y
+
+
+def frames_to_u8(tok, out=None):
+    """Decoded frames tok [pixels, ld] fp16 (RGB in columns 0..2, a row-strided view is fine) -> uint8 [pixels, 3]."""
+    l = _lib.lib()
+    px = tok.shape[0]
+    out = torch.empty((px, 3), device=tok.device, dtype=torch.uint8) if out is None else out
+    _lib.check(l.t2v_op_frames_to_u8(_lib.ptr(tok), tok.stride(0), _lib.ptr(out), px, _lib.stream_ptr()), 'op_frames_to_u8')
+    return out
+
+
+def frames_to_f32(tok, n, H, W, out=None):
+    """Decoded frames tok [n*H*W, ld] fp16 (RGB in columns 0..2) -> fp32 [n, 3, H, W]."""
+    l = _lib.lib()
+    out = torch.empty((n, 3, H, W), device=tok.device, dtype=torch.float32) if out is None else out
+    _lib.check(l.t2v_op_frames_to_f32(_lib.ptr(tok), tok.stride(0), _lib.ptr(out), n, H, W, _lib.stream_ptr()), 'op_frames_to_f32')
+    return out
+
+
+def convert_to_f16(src, out=None):
+    """Contiguous fp32 or fp16 CUDA tensor -> fp16 of the same shape (round to nearest even)."""
+    l = _lib.lib()
+    out = torch.empty(src.shape, device=src.device, dtype=torch.float16) if out is None else out
+    rc = l.t2v_op_convert_to_f16(_lib.ptr(src), int(src.dtype == torch.float32), _lib.ptr(out), src.numel(), _lib.stream_ptr())
+    _lib.check(rc, 'op_convert_to_f16')
+    return out
 
 
 def time_sinusoid(t, dim):
