@@ -319,6 +319,19 @@ int t2v_ddim_step(const float* x, const void* eps_c, const void* eps_u, int eps_
                   long long chan_stride,
                   int C, int guided_channels, float g, int mode, float a0, float a1, float a2, float a3, float a4,
                   const float* noise, int cfg_fp16, void* stream);
+/* t2v_ddim_step with VideoCrafter's per-step outputs (videocrafter/lvdm/samplers/ddim.py:230-279):
+ *   cfg_variant  the guidance formula on the guided channels, fp32 op by op as torch evaluates it (uc_type):
+ *                0 u + g (c - u) (None; the formula of t2v_ddim_step, fp16 rounding when cfg_fp16), 1 c + g (c - u)
+ *                ('cfg_original'), 2 c + g (u - c) ('cfg_ours').  Variants 1 and 2 need cfg_fp16 = 0.  Without eps_u no
+ *                guidance runs, whatever the variant.
+ *   x0_out       NULL, or n fp32 elements that receive pred_x0 = (x - a0 e) / a1, the exact value the update then uses;
+ *                mode 1 only.  The same pass writes it: one extra 4-byte store per element.
+ * Variant 0 with x0_out = NULL launches the kernel t2v_ddim_step launches, so its output is bit-identical.  Errors (-1, before
+ * any launch): cfg_variant outside 0..2, a variant 1 or 2 with cfg_fp16, x0_out with mode != 1, and x0_out overlapping x,
+ * x_out, eps_c, eps_u or noise.                                                                                            */
+int t2v_ddim_step_ex(const float* x, const void* eps_c, const void* eps_u, int eps_is_f32, float* x_out, long long n,
+                     long long chan_stride, int C, int guided_channels, float g, int mode, float a0, float a1, float a2, float a3,
+                     float a4, const float* noise, int cfg_fp16, int cfg_variant, float* x0_out, void* stream);
 int t2v_cfg_x0(const float* x, const void* eps_c, const void* eps_u, int eps_is_f32, float* x0, long long n, float g,
                float alpha, float sigma, int cfg_fp16, void* stream);
 int t2v_lincomb(float* out, const float* const* src, const float* coef, int n_src, long long n, void* stream);

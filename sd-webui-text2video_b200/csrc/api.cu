@@ -492,7 +492,43 @@ int t2v_ddim_step(const float* x, const void* eps_c, const void* eps_u, int eps_
     p.x = x; p.eps_c = eps_c; p.eps_u = eps_u; p.eps_is_f32 = eps_is_f32;
     p.x_out = x_out; p.n = n; p.chan_stride = chan_stride; p.C = C; p.guided_channels = guided_channels; p.g = g;
     p.mode = mode; p.a0 = a0; p.a1 = a1; p.a2 = a2; p.a3 = a3; p.a4 = a4; p.noise = noise; p.cfg_fp16 = cfg_fp16;
-    return ddim_step(p, reinterpret_cast<cudaStream_t>(stream));
+    return ddim_step(p, 0, nullptr, reinterpret_cast<cudaStream_t>(stream));
+}
+static bool ranges_overlap(const void* a, long long a_bytes, const void* b, long long b_bytes) {
+    if (a == nullptr || b == nullptr) return false;
+    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
+    return pa < pb + static_cast<uintptr_t>(b_bytes) && pb < pa + static_cast<uintptr_t>(a_bytes);
+}
+int t2v_ddim_step_ex(const float* x, const void* eps_c, const void* eps_u, int eps_is_f32, float* x_out, long long n,
+                     long long chan_stride, int C, int guided_channels, float g, int mode, float a0, float a1, float a2, float a3,
+                     float a4, const float* noise, int cfg_fp16, int cfg_variant, float* x0_out, void* stream) {
+    if (cfg_variant < 0 || cfg_variant > 2) {
+        set_error("ddim_step_ex: cfg_variant must be 0 (None), 1 ('cfg_original') or 2 ('cfg_ours'), got %d", cfg_variant);
+        return -1;
+    }
+    if (cfg_variant != 0 && cfg_fp16 != 0) {
+        set_error("ddim_step_ex: cfg_variant %d is fp32 only (cfg_fp16 must be 0)", cfg_variant);
+        return -1;
+    }
+    if (x0_out != nullptr) {
+        if (mode != 1) {
+            set_error("ddim_step_ex: x0_out needs mode 1 (the ldm / VideoCrafter DDIM update), got mode %d", mode);
+            return -1;
+        }
+        const long long f32 = n * 4, eps = n * (eps_is_f32 ? 4 : 2);
+        if (ranges_overlap(x0_out, f32, x, f32) || ranges_overlap(x0_out, f32, x_out, f32) ||
+            ranges_overlap(x0_out, f32, eps_c, eps) || ranges_overlap(x0_out, f32, eps_u, eps) ||
+            ranges_overlap(x0_out, f32, noise, f32)) {
+            set_error("ddim_step_ex: x0_out overlaps x, x_out, eps_c, eps_u or noise");
+            return -1;
+        }
+    }
+    DdimStepParams p;
+    p.x = x; p.eps_c = eps_c; p.eps_u = eps_u; p.eps_is_f32 = eps_is_f32;
+    p.x_out = x_out; p.n = n; p.chan_stride = chan_stride; p.C = C; p.guided_channels = guided_channels; p.g = g;
+    p.mode = mode; p.a0 = a0; p.a1 = a1; p.a2 = a2; p.a3 = a3; p.a4 = a4; p.noise = noise; p.cfg_fp16 = cfg_fp16;
+    clear_pending_error("ddim_step_ex");
+    return ddim_step(p, cfg_variant, x0_out, reinterpret_cast<cudaStream_t>(stream));
 }
 long long t2v_abs_quantile_workspace(int B) { return static_cast<long long>(abs_quantile_workspace(B)); }
 static int check_quantile_args(const char* what, const float* x, int B, long long n, const float* out, const void* ws,

@@ -422,12 +422,25 @@ __device__ __forceinline__ float load_eps(const void* p, long long i, int is_f32
     return is_f32 ? reinterpret_cast<const float*>(p)[i] : __half2float(reinterpret_cast<const __half*>(p)[i]);
 }
 
-__global__ void ddim_step_kernel(DdimStepParams p) {
+// VideoCrafter's uc_type formulas (lvdm/samplers/ddim.py:233-241) in fp32, op by op; kVariant 0 is cfg_combine itself.
+// The host allows kVariant 1 and 2 only with fp16 == 0.
+template <int kVariant>
+__device__ __forceinline__ float cfg_variant(float c, float u, float g, int fp16) {
+    if constexpr (kVariant == 1) return __fadd_rn(c, __fmul_rn(g, __fsub_rn(c, u)));     // 'cfg_original'
+    else if constexpr (kVariant == 2) return __fadd_rn(c, __fmul_rn(g, __fsub_rn(u, c)));   // 'cfg_ours'
+    else return cfg_combine(c, u, g, fp16);
+}
+
+// kX0: also store mode 1's x0 (the value the update uses) to x0_out; the host allows it only in mode 1.
+// <false, 0> is the kernel t2v_ddim_step has always launched; x0_out is unused there.
+template <bool kX0, int kVariant>
+__global__ void ddim_step_kernel(DdimStepParams p, float* x0_out) {
     GRID_STRIDE(i, p.n) {
         const int ch = static_cast<int>((i / p.chan_stride) % p.C);
         const float c = load_eps(p.eps_c, i, p.eps_is_f32);
         float e = c;
-        if (p.eps_u != nullptr && ch < p.guided_channels) e = cfg_combine(c, load_eps(p.eps_u, i, p.eps_is_f32), p.g, p.cfg_fp16);
+        if (p.eps_u != nullptr && ch < p.guided_channels)
+            e = cfg_variant<kVariant>(c, load_eps(p.eps_u, i, p.eps_is_f32), p.g, p.cfg_fp16);
         const float x = p.x[i];
         const float nz = (p.noise != nullptr && p.a4 != 0.f) ? __fmul_rn(p.a4, p.noise[i]) : 0.f;
         float xn;
@@ -438,6 +451,7 @@ __global__ void ddim_step_kernel(DdimStepParams p) {
             xn = __fadd_rn(__fadd_rn(__fmul_rn(p.a2, x0), __fmul_rn(p.a3, eps)), nz);
         } else {
             const float x0 = __fdiv_rn(__fsub_rn(x, __fmul_rn(p.a0, e)), p.a1);
+            if constexpr (kX0) x0_out[i] = x0;
             xn = __fadd_rn(__fadd_rn(__fmul_rn(p.a2, x0), __fmul_rn(p.a3, e)), nz);
         }
         p.x_out[i] = xn;
@@ -727,8 +741,20 @@ int convert_to_f16(const void* src, int src_is_f32, __half* dst, long long n, cu
     convert_kernel<<<grid_for(n, 256), 256, 0, stream>>>(src, src_is_f32, dst, n);
     return ok();
 }
-int ddim_step(const DdimStepParams& p, cudaStream_t stream) {
-    ddim_step_kernel<<<grid_for(p.n, 256), 256, 0, stream>>>(p);
+template <int kVariant>
+static void launch_ddim_step(const DdimStepParams& p, float* x0_out, cudaStream_t stream) {
+    if (x0_out != nullptr)
+        ddim_step_kernel<true, kVariant><<<grid_for(p.n, 256), 256, 0, stream>>>(p, x0_out);
+    else
+        ddim_step_kernel<false, kVariant><<<grid_for(p.n, 256), 256, 0, stream>>>(p, nullptr);
+}
+int ddim_step(const DdimStepParams& p, int cfg_variant, float* x0_out, cudaStream_t stream) {
+    switch (cfg_variant) {
+        case 0: launch_ddim_step<0>(p, x0_out, stream); break;
+        case 1: launch_ddim_step<1>(p, x0_out, stream); break;
+        case 2: launch_ddim_step<2>(p, x0_out, stream); break;
+        default: return -1;
+    }
     return ok();
 }
 int ddim_threshold_step(const DdimStepParams& p, int B, float percentile, float* s, void* ws, cudaStream_t stream) {

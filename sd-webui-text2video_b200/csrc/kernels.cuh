@@ -193,7 +193,9 @@ struct DdimStepParams {
     const float* noise;       // may be null when a4 == 0
     int cfg_fp16;             // 1: CFG combine rounded to fp16 op by op, as under the reference's autocast
 };
-int ddim_step(const DdimStepParams& p, cudaStream_t stream);
+// cfg_variant: 0 u + g (c - u) (fp16 rounding when p.cfg_fp16), 1 c + g (c - u), 2 c + g (u - c), both fp32 only.
+// x0_out != null (mode 1 only): also stores x0.  Arguments are checked by the caller; -1 for a variant outside 0..2.
+int ddim_step(const DdimStepParams& p, int cfg_variant, float* x0_out, cudaStream_t stream);
 // DDIM_Gaussian's step (mode 0) with x0 restricted as gaussian_sampler.py:110-120 does, for B samples of p.n / B elements:
 // percentile > 0: s[b] = the percentile-quantile of |x0| of sample b (abs_quantile, written to s; x_out holds x0 meanwhile),
 // then x0 = min(s', max(-s', x0)) / s', s' = max(s[b], 1); percentile == 0: x0 clamped to [-1, 1] (s, ws unused).

@@ -85,6 +85,8 @@ SIGNATURES = {
     't2v_adapter_encode': (c_int, [P, P, c_int, P, c_int, c_int, c_int, P]),
     't2v_ddim_step': (c_int, [P, P, P, c_int, P, c_ll, c_ll, c_int, c_int, c_float, c_int, c_float, c_float, c_float, c_float,
                               c_float, P, c_int, P]),
+    't2v_ddim_step_ex': (c_int, [P, P, P, c_int, P, c_ll, c_ll, c_int, c_int, c_float, c_int, c_float, c_float, c_float, c_float,
+                                 c_float, P, c_int, c_int, P, P]),
     't2v_cfg_x0': (c_int, [P, P, P, c_int, P, c_ll, c_float, c_float, c_float, c_int, P]),
     't2v_lincomb': (c_int, [P, C.POINTER(P), C.POINTER(c_float), c_int, c_ll, P]),
     't2v_ddim_step_threshold': (c_int, [P, P, P, c_int, P, c_ll, c_ll, c_int, c_int, c_float, c_float, c_float, c_float, c_float,

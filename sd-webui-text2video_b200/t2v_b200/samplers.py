@@ -38,6 +38,9 @@ except Exception:                                       # pragma: no cover - exe
         skipped = False
         sampling_step = 0
         sampling_steps = 0
+        job = ''
+        job_no = 0
+        job_count = 0
 
     state = _State()
 
@@ -97,6 +100,28 @@ def _step_kernel(x, e_c, e_u, g, guided_channels, mode, a, noise, cfg_fp16):
                          int(cfg_fp16), _lib.stream_ptr())
     _lib.check(rc, 'ddim_step')
     return out
+
+
+def _step_kernel_ex(x, e_c, e_u, g, guided_channels, mode, a, noise, cfg_fp16, cfg_variant=0, want_x0=False):
+    """_step_kernel through t2v_ddim_step_ex: `cfg_variant` picks the guidance formula (0 u + g (c - u), 1 c + g (c - u),
+    2 c + g (u - c)), and `want_x0` (mode 1) also returns the step's x0 in a new fp32 tensor.  Returns (x_{t-1}, x0 or None)."""
+    l = _lib.lib()
+    x = x.contiguous()
+    out = torch.empty_like(x)
+    x0 = torch.empty_like(x) if want_x0 else None
+    if e_c.dtype not in (torch.float16, torch.float32):
+        e_c = e_c.float()
+    e_c = e_c.contiguous()
+    if e_u is not None:
+        e_u = e_u.to(e_c.dtype).contiguous()
+    B, Cc = x.shape[0], x.shape[1]
+    rc = l.t2v_ddim_step_ex(_lib.ptr(x), _lib.ptr(e_c), _lib.ptr(e_u), int(e_c.dtype == torch.float32), _lib.ptr(out),
+                            x.numel(), x.numel() // (B * Cc), Cc, guided_channels, float(g), mode,
+                            float(a[0]), float(a[1]), float(a[2]), float(a[3]), float(a[4]),
+                            _lib.ptr(noise) if (noise is not None and float(a[4]) != 0.0) else C.c_void_p(0),
+                            int(cfg_fp16), int(cfg_variant), _lib.ptr(x0), _lib.stream_ptr())
+    _lib.check(rc, 'ddim_step_ex')
+    return out, x0
 
 
 def _threshold_step_kernel(x, e_c, e_u, g, guided_channels, a, noise, cfg_fp16, percentile):

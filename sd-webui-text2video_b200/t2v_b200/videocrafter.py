@@ -24,7 +24,8 @@ Mirrors, with the reference's names / signatures for the calls on the path:
 
 Arithmetic: the UNet runs in fp16 storage / fp32 accumulate (the reference runs this path in fp32; tolerance in
 tests/test_model_gpu.py), CFG `e_u + g (e_c - e_u)` and the DDIM update in fp32 inside ONE fused kernel per step
-(`t2v_ddim_step`, mode 1), cond + uncond evaluated as one B = 2 forward.  q_sample and the masked blend run in a second
+(`t2v_ddim_step_ex`, mode 1: `t2v_ddim_step`'s kernel, with the `uc_type` formulas and, on the steps that need it, pred_x0
+written by the same pass), cond + uncond evaluated as one B = 2 forward.  q_sample and the masked blend run in a second
 fp32 kernel (`t2v_q_sample_blend`), launched only when a mask is given; its output is bit-identical to torch's fp32 ops.
 No CPU / PyTorch fallback.
 """
@@ -36,10 +37,13 @@ import torch
 import torch.nn as nn
 
 from .modules import UNetModel, AutoencoderKL, DiagonalGaussianDistribution
-from .samplers import _step_kernel, _f32, _need_cuda
+from .samplers import _step_kernel_ex, _f32, _need_cuda
+from . import samplers as _samplers
 from .ops import q_sample_blend
 from .distributed import gather_clips
 from . import distributed as _dist
+
+_UC_TYPES = {None: 0, 'cfg_original': 1, 'cfg_ours': 2}        # uc_type -> t2v_ddim_step_ex's cfg_variant
 
 VAE_DDCONFIG = dict(double_z=True, z_channels=4, resolution=256, in_channels=3, out_ch=3, ch=128, ch_mult=[1, 2, 4, 4],
                     num_res_blocks=2, attn_resolutions=[], dropout=0.0)                 # model_config.yaml:53-66
@@ -351,8 +355,8 @@ class DDIMSampler(object):
     @torch.no_grad()
     def sample(self, S, batch_size, shape, conditioning=None, callback=None, img_callback=None, eta=0.0, mask=None, x0=None,
                temperature=1.0, noise_dropout=0.0, verbose=True, schedule_verbose=False, x_T=None, log_every_t=100,
-               unconditional_guidance_scale=1.0, unconditional_conditioning=None, sample_noise=None, features_adapter=None,
-               timesteps=None, **kwargs):
+               unconditional_guidance_scale=1.0, unconditional_conditioning=None, postprocess_fn=None, sample_noise=None,
+               features_adapter=None, timesteps=None, uc_type=None, **kwargs):
         """`features_adapter` (T2VAdapterDepth.get_adapter_features) reaches every apply_model call, conditional and
         unconditional, as in ddim.py:219-229.  Other keywords of adapter_guided_synthesis (`temporal_length`,
         `conditional_guidance_scale_temporal`) reach modules that ignore them in the reference: accepted and ignored.
@@ -361,7 +365,16 @@ class DDIMSampler(object):
         included, img = q_sample(x0, step - 1) * mask + (1 - mask) * img, with one torch.randn_like(x0) per step drawn after the
         step's CPU noise; mask and x0 broadcast to the latent as torch broadcasts, the mask is used in fp32.  `timesteps=k`
         (ddim.py:153-157; SDEdit-style vid2vid from x_T = model.q_sample(z, t)): only the prefix
-        ddim_timesteps[:int(min(k / n, 1) * n) - 1] runs, n = len(ddim_timesteps), with the reference's float64 rounding."""
+        ddim_timesteps[:int(min(k / n, 1) * n) - 1] runs, n = len(ddim_timesteps), with the reference's float64 rounding.
+
+        Per step, in the reference's order (ddim.py:166-204): `state.sampling_step = i` and InterruptedException when
+        `state.interrupted` (webui Interrupt); `img = postprocess_fn(img, ts)`; the step; the mask blend; `callback(i)`, then
+        `img_callback(pred_x0, i)`; every `log_every_t`-th step and the last one append img (after the blend) to
+        intermediates['x_inter'] and pred_x0 (before it) to intermediates['pred_x0']; `state.skipped` (webui Skip) ends the
+        run after the step.  pred_x0 = (x - sqrt(1 - a_t) e_t) / sqrt(a_t) is written by the step kernel itself, only on steps
+        that pass or log it, each time into a new tensor.  `uc_type` (ddim.py:233-241): None e_u + g (e_c - e_u),
+        'cfg_original' e_c + g (e_c - e_u), 'cfg_ours' e_c + g (e_u - e_c); any other value raises NotImplementedError on a
+        guided run, and an unguided run ignores it."""
         if noise_dropout > 0.0 or kwargs.get('score_corrector') is not None or kwargs.get('cond_fn'):
             raise NotImplementedError('noise dropout / score correctors are not on the text2video path')
         if mask is not None:
@@ -372,8 +385,9 @@ class DDIMSampler(object):
         size = (batch_size, *shape)
         return self.ddim_sampling(conditioning, size, callback=callback, img_callback=img_callback, temperature=temperature,
                                   x_T=x_T, log_every_t=log_every_t, unconditional_guidance_scale=unconditional_guidance_scale,
-                                  unconditional_conditioning=unconditional_conditioning, sample_noise=sample_noise,
-                                  features_adapter=features_adapter, mask=mask, x0=x0, timesteps=timesteps)
+                                  unconditional_conditioning=unconditional_conditioning, postprocess_fn=postprocess_fn,
+                                  sample_noise=sample_noise, features_adapter=features_adapter, mask=mask, x0=x0,
+                                  timesteps=timesteps, uc_type=uc_type)
 
     def timestep_prefix(self, timesteps=None):
         """The DDIM timesteps a run with `timesteps` visits (ddim.py:153-157), after make_schedule."""
@@ -408,10 +422,15 @@ class DDIMSampler(object):
 
     @torch.no_grad()
     def ddim_sampling(self, cond, shape, x_T=None, callback=None, img_callback=None, log_every_t=100, temperature=1.0,
-                      unconditional_guidance_scale=1.0, unconditional_conditioning=None, sample_noise=None, features_adapter=None,
-                      mask=None, x0=None, timesteps=None, **kwargs):
+                      unconditional_guidance_scale=1.0, unconditional_conditioning=None, postprocess_fn=None, sample_noise=None,
+                      features_adapter=None, mask=None, x0=None, timesteps=None, uc_type=None, **kwargs):
         device = self.model.device
         fa = {} if features_adapter is None else {'features_adapter': features_adapter}
+        g = float(unconditional_guidance_scale)
+        unguided = unconditional_conditioning is None or g == 1.0
+        if not unguided and uc_type not in _UC_TYPES:
+            raise NotImplementedError(f'uc_type {uc_type!r}: None, \'cfg_original\' or \'cfg_ours\'')
+        variant = 0 if unguided else _UC_TYPES[uc_type]
         # NB the reference draws x_T from the GLOBAL RNG when it is not given (ddim.py:148-149); kept
         img = torch.randn(shape, device=device) if x_T is None else x_T
         _need_cuda(img)
@@ -426,11 +445,16 @@ class DDIMSampler(object):
             t_prev = torch.as_tensor(np.flip(timesteps) - 1, device=device)
             coef = [c[t_prev][:, None].expand(total, b).contiguous() for c in self.model.q_coefficients(device)]
         intermediates = {'x_inter': [img], 'pred_x0': [img]}
-        g = float(unconditional_guidance_scale)
+        state = _samplers.state
+        state.sampling_steps = total
         for i, step in enumerate(np.flip(timesteps)):
+            state.sampling_step = i
+            if state.interrupted:
+                raise _samplers.InterruptedException
             index = total - i - 1
             ts = torch.full((b,), int(step), device=device, dtype=torch.long)
-            unguided = unconditional_conditioning is None or g == 1.0
+            if postprocess_fn is not None:
+                img = postprocess_fn(img, ts).float()
             if unguided:
                 e_c, e_u = self.model.apply_model(img, ts, self._ctx(cond), **fa), None
             else:
@@ -441,15 +465,21 @@ class DDIMSampler(object):
                 noise = torch.randn(img.shape, generator=self.noise_gen).to(device) if float(sigma) != 0.0 else None
             else:
                 noise = sample_noise
-            img = _step_kernel(img, e_c, e_u, 1.0 if unguided else g, img.shape[1], 1,
-                               (s1m, a_t.sqrt(), a_prev.sqrt(), (1.0 - a_prev - sigma ** 2).sqrt(), sigma * temperature),
-                               noise, cfg_fp16=False)
+            logged = index % log_every_t == 0 or index == total - 1
+            img, pred_x0 = _step_kernel_ex(img, e_c, e_u, 1.0 if unguided else g, img.shape[1], 1,
+                                           (s1m, a_t.sqrt(), a_prev.sqrt(), (1.0 - a_prev - sigma ** 2).sqrt(), sigma * temperature),
+                                           noise, cfg_fp16=False, cfg_variant=variant, want_x0=logged or img_callback is not None)
             if mask is not None:
                 q_sample_blend(x0.float(), torch.randn_like(x0).float(), coef[0][i], coef[1][i], mask=mask, img=img, out=img)
             if callback:
                 callback(i)
-            if index % log_every_t == 0 or index == total - 1:
+            if img_callback:
+                img_callback(pred_x0, i)
+            if logged:
                 intermediates['x_inter'].append(img)
+                intermediates['pred_x0'].append(pred_x0)
+            if state.skipped:
+                break
         return img, intermediates
 
 
@@ -502,6 +532,11 @@ def process_videocrafter(args_dict, model=None):
     the data-URL are webui plumbing outside the path: pass `model` (a `LatentDiffusion`) or install one in `model_cache`;
     `prompt_embeds` / `n_prompt_embeds` keys may carry pre-encoded conditioning.
 
+    webui state (process_videocrafter.py:59-69): `state.job_count`, and per batch `state.job_no` / `state.job`; a Skip
+    (`state.skipped`) ends the running batch's sampling early and is cleared before the next batch, an Interrupt
+    (`state.interrupted`) raises InterruptedException inside sampling and stops the loop before the next batch, which returns
+    the clips finished so far.
+
     LoRA (sample_text2video.py:42-46, :202-206, :231-233): `inject_lora`, `lora_path` (a path or a loaded dict), `lora_scale`
     and `lora_trigger_word`, which is appended to a string prompt.  The model keeps the LoRA merged between calls; a call with
     another LoRA or scale, or without inject_lora, switches with change_lora_v2 (exact restore, then the new merge)."""
@@ -522,7 +557,15 @@ def process_videocrafter(args_dict, model=None):
     n_prompt = a.n_prompt if n_prompt is None else n_prompt
     outputs = []
     bs = int(getattr(a, 'batch_size', 1))          # clips per sample_text2video call, sampled as one batch
+    state = _samplers.state
+    state.job_count = a.batch_count
     for batch in range(a.batch_count):
+        state.job_no = batch + 1
+        if state.skipped:                          # Skip ended the last batch's sampling early; this batch runs in full
+            state.skipped = False
+        if state.interrupted:
+            break
+        state.job = f"Batch {batch + 1} out of {a.batch_count}"
         sampler.noise_gen.manual_seed(a.seed + batch if a.seed != -1 else -1)
         samples = sample_text2video(model, prompt, n_prompt, bs, bs, sample_type='ddim', sampler=sampler, ddim_steps=a.steps,
                                     eta=a.eta, cfg_scale=a.cfg_scale, decode_frame_bs=1, ddp=False,
