@@ -229,6 +229,17 @@ int t2v_vae_set_memory_budget(t2v_vae* v, size_t bytes);
 size_t t2v_vae_get_memory_budget(t2v_vae* v);
 int t2v_vae_last_chunking(t2v_vae* v, int direction, int* chunk_frames, int* n_chunks);
 int t2v_vae_cached_plans(t2v_vae* v, int direction, size_t* slab_bytes);
+/* Block outputs for parity tests.  enable_taps drops both directions' cached plans; plans built while taps are on keep the
+ * output of every block under the reference module's name and never reuse its bytes (a larger arena; plan_bytes counts
+ * it).  Decoder: "decoder.conv_in", "decoder.mid.block_1", "decoder.mid.attn_1", "decoder.mid.block_2", "decoder.up.<lvl>"
+ * (after the level's upsample conv, if any), "decoder.norm_out" (GroupNorm + swish).  Encoder: "encoder.conv_in",
+ * "encoder.down.<lvl>" (after the level's downsample conv, if any), "encoder.mid.block_1", "encoder.mid.attn_1",
+ * "encoder.mid.block_2", "encoder.norm_out".  tap_info / read_tap read the most
+ * recent plan of the tap's direction (a chunked call keeps none): rows x C tokens of frames of h x w, read as fp16
+ * [rows / (h w), C, h, w].  read_tap returns the element count, or < 0 with the error set.                          */
+int t2v_vae_enable_taps(t2v_vae* v, int on, void* stream);
+int t2v_vae_tap_info(t2v_vae* v, const char* name, long long* rows, int* C, int* h, int* w);
+long long t2v_vae_read_tap(t2v_vae* v, const char* name, void* dst, long long cap_elems, void* stream);
 /* VideoCrafter LoRA on the decoder's and the encoder's weights (see "VideoCrafter LoRA" above) */
 int t2v_vae_lora_apply(t2v_vae* v, const char* weight_name, const void* up, const void* down, int dtype, int rank, float alpha,
                        void* stream);

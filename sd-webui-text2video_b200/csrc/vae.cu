@@ -7,9 +7,11 @@
 #include "../../include/t2v_b200.h"
 #include "runtime.cuh"
 
+#include <algorithm>
 #include <cstdio>
 #include <cstring>
 #include <memory>
+#include <vector>
 
 namespace t2v {
 namespace {
@@ -40,6 +42,7 @@ struct t2v_vae {
     GnWorkspace gn_ws;          // shared by the decoder's and the encoder's plans
     size_t budget = 0;          // plan bytes (arena + GroupNorm workspace) one direction may hold; 0: automatic
     int last_chunk[2] = {0, 0}, last_n_chunks[2] = {0, 0};      // how the last decode [0] / encode [1] was split
+    bool taps_enabled = false;  // plans built meanwhile keep every block's output (t2v_vae_enable_taps)
 };
 
 namespace t2v {
@@ -53,6 +56,24 @@ bool ensure_gn_ws(t2v_vae* v, size_t need, cudaStream_t stream) {
     }
     return v->gn_ws.ptr != nullptr;
 }
+
+// Block outputs a plan keeps for the parity tests (t2v_vae_read_tap).  With taps on, a tapped activation is recorded under
+// the reference module's name and never freed, so the arena cannot reuse its bytes; the dry pass makes the same choices,
+// so plan_bytes and the chunking policy see the larger plan.  With taps off, keep() records nothing and release() frees.
+struct Taps {
+    Plan* plan;
+    Builder* b;
+    bool on;
+    std::vector<const __half*> kept;
+    void keep(const std::string& name, const Tok& t, int h, int w) {
+        if (!on) return;
+        kept.push_back(t.p);
+        if (!b->dry()) plan->taps[name] = {t, {h, w}};
+    }
+    void release(const Tok& t) {
+        if (std::find(kept.begin(), kept.end(), t.p) == kept.end()) b->free(t);
+    }
+};
 
 void expect_params(t2v_vae* v) {
     ParamStore& P = v->params;
@@ -203,6 +224,7 @@ Tok attn_block(NetCtx& c, const Tok& x, const std::string& p, int frames, int hc
 int build(t2v_vae* v, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, int frames, int h, int w, VIO* io) {
     Builder bld(plan, arena, dry, num_sms());
     NetCtx c{&v->params, &bld, stream, v->gn_ws.ptr};
+    Taps taps{plan, &bld, v->taps_enabled};
     const t2v_vae_config& cfg = v->cfg;
     const long long R0 = static_cast<long long>(frames) * h * w;
     const int zpad = round_up(cfg.z_channels, 8);
@@ -220,20 +242,24 @@ int build(t2v_vae* v, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, i
     int block_in = cfg.ch * cfg.ch_mult[cfg.n_mult - 1];
     Tok x = conv3x3(c, zq, "decoder.conv_in.weight", prm(c, "decoder.conv_in.bias"), 0, 0, block_in, hc, wc, nullptr);
     bld.free(zq);
+    taps.keep("decoder.conv_in", x, hc, wc);
     Tok y = resnet(c, x, "decoder.mid.block_1", block_in, hc, wc);
-    bld.free(x);
+    taps.release(x);
     x = y;
+    taps.keep("decoder.mid.block_1", x, hc, wc);
     y = attn_block(c, x, "decoder.mid.attn_1", frames, hc, wc);
-    bld.free(x);
+    taps.release(x);
     x = y;
+    taps.keep("decoder.mid.attn_1", x, hc, wc);
     y = resnet(c, x, "decoder.mid.block_2", block_in, hc, wc);
-    bld.free(x);
+    taps.release(x);
     x = y;
+    taps.keep("decoder.mid.block_2", x, hc, wc);
     for (int lvl = cfg.n_mult - 1; lvl >= 0; --lvl) {
         const int block_out = cfg.ch * cfg.ch_mult[lvl];
         for (int j = 0; j < cfg.num_res_blocks + 1; ++j) {
             y = resnet(c, x, "decoder.up." + std::to_string(lvl) + ".block." + std::to_string(j), block_out, hc, wc);
-            bld.free(x);
+            taps.release(x);
             x = y;
         }
         if (lvl != 0) {
@@ -250,11 +276,13 @@ int build(t2v_vae* v, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, i
             x = conv3x3(c, u, up + ".weight", prm(c, up + ".bias"), 0, 0, u.C, hc, wc, nullptr);
             bld.free(u);
         }
+        taps.keep("decoder.up." + std::to_string(lvl), x, hc, wc);
     }
     Tok g = group_norm(c, x, "decoder.norm_out", static_cast<long long>(hc) * wc, 1e-6f, true);
-    bld.free(x);
+    taps.release(x);
+    taps.keep("decoder.norm_out", g, hc, wc);
     Tok o = conv3x3(c, g, "decoder.conv_out.weight", prm(c, "decoder.conv_out.bias"), 0, 0, cfg.out_ch, hc, wc, nullptr, 16);
-    bld.free(g);
+    taps.release(g);
     io->out_tok = o.p;
     io->out_ld = static_cast<int>(o.ld);
     return bld.error;
@@ -287,17 +315,19 @@ PlanCache<VIO>::Entry* get_plan(t2v_vae* v, int frames, int h, int w, cudaStream
 int build_enc(t2v_vae* v, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, int frames, int H, int W, EncIO* io) {
     Builder bld(plan, arena, dry, num_sms());
     NetCtx c{&v->enc_params, &bld, stream, v->gn_ws.ptr};
+    Taps taps{plan, &bld, v->taps_enabled};
     const t2v_vae_config& cfg = v->cfg;
     int hc = H, wc = W;
     Tok x0 = bld.alloc(static_cast<long long>(frames) * H * W, 8);          // RGB zero-padded to 8 channels
     io->x_tok = x0.p;
     Tok x = conv3x3(c, x0, "encoder.conv_in.weight", prm(c, "encoder.conv_in.bias"), 0, 0, cfg.ch, hc, wc, nullptr);
+    taps.keep("encoder.conv_in", x, hc, wc);
     int block_in = cfg.ch;
     for (int lvl = 0; lvl < cfg.n_mult; ++lvl) {
         const int block_out = cfg.ch * cfg.ch_mult[lvl];
         for (int j = 0; j < cfg.num_res_blocks; ++j) {
             Tok y = resnet(c, x, "encoder.down." + std::to_string(lvl) + ".block." + std::to_string(j), block_out, hc, wc);
-            bld.free(x);
+            taps.release(x);
             x = y;
             block_in = block_out;
         }
@@ -313,26 +343,31 @@ int build_enc(t2v_vae* v, Plan* plan, Arena* arena, bool dry, cudaStream_t strea
             const __half* w = w_conv_kmajor(c, dn + ".weight");
             Tok y = linear(c, col, w, block_in, prm(c, dn + ".bias"), nullptr);
             bld.free(col);
-            bld.free(x);
+            taps.release(x);
             x = y;
             hc = ho;
             wc = wo;
         }
+        taps.keep("encoder.down." + std::to_string(lvl), x, hc, wc);
     }
     Tok y = resnet(c, x, "encoder.mid.block_1", block_in, hc, wc);
-    bld.free(x);
+    taps.release(x);
     x = y;
+    taps.keep("encoder.mid.block_1", x, hc, wc);
     y = attn_block(c, x, "encoder.mid.attn_1", frames, hc, wc);
-    bld.free(x);
+    taps.release(x);
     x = y;
+    taps.keep("encoder.mid.attn_1", x, hc, wc);
     y = resnet(c, x, "encoder.mid.block_2", block_in, hc, wc);
-    bld.free(x);
+    taps.release(x);
     x = y;
+    taps.keep("encoder.mid.block_2", x, hc, wc);
     Tok g = group_norm(c, x, "encoder.norm_out", static_cast<long long>(hc) * wc, 1e-6f, true);
-    bld.free(x);
+    taps.release(x);
+    taps.keep("encoder.norm_out", g, hc, wc);
     const int M = 2 * cfg.z_channels;
     Tok h = conv3x3(c, g, "encoder.conv_out.weight", prm(c, "encoder.conv_out.bias"), 0, 0, M, hc, wc, nullptr, 16);
-    bld.free(g);
+    taps.release(g);
     Tok mom = bld.alloc(h.rows, 2 * cfg.embed_dim, round_up(2 * cfg.embed_dim, 8));
     {
         const __half* w = w_conv(c, "quant_conv.weight", 1, 16, static_cast<int>(h.ld));
@@ -468,6 +503,18 @@ int run_in_chunks(t2v_vae* v, int dir, PlanCache<IO>& cache, const ParamStore& P
     }
     if (n_chunks > 1) cache.clear(stream);
     return rc;
+}
+
+// A tap of the most recent decoder plan ("decoder.*") or encoder plan ("encoder.*"); null, with the error set, if none.
+const std::pair<Tok, std::pair<int, int>>* find_tap(t2v_vae* v, const char* name) {
+    auto* plan = strncmp(name, "encoder.", 8) == 0 ? (v->enc_plans.latest() ? v->enc_plans.latest()->plan.get() : nullptr)
+                                                   : (v->plans.latest() ? v->plans.latest()->plan.get() : nullptr);
+    if (plan) {
+        auto it = plan->taps.find(name);
+        if (it != plan->taps.end()) return &it->second;
+    }
+    set_error("VAE tap '%s' not found (enable taps before a whole-clip decode / encode)", name);
+    return nullptr;
 }
 
 }  // namespace
@@ -629,6 +676,40 @@ int t2v_vae_cached_plans(t2v_vae* v, int direction, size_t* slab_bytes) {
     const size_t n = direction == DEC ? v->plans.size() : v->enc_plans.size();
     if (slab_bytes) *slab_bytes = direction == DEC ? v->plans.slab_bytes() : v->enc_plans.slab_bytes();
     return static_cast<int>(n);
+}
+
+int t2v_vae_enable_taps(t2v_vae* v, int on, void* stream) {
+    if (!v) return -1;
+    v->taps_enabled = on != 0;
+    v->plans.clear(reinterpret_cast<cudaStream_t>(stream));
+    v->enc_plans.clear(reinterpret_cast<cudaStream_t>(stream));
+    return 0;
+}
+
+int t2v_vae_tap_info(t2v_vae* v, const char* name, long long* rows, int* C, int* h, int* w) {
+    const auto* tap = find_tap(v, name);
+    if (!tap) return -1;
+    if (rows) *rows = tap->first.rows;
+    if (C) *C = tap->first.C;
+    if (h) *h = tap->second.first;
+    if (w) *w = tap->second.second;
+    return 0;
+}
+
+long long t2v_vae_read_tap(t2v_vae* v, const char* name, void* dst, long long cap_elems, void* stream_) {
+    const auto* tap = find_tap(v, name);
+    if (!tap) return -1;
+    const Tok& t = tap->first;
+    const int h = tap->second.first, w = tap->second.second;
+    const long long n = t.rows * t.C;
+    if (n > cap_elems) {
+        set_error("VAE tap '%s' needs %lld elements", name, n);
+        return -2;
+    }
+    // [frames, h, w, C] tokens -> fp16 [frames, C, h, w]
+    const int frames = static_cast<int>(t.rows / (static_cast<long long>(h) * w));
+    if (egress_latent(t.p, t.ld, dst, 0, frames, t.C, 1, h, w, reinterpret_cast<cudaStream_t>(stream_)) != 0) return -3;
+    return n;
 }
 
 }  // extern "C"

@@ -72,6 +72,9 @@ SIGNATURES = {
     't2v_vae_get_memory_budget': (C.c_size_t, [P]),
     't2v_vae_last_chunking': (c_int, [P, c_int, C.POINTER(c_int), C.POINTER(c_int)]),
     't2v_vae_cached_plans': (c_int, [P, c_int, C.POINTER(C.c_size_t)]),
+    't2v_vae_enable_taps': (c_int, [P, c_int, P]),
+    't2v_vae_tap_info': (c_int, [P, c_char_p, C.POINTER(c_ll), C.POINTER(c_int), C.POINTER(c_int), C.POINTER(c_int)]),
+    't2v_vae_read_tap': (c_ll, [P, c_char_p, P, c_ll, P]),
     't2v_clip_create': (c_int, [P, C.POINTER(P)]),
     't2v_clip_destroy': (None, [P]),
     't2v_clip_set_param': (c_int, [P, c_char_p, P, c_int, c_int, C.POINTER(C.c_int64), P]),

@@ -658,3 +658,19 @@ class AutoencoderKL(_NativeModule):
         nbytes = C.c_size_t(0)
         n = _lib.load_library().t2v_vae_cached_plans(self._handle, int(encode), C.byref(nbytes))
         return n, nbytes.value
+
+    def enable_taps(self, on=True):
+        """Keep every block's output in the plans built from now on (drops the cached plans; include/t2v_b200.h)."""
+        _lib.check(_lib.lib().t2v_vae_enable_taps(self._handle, int(on), _lib.stream_ptr()), 'vae_enable_taps')
+
+    def read_tap(self, name):
+        """The output of block `name` (e.g. 'decoder.mid.attn_1') of the last whole-clip decode / encode as fp16
+        [frames, C, h, w]."""
+        rows, c, h, w = C.c_longlong(0), C.c_int(0), C.c_int(0), C.c_int(0)
+        _lib.check(_lib.lib().t2v_vae_tap_info(self._handle, name.encode(), C.byref(rows), C.byref(c), C.byref(h), C.byref(w)),
+                   'vae_tap_info')
+        out = torch.empty((rows.value // (h.value * w.value), c.value, h.value, w.value), device='cuda', dtype=torch.float16)
+        n = _lib.lib().t2v_vae_read_tap(self._handle, name.encode(), _lib.ptr(out), out.numel(), _lib.stream_ptr())
+        if n != out.numel():
+            raise RuntimeError(f'read_tap({name}): {n} vs {out.numel()}: {_lib.load_library().t2v_last_error().decode()}')
+        return out
