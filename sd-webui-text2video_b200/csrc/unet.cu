@@ -869,6 +869,16 @@ int build(t2v_unet* u, Plan* plan, Arena* arena, bool dry, cudaStream_t stream, 
         to_layout(false);                // skip connections (and the next block's ResBlock) are frame-sharded
         if (feats_B > 0 && feature_block(static_cast<int>(id))) {       // h = h + features_adapter[i], before the push
             const Tok xx = x;
+            if (u->taps_enabled) {       // the add is in place: the block's tap keeps a copy of its output from before it
+                const Tok snap = bld.alloc(xx.rows, xx.C);
+                bld.step([=](cudaStream_t s) {
+                    if (cudaMemcpy2DAsync(snap.p, snap.ld * sizeof(__half), xx.p, xx.ld * sizeof(__half), xx.C * sizeof(__half),
+                                          xx.rows, cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+                        return launch_status("feature tap copy");
+                    return 0;
+                });
+                tap(c, u->ins[id].back().prefix, snap, hc, wc);
+            }
             const __half* f = io->feat[feat_i++];
             const long long per_sample = static_cast<long long>(F) * hc * wc;
             const int fb = feats_B;

@@ -83,27 +83,27 @@ def to_video_features(feats, b, t):
     return [f.reshape(b, t, *f.shape[1:]).permute(0, 2, 1, 3, 4) for f in feats]
 
 
-def vc_unet_forward(W, cfg: VC.VCConfig, x, t, ctx, features_adapter=None):
-    """UNetModel.forward with features_adapter (openaimodel3d.py:632-670)."""
+def vc_unet_forward(W, cfg: VC.VCConfig, x, t, ctx, features_adapter=None, taps=None):
+    """UNetModel.forward with features_adapter (openaimodel3d.py:632-670).  `taps` as in vc_oracle's forward."""
     L = VC.vc_enumerate(cfg)
     emb = VC.vc_timestep_embedding(t, cfg.model_channels)
-    emb = F.linear(emb, W['time_embed.0.weight'], W['time_embed.0.bias'])
+    emb = F.linear(emb.to(W['time_embed.0.weight'].dtype), W['time_embed.0.weight'], W['time_embed.0.bias'])
     emb = F.linear(F.silu(emb), W['time_embed.2.weight'], W['time_embed.2.bias'])
     hs = []
     h = x
     adapter_idx = 0
     for idx, blk in enumerate(L.input_blocks):
-        h = VC._run(W, blk, h, emb, ctx, cfg)
+        h = VC._run(W, blk, h, emb, ctx, cfg, taps)
         if (idx + 1) % 3 == 0 and features_adapter is not None:
             h = h + features_adapter[adapter_idx]
             adapter_idx += 1
         hs.append(h)
     if features_adapter is not None:
         assert len(features_adapter) == adapter_idx, 'Mismatch features adapter'
-    h = VC._run(W, L.middle, h, emb, ctx, cfg)
+    h = VC._run(W, L.middle, h, emb, ctx, cfg, taps)
     for blk in L.output_blocks:
         h = torch.cat([h, hs.pop()], dim=1)
-        h = VC._run(W, blk, h, emb, ctx, cfg)
+        h = VC._run(W, blk, h, emb, ctx, cfg, taps)
     h = F.silu(VC._gn(W, 'out.0', h, 1e-5))
     return F.conv3d(h, W['out.2.weight'], W['out.2.bias'], padding=(0, 1, 1))
 
