@@ -435,6 +435,17 @@ int t2v_op_pack_conv_weight(const void* src, int src_is_f32, void* dst, int Cout
                             int k_alloc, void* stream);
 int t2v_op_pack_geglu_weight(const void* w, const void* b, int src_is_f32, void* wdst, void* bdst, int H, int K, int bn,
                              void* stream);
+/* The LoRA merge kernels of t2v_unet_lora_merge and t2v_*_lora_apply on a plain fp16 buffer w [out, cols] (the first
+ * out * cols elements are written, nothing past them):
+ *   t2v_op_lora_merge  w = fp16(w + fp16(fp16(B @ A) * alpha)), B [out, rank], A [rank, cols] fp16 (A [rank, 3 * cols] with
+ *                      temporal_mean: the product viewed [out, cols / 3, 3, 3] and averaged over its last axis);
+ *   t2v_op_lora_apply  w = fp16(w + alpha * up @ down) in fp32, up [out, rank], down [rank, cols], fp16 (dtype 0) or fp32
+ *                      (dtype 1).
+ * All pointers are device pointers.  Errors (-1, before any launch): rank, out or cols < 1, dtype other than 0 or 1. */
+int t2v_op_lora_merge(void* w, const void* A, const void* B, int out, int cols, int rank, float alpha, int temporal_mean,
+                      void* stream);
+int t2v_op_lora_apply(void* w, const void* up, const void* down, int dtype, int out, int cols, int rank, float alpha,
+                      void* stream);
 /* GroupNorm (32 groups, + SiLU when silu) of instances of rows_per_inst consecutive rows of x [rows, C] -> y.
  * phase 0: what the model runs on one GPU (one fused launch where the grid can be co-resident, else statistics + apply).
  * phase 1: statistics only, with the chunking of the frame-sharded plans; (mean, rstd) per (instance, group) go to

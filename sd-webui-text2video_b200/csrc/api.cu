@@ -315,6 +315,27 @@ int t2v_op_pack_conv_weight(const void* src, int src_is_f32, void* dst, int Cout
     return pack_conv_weight(src, src_is_f32, reinterpret_cast<__half*>(dst), Cout, Cin, taps, n_alloc, k_alloc,
                             reinterpret_cast<cudaStream_t>(stream));
 }
+int t2v_op_lora_merge(void* w, const void* A, const void* B, int out, int cols, int rank, float alpha, int temporal_mean,
+                      void* stream) {
+    if (rank < 1 || out < 1 || cols < 1) {
+        set_error("op_lora_merge: rank, out and cols must be >= 1 (rank %d, out %d, cols %d)", rank, out, cols);
+        return -1;
+    }
+    clear_pending_error("op_lora_merge");
+    return lora_merge_weight(reinterpret_cast<__half*>(w), reinterpret_cast<const __half*>(A), reinterpret_cast<const __half*>(B),
+                             out, cols, rank, alpha, temporal_mean, reinterpret_cast<cudaStream_t>(stream));
+}
+int t2v_op_lora_apply(void* w, const void* up, const void* down, int dtype, int out, int cols, int rank, float alpha,
+                      void* stream) {
+    if (rank < 1 || out < 1 || cols < 1 || (dtype != 0 && dtype != 1)) {
+        set_error("op_lora_apply: rank, out and cols must be >= 1 and dtype 0 (fp16) or 1 (fp32) (rank %d, out %d, cols %d, "
+                  "dtype %d)", rank, out, cols, dtype);
+        return -1;
+    }
+    clear_pending_error("op_lora_apply");
+    return lora_apply_weight(reinterpret_cast<__half*>(w), up, down, dtype, out, cols, rank, alpha,
+                             reinterpret_cast<cudaStream_t>(stream));
+}
 int t2v_op_pack_geglu_weight(const void* w, const void* b, int src_is_f32, void* wdst, void* bdst, int H, int K, int bn,
                              void* stream) {
     return pack_geglu_weight(w, b, src_is_f32, reinterpret_cast<__half*>(wdst), reinterpret_cast<__half*>(bdst), H, K, bn,

@@ -108,6 +108,8 @@ SIGNATURES = {
     't2v_op_ln_linear': (c_int, [P, c_ll, c_ll, c_int, P, P, P, P, c_int, c_int, P, P, P, P, P, c_ll, P, c_ll, c_int, c_int, P]),
     't2v_op_pack_conv_weight': (c_int, [P, c_int, P, c_int, c_int, c_int, c_int, c_int, P]),
     't2v_op_pack_geglu_weight': (c_int, [P, P, c_int, P, P, c_int, c_int, c_int, P]),
+    't2v_op_lora_merge': (c_int, [P, P, P, c_int, c_int, c_int, c_float, c_int, P]),
+    't2v_op_lora_apply': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_float, P]),
     't2v_op_groupnorm': (c_int, [P, c_ll, P, c_ll, c_ll, c_int, c_int, P, P, c_float, c_int, c_int, P, P]),
     't2v_op_layernorm': (c_int, [P, c_ll, P, c_ll, c_ll, c_int, P, P, c_float, P]),
     't2v_op_attention': (c_int, [P, P, P, P, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_int,

@@ -277,6 +277,37 @@ def pack_geglu_weight(w, b, bn):
     return wd, bd
 
 
+def _lora_target(w, out, cols):
+    if w.dtype != torch.float16 or not w.is_contiguous():
+        raise ValueError('the LoRA target must be a contiguous fp16 tensor (it is updated in place)')
+    out = w.shape[0] if out is None else out
+    return out, (w.numel() // max(out, 1) if cols is None else cols)
+
+
+def lora_merge_(w, A, B, alpha, temporal_mean=False, out=None, cols=None):
+    """In place: w [out, cols] = fp16(w + fp16(fp16(B @ A) * alpha)), the Stable-LoRA merge of t2v_unet_lora_merge.
+    A [rank, cols] (x3 columns with temporal_mean), B [out, rank] fp16.  out / cols default to w's first dimension and
+    the rest; given, only the first out * cols elements of w are written."""
+    out, cols = _lora_target(w, out, cols)
+    A, B = A.to(torch.float16).contiguous(), B.to(torch.float16).contiguous()
+    rc = _lib.lib().t2v_op_lora_merge(_lib.ptr(w), _lib.ptr(A), _lib.ptr(B), out, cols, A.shape[0], float(alpha),
+                                      int(temporal_mean), _lib.stream_ptr())
+    _lib.check(rc, 'op_lora_merge')
+    return w
+
+
+def lora_apply_(w, up, down, alpha, out=None, cols=None):
+    """In place: w [out, cols] = fp16(w + alpha * up @ down) in fp32, the VideoCrafter merge of t2v_*_lora_apply.
+    up [out, rank], down [rank, cols]: fp32 when either is, else fp16."""
+    out, cols = _lora_target(w, out, cols)
+    dt = torch.float16 if up.dtype == down.dtype == torch.float16 else torch.float32
+    up, down = up.to(dt).contiguous(), down.to(dt).contiguous()
+    rc = _lib.lib().t2v_op_lora_apply(_lib.ptr(w), _lib.ptr(up), _lib.ptr(down), int(dt == torch.float32), out, cols,
+                                      up.shape[1], float(alpha), _lib.stream_ptr())
+    _lib.check(rc, 'op_lora_apply')
+    return w
+
+
 def conv_taps_2d():
     """tap = ky*3+kx over row dims (w, h, frames)."""
     return [[kx - 1, ky - 1, 0] for ky in range(3) for kx in range(3)]
